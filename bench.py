@@ -1,8 +1,13 @@
 #!/usr/bin/env python
-"""bench.py -- mocap frames solved/sec (MoSh++ Stage II) on N B200s.
+"""bench.py -- mocap frames solved/sec (MoSh++ Stage II) on N H100s.
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU algorithm (oracle port)
+    python bench.py --gpus 1 --steps K --warmup W --dump-outputs DIR
+
+--dump-outputs DIR (N = 1): after the timed steps, the result arrays of the last timed step of the headline workload
+(what ``chmosh.solve_verified`` hands its caller) go to DIR/<name>.npy as float64; the inputs are seeded, so two
+builds can be compared output for output.
 
 N = 1   workload = the configuration BASELINE.json's north star quotes its target on: ONE 4000-frame SMPL-H sequence
         (V = 6890, 52 joints, 53 markers, fingers on: 111 free variables in Step 2).  A step = one pass of the hot path
@@ -23,6 +28,7 @@ JSON keys follow the driver contract; DESIGN.md section 7 says how each number i
 from __future__ import annotations
 
 import argparse
+import atexit
 import json
 import os
 import subprocess
@@ -54,8 +60,8 @@ def algorithmic_bytes(pk, has_velo=True, fingers=True):
 
 
 class ClockSampler:
-    """Samples nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md): one
-    `nvidia-smi -lms 100` child process from the warm-up to the end of the end-to-end leg."""
+    """Samples nvidia-smi clocks / throttle reasons during the timed region: one `nvidia-smi -lms 100` child process
+    from the warm-up to the end of the end-to-end leg."""
 
     Q = ('clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,'
@@ -68,21 +74,24 @@ class ClockSampler:
         try:
             self.proc = subprocess.Popen(['nvidia-smi', f'--query-gpu={self.Q}', '--format=csv,noheader,nounits',
                                           '-i', str(self.index), '-lms', '100'], stdout=subprocess.PIPE, text=True)
+            atexit.register(self.stop)          # the sampler never outlives the benchmark, also when it fails
         except Exception:
             self.proc = None
 
     def stop(self):
         if self.proc is None:
             return
+        proc, self.proc = self.proc, None
         try:
-            self.proc.terminate()
-            out, _ = self.proc.communicate(timeout=5)
+            proc.terminate()
+            out, _ = proc.communicate(timeout=5)
             for line in out.strip().splitlines():
                 r = [x.strip() for x in line.split(',')]
                 if len(r) >= 7:
                     self.rows.append(r)
         except Exception:
-            pass
+            proc.kill()
+            proc.wait()
 
     def summary(self):
         if not self.rows:
@@ -175,41 +184,25 @@ def run_reference(args, rank):
     print(json.dumps(line), flush=True)
 
 
-def load_traffic(key):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the Stage-II kernel from this round's
-    `ncu --set full` capture of the same workload (profiles/traffic.json), or None."""
-    tfile = os.path.join(ROOT, 'profiles', 'traffic.json')
-    try:
-        t = json.load(open(tfile))
-        e = t.get(key)
-        if isinstance(e, dict):
-            return e.get('dram_bytes_per_launch'), e.get('source')
-    except Exception:
-        pass
-    return None, None
-
-
-def roofline(ab, builds, useful_builds, ms, traffic_key):
+def roofline(ab, builds, useful_builds, ms):
     peaks = {}
     try:
         peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
     except Exception:
         pass
-    peak = float(peaks.get('hbm_gbs', 6650.0))
+    peak = float(peaks.get('hbm_gbs', 3350.0))
     per_unit = ab['B_K1'] + ab['B_K2']
     achieved = per_unit * builds / (ms * 1e-3) / 1e9
     useful = per_unit * useful_builds / (ms * 1e-3) / 1e9
-    traffic, src = load_traffic(traffic_key)
     return {'bound': 'hbm', 'achieved': achieved, 'peak': peak, 'unit': 'GB/s', 'frac': achieved / peak,
-            'traffic': traffic, 'traffic_source': src,
             'achieved_useful': useful, 'frac_useful': useful / peak,
             'bytes_per_frame_iteration': per_unit, 'frame_iterations_per_launch': builds,
             'useful_frame_iterations_per_launch': useful_builds,
             'note': 'achieved = (B_K1+B_K2) x frame-iterations executed / kernel time (SURVEY 8(d) effective-bandwidth '
                     'definition of the J-materialising formulation); *_useful counts only the iterations of the emitted '
                     'frames (what the sequential solve needs), i.e. without the warm-up of the time-parallel chunks. The '
-                    'fused kernel keeps J on chip: its DRAM traffic is `traffic`. peak: '
-                    + ('measured copy bandwidth (MEASURED_PEAKS.json)' if peaks else 'fallback 6650 GB/s')}
+                    'fused kernel keeps J on chip. peak: '
+                    + ('measured copy bandwidth (MEASURED_PEAKS.json)' if peaks else 'H100 SXM data sheet, 3350 GB/s')}
 
 
 def main():
@@ -227,6 +220,8 @@ def main():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-secondary', action='store_true', help='N=1: skip the C2 and C5-on-one-GPU legs')
     ap.add_argument('--sequences', type=int, default=C5_SEQUENCES, help='N>1: number of 4000-frame sequences')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='N=1: write the result arrays of the last timed step to DIR/<name>.npy (float64)')
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == 'ours' else args.warmup
 
@@ -242,7 +237,7 @@ def main():
     from moshpp_b200 import chmosh
 
     if not torch.cuda.is_available():
-        raise SystemExit('bench.py needs a B200: the Stage-II path has no CPU fallback')
+        raise SystemExit('bench.py needs an H100: the Stage-II path has no CPU fallback')
     torch.cuda.set_device(local_rank)
     if args.chunk_warmup is None:
         args.chunk_warmup = chmosh.DEFAULT_WARMUP
@@ -257,16 +252,17 @@ def main():
 # ------------------------------------------------------------------------------------------------------------------
 # N = 1
 # ------------------------------------------------------------------------------------------------------------------
-def time_job(model, pk, opts, obs, vis, args, chunk_len, flush, steps, warmup):
+def time_job(model, pk, opts, obs, vis, args, chunk_len, flush, steps, warmup, dump_dir=None):
     """Device time of `steps` passes of the product's solve on one resident job: the launch over all chunks, the boundary
-    check and the repair launches (chmosh.launch_verified), each launch bracketed by CUDA events on the job's stream."""
+    check and the repair launches (chmosh.launch_verified), each launch bracketed by CUDA events on the job's stream.
+    ``dump_dir``: the result arrays of the last timed pass go there (see --dump-outputs)."""
     from moshpp_b200 import chmosh, lib
     prec = {'f32': lib.MOSH2_F32, 'f64': lib.MOSH2_F64}[args.precision]
     tol = chmosh.BOUNDARY_TOL['fast']
     F = obs.shape[0]
     extra = chmosh.first_chunk_extra(args.chunk_warmup, args.warmup_full)
     if chunk_len is None:            # the product's own plan (chmosh.mosh_stageii)
-        chunk_len = chmosh.plan_chunk_len([F], chmosh.NUM_SMS_B200, args.chunk_warmup, args.warmup_full, first_extra=extra)
+        chunk_len = chmosh.plan_chunk_len([F], chmosh.NUM_SMS, args.chunk_warmup, args.warmup_full, first_extra=extra)
     job = model.job(F, opts, chunk_len=chunk_len, chunk_warmup=args.chunk_warmup, warmup_full=args.warmup_full, precision=prec,
                     first_extra=extra)
     job.upload(obs, vis)
@@ -284,6 +280,8 @@ def time_job(model, pk, opts, obs, vis, args, chunk_len, flush, steps, warmup):
         launches += len(rep['kernel_ms'])
     wall = time.perf_counter() - t0
     totals = job.totals()
+    if dump_dir is not None:
+        dump_outputs(dump_dir, chmosh.download_verified(job, bad, dict(rep)))
     # C-ABI job-level end to end: pinned H2D + launches + D2H of all result arrays
     e2e = []
     for i in range(2 + steps):
@@ -297,6 +295,13 @@ def time_job(model, pk, opts, obs, vis, args, chunk_len, flush, steps, warmup):
                boundary=rep)
     job.close()
     return out
+
+
+def dump_outputs(out_dir, res):
+    """The arrays a caller of the solve receives, one float64 .npy each (about 13 MB for the 4000-frame workload)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name in ('fullpose', 'pose', 'trans', 'dmpls', 'markers_sim', 'errs', 'status', 'counters'):
+        np.save(os.path.join(out_dir, f'{name}.npy'), np.asarray(getattr(res, name), dtype=np.float64))
 
 
 def time_plugin(case, args, steps, warmup, chunk_len=None):
@@ -327,7 +332,7 @@ def run_single(args):
     from moshpp_b200 import chmosh, lib, shard
 
     dev = 0
-    flush_buf = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=f'cuda:{dev}')   # > 126 MB L2
+    flush_buf = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=f'cuda:{dev}')   # > 50 MB L2
 
     def flush():
         flush_buf.add_(1)
@@ -343,7 +348,7 @@ def run_single(args):
     obs, vis = dense(case)
     F = obs.shape[0]
     model = lib.Model(pk, device=dev)
-    ns = time_job(model, pk, opts, obs, vis, args, args.chunk_len, flush, args.steps, args.warmup)
+    ns = time_job(model, pk, opts, obs, vis, args, args.chunk_len, flush, args.steps, args.warmup, dump_dir=args.dump_outputs)
     chunk_len = ns['chunk_len']
     e2e_ms, out, e2e_each, e2e_cold = time_plugin(case, args, args.steps, 2, chunk_len=args.chunk_len)
     b = out['stageii_debug_details']['b200']
@@ -366,7 +371,7 @@ def run_single(args):
                                                                      'boundary_delta_first', 'boundary_delta_max', 'unverified_chunks')},
                    'schedule': 'time-parallel chunks, verified: launch over all chunks + boundary check + resume-mode repair '
                                'launches of the chunks whose warm-up left more than the tolerance (all inside ms_per_step)'},
-        'roofline': roofline(ab, ns['totals']['builds'], ns['totals']['emitted_builds'], ns['ms'], 'NS'),
+        'roofline': roofline(ab, ns['totals']['builds'], ns['totals']['emitted_builds'], ns['ms']),
         'e2e': {'value': F / (e2e_ms * 1e-3), 'unit': UNIT, 'h2d_bytes_per_step': int(h2d), 'd2h_bytes_per_step': int(d2h),
                 'ms_per_step': e2e_ms,
                 'what': 'wall clock of chmosh.mosh_stageii(mocap_fname, cfg, ...) per call: mocap file read, label plan, job '
@@ -587,7 +592,7 @@ def run_sharded(args, rank, local_rank, world):
                        'collectives': 'grouped NCCL send/recv: scatter of observations from rank 0, gather of result rows to rank 0 '
                                       '(inside e2e; the device-timed value has the observations resident)',
                        'single_gpu_base': 'bench.py --gpus 1 reports the same 32-sequence workload on one GPU under c5_one_gpu'},
-            'roofline': roofline(ab, builds / world, useful / world, ms_step, 'C5'),
+            'roofline': roofline(ab, builds / world, useful / world, ms_step),
             'e2e': {'value': total_frames / (e2e_ms * 1e-3), 'unit': UNIT, 'h2d_bytes_per_step': int(h2d), 'd2h_bytes_per_step': int(d2h),
                     'ms_per_step': e2e_ms,
                     'what': 'shard.solve_sharded: pinned host observations on rank 0 -> H2D -> NCCL scatter -> per-rank solves '

@@ -1,5 +1,5 @@
 /*
- * mosh2.h -- C-ABI of libmosh2.so, the B200 (sm_100a) MoSh++ Stage-II pose solver.
+ * mosh2.h -- C-ABI of libmosh2.so, the H100 (sm_90a) MoSh++ Stage-II pose solver.
  *
  * The reference has no FFI: its Stage-II plug-in point is a Python callable,
  *     MoSh.mosh_stageii(self, mosh_stageii_func)          src/moshpp/mosh_head.py:268-301
@@ -29,7 +29,7 @@ enum {
     MOSH2_OK = 0,
     MOSH2_E_INVALID = -1,   /* bad argument / inconsistent sizes            */
     MOSH2_E_CUDA = -2,      /* CUDA runtime error (message in last_error)   */
-    MOSH2_E_NO_DEVICE = -3, /* no usable sm_100 device                      */
+    MOSH2_E_NO_DEVICE = -3, /* no usable sm_90 device                       */
     MOSH2_E_TOO_LARGE = -4  /* model does not fit the kernel (shared memory, tree depth > 16, > 254 joints) */
 };
 

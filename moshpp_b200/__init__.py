@@ -1,4 +1,4 @@
-"""mosh2-b200: a B200-native MoSh++ Stage-II pose solver.
+"""mosh2-b200: an H100-native MoSh++ Stage-II pose solver.
 
 The package holds only what the Stage-II hot path needs (SURVEY.md section 8):
 

@@ -1,4 +1,4 @@
-"""In-tree build of libmosh2.so (nvcc, sm_100a only) and of the oracle-side helper libraries.
+"""In-tree build of libmosh2.so (nvcc, sm_90a only) and of the oracle-side helper libraries.
 
 ``python -m moshpp_b200.build`` or ``__graft_entry__.build()``.  nvcc cross-compiles without a GPU.
 """
@@ -15,10 +15,10 @@ CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libmosh2.so')
 EMU_SRC = os.path.join(ROOT, 'tests', 'emu', 'mosh2_emu.cpp')
 EMU_LIB = os.path.join(ROOT, 'tests', 'emu', '_build', 'libmosh2_emu.so')
-TC_SRC = os.path.join(ROOT, 'tests', 'tc', 'jtj_tcgen05_test.cu')
+TC_SRC = os.path.join(ROOT, 'tests', 'tc', 'jtj_tf32_test.cu')
 TC_BIN = os.path.join(ROOT, 'tests', 'tc', '_build', 'jtj_test')
 
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-shared', '-Xcompiler', '-fPIC']
 
 
@@ -62,10 +62,10 @@ def build_emu(force: bool = False) -> str:
 
 
 def build_tc_test(force: bool = False) -> str:
-    """TEST-ONLY stand-alone check of the tcgen05 J^T J building block (tests/tc/jtj_tcgen05_test.cu)."""
-    if force or _stale(TC_BIN, [TC_SRC]):
+    """TEST-ONLY stand-alone check of the split-TF32 J^T J building block (tests/tc/jtj_tf32_test.cu)."""
+    if force or _stale(TC_BIN, [TC_SRC, os.path.join(CSRC, 'mosh2_device.cuh')]):
         os.makedirs(os.path.dirname(TC_BIN), exist_ok=True)
-        cmd = [_nvcc(), '-gencode', 'arch=compute_100a,code=sm_100a', '-O2', '-o', TC_BIN, TC_SRC]
+        cmd = [_nvcc(), '-gencode', 'arch=compute_90a,code=sm_90a', '-O2', '-std=c++17', '-o', TC_BIN, TC_SRC]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError('nvcc failed:\n' + r.stdout + r.stderr)

@@ -1,4 +1,4 @@
-"""``mosh_stageii`` -- drop-in for the reference's Stage-II callable, running on libmosh2.so (B200).
+"""``mosh_stageii`` -- drop-in for the reference's Stage-II callable, running on libmosh2.so (H100).
 
 Reference: src/moshpp/chmosh.py:458-741.  Same positional signature, same return dictionary
 (chmosh.py:726-741), same frame-skip rule (586-588); it plugs into the reference's own call site
@@ -37,7 +37,7 @@ from .mocap_interface import MocapSession, rotation_xyz as _rotation_xyz
 
 logger = logging.getLogger('moshpp_b200')
 
-NUM_SMS_B200 = 148
+NUM_SMS = 132                # H100 SXM: thread blocks of the Stage-II kernel that run at once (one per SM)
 DEFAULT_WARMUP = 64          # solved frames every chunk is started early (DESIGN.md section 4)
 DEFAULT_WARMUP_FULL = 48     # the last 48 of them with the full per-frame schedule, the first 16 with one Step-2 iteration
 
@@ -96,7 +96,7 @@ def count_chunks(n_frames: int, chunk_len: int, first_extra: int = 0) -> int:
     return -(-n_frames // chunk_len)
 
 
-def plan_chunk_len(frame_counts, sm_budget: int = NUM_SMS_B200, warmup: int = DEFAULT_WARMUP,
+def plan_chunk_len(frame_counts, sm_budget: int = NUM_SMS, warmup: int = DEFAULT_WARMUP,
                    warmup_full: int = DEFAULT_WARMUP_FULL, min_len: int = 4, first_extra: int = 0) -> int:
     """Chunk length for a set of sequences that are solved together on one GPU (one thread block per chunk, one block
     per SM at a time).  The chunks run in waves of ``sm_budget``; a wave lasts as long as its longest chunk, i.e. about
@@ -124,7 +124,7 @@ def plan_chunk_len(frame_counts, sm_budget: int = NUM_SMS_B200, warmup: int = DE
     return best[1]
 
 
-def auto_chunk_len(n_frames: int, sm_budget: int = NUM_SMS_B200) -> int:
+def auto_chunk_len(n_frames: int, sm_budget: int = NUM_SMS) -> int:
     """Shortest chunks that still give about one chunk per available SM (latency = chunk_len + warm-up)."""
     return max(4, int(math.ceil(n_frames / max(1, sm_budget))))
 
@@ -413,6 +413,13 @@ def solve_verified(job, obs, vis, *, tol, max_rounds: int = 12, while_running=No
     if obs is not None:          # (None: the caller has uploaded already, e.g. through Job.upload_markers)
         job.upload(obs, vis)
     bad, report = launch_verified(job, tol, max_rounds, while_running)
+    res = download_verified(job, bad, report)
+    return res, report
+
+
+def download_verified(job, bad, report):
+    """The job's result arrays after ``launch_verified``; the solved frames of the chunks in ``bad`` (still over
+    tolerance) carry MOSH2_ST_SHORT_WARMUP."""
     res = job.download()
     if len(bad):
         report['unverified_chunks'] = int(len(bad))
@@ -422,16 +429,16 @@ def solve_verified(job, obs, vis, *, tol, max_rounds: int = 12, while_running=No
             res.status[sl] |= np.where((res.status[sl] & _lib.ST_SOLVED) != 0, _lib.ST_SHORT_WARMUP, 0).astype(res.status.dtype)
         logger.warning('%d chunks did not pass the boundary check after %d repair rounds (max delta %s); their frames carry '
                        'MOSH2_ST_SHORT_WARMUP', len(bad), report['rounds'], report['boundary_delta_max'])
-    return res, report
+    return res
 
 
 def mosh_stageii(mocap_fname: str, cfg, markers_latent: np.ndarray, latent_labels: list, betas: np.ndarray,
                  marker_meta: dict, v_template_fname=None, *, device: int = 0, mode: str = 'fast',
                  chunk_len: Optional[int] = None, chunk_warmup: Optional[int] = None, warmup_full: Optional[int] = None,
                  first_extra: Optional[int] = None, precision: Optional[str] = None, verify: bool = True, boundary_tol=None,
-                 sm_budget: int = NUM_SMS_B200, labels_map='general', subject_cache: bool = True,
+                 sm_budget: int = NUM_SMS, labels_map='general', subject_cache: bool = True,
                  device_adapter: bool = True) -> dict:
-    """Stage II of MoSh++ on one B200.  Positional arguments as in the reference (chmosh.py:458-459).
+    """Stage II of MoSh++ on one H100.  Positional arguments as in the reference (chmosh.py:458-459).
 
     Keyword-only extras.  ``mode``: 'fast' (default) = float32, chunked in time with a verified warm-up -- within
     BASELINE.md section 4's tolerances of the reference's sequential float64 result except on the few frames where that

@@ -1,7 +1,7 @@
 // mosh2.cu -- libmosh2.so: kernels and the C-ABI declared in include/mosh2.h.
 //
 // One CUDA thread block per chunk of frames runs the whole Stage-II schedule of
-// src/moshpp/chmosh.py:584-724 on device (mosh2_device.cuh).  Built for sm_100a only.
+// src/moshpp/chmosh.py:584-724 on device (mosh2_device.cuh).  Built for sm_90a (H100) only.
 #include "../../include/mosh2.h"
 
 #include <cuda_runtime.h>
@@ -126,23 +126,7 @@ mosh2_stageii_kernel(const __grid_constant__ mosh2::Model<real> m, const __grid_
     }
     mosh2::Cta c{int(threadIdx.x), int(blockDim.x)};
     mosh2::Solver<real, BIG> s(m, job, w, d, c);
-    // f32 with the workspace in shared memory: J^T J accumulates on the tensor cores (tcgen05, accumulator in
-    // tensor memory); warp 0 owns the allocation
-    if (w.tc) {
-        if (threadIdx.x < 32) mosh2::tc::tmem_alloc(mosh2::tc::smem_u32(w.tmem_slot), mosh2::kTcCols);
-        if (threadIdx.x == 32) mosh2::tc::mbar_init(mosh2::tc::smem_u32(w.mbar), 1);
-        mosh2::tc::fence_before();
-        __syncthreads();
-        mosh2::tc::fence_after();
-        s.tc_tmem = *w.tmem_slot;
-        s.tc_kt = 4 * d.tmk;
-    }
     s.run_chunk(job.chunk_ids ? job.chunk_ids[blockIdx.x] : int(blockIdx.x));
-    if (w.tc) {
-        mosh2::tc::fence_before();
-        __syncthreads();
-        if (threadIdx.x < 32) mosh2::tc::tmem_dealloc(s.tc_tmem, mosh2::kTcCols);
-    }
 }
 
 // device copy of every model array in one precision
@@ -574,7 +558,8 @@ int mosh2_model_create(const mosh2_model_desc *d, int device, mosh2_model **out)
     CU(cudaSetDevice(device));
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) return fail(MOSH2_E_NO_DEVICE, "device %d is sm_%d%d; libmosh2 is built for sm_100a only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(MOSH2_E_NO_DEVICE, "device %d is sm_%d%d; libmosh2 is built for sm_90a only", device, prop.major, prop.minor);
     mosh2_model *m = new (std::nothrow) mosh2_model;
     if (!m) return fail(MOSH2_E_INVALID, "out of host memory");
     m->device = device; m->n_joints = d->n_joints; m->n_markers = d->n_markers; m->p_red = d->p_red; m->n_dmpl = d->n_dmpl;
@@ -1061,9 +1046,11 @@ int mosh2_mesh_distance(int32_t device, int32_t kind, double sigma, int32_t n_sa
         convert_kernel<double, float><<<int((S * 3 + 255) / 256), 256, 0, st>>>(static_cast<const double *>(d_s.p), static_cast<float *>(d_sf.p), S * 3);
         mosh2_md::soup_kernel<<<int((T + 255) / 256), 256, 0, st>>>(static_cast<const double *>(d_v.p), static_cast<const int *>(d_f.p), int(T), static_cast<float *>(d_soup.p));
         chk(cudaMemsetAsync(d_best.p, 0xff, S * sizeof(unsigned long long), st));
-        // triangle ranges: enough blocks to fill the GPU (148 SMs, several blocks each), whole tiles per block
+        // triangle ranges: enough blocks to fill the GPU (four blocks per SM), whole tiles per block
+        int n_sm = 0;
+        chk(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device));
         const int sblocks = int((S + mosh2_md::kSamplesPerBlock - 1) / mosh2_md::kSamplesPerBlock);
-        int splits = (4 * 148 + sblocks - 1) / sblocks;
+        int splits = (4 * std::max(n_sm, 1) + sblocks - 1) / sblocks;
         const int tiles = int((T + mosh2_md::kTileTris - 1) / mosh2_md::kTileTris);
         if (splits > tiles) splits = tiles;
         if (splits < 1) splits = 1;

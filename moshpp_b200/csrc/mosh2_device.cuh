@@ -14,8 +14,8 @@
 //   Jacobian  d v / d w_{a,k} = u_{a,k} x sum_{j in subtree(a)} w_j (p_j - tg_a)            (rigid part)
 //                              + Rskin Pd_j dvec(R_j)/dw_k                                    (pose blend)
 //             with u_{a,k} = Rg_par(a) vee(dR_{a,k} R_a^T); hand columns chained through C^T.
-//   normal eq A = J^T J and g = -J^T r are accumulated marker tile by marker tile (f32: J^T J on the tensor cores,
-//             tcgen05 with the accumulator in tensor memory); the prior, velocity, finger, face and DMPL / expression
+//   normal eq A = J^T J and g = -J^T r are accumulated marker tile by marker tile (J^T J on the tensor cores: f32 as
+//             split TF32 with mma.sync m16n8k8, f64 with DMMA m8n8k4); the prior, velocity, finger, face and DMPL / expression
 //             terms have closed-form contributions (Q_k = .5 inv(cov_k), diagonals).
 //   The workspace layout (struct Work) is computed on the host and arrives as a kernel parameter of shared-memory offsets.
 #pragma once
@@ -391,51 +391,63 @@ struct Work {
     SPtr<uint8_t> vis;
     SPtr<uint32_t> c_chain;   // [joint][4 words]: the joint's ancestor chain, root first, one byte per joint id, 255-padded
     SPtr<uint8_t> c_amask;    // [slot][joint]: bit i set <=> the slot's i-th skinning joint lies in the subtree of the joint
-    // tensor-core J^T J (f32, shared-memory workspace only): operand buffers (they alias A, which is idle while the
-    // tiles accumulate in tensor memory), completion barrier, tensor-memory address slot
-    SPtr<float> Xhi, Xlo;
-    SPtr<unsigned long long> mbar;
-    SPtr<unsigned int> tmem_slot;
+    SPtr<unsigned long long> mbar;   // completion barrier of the table staging
     uint32_t stage_ofs, stage_bytes;   // the staged per-model tables: one contiguous, 16-byte aligned region (c_parents ... hct)
-    int tc_ok;                // the model qualifies (f32, workspace in shared memory, n2 <= kTcM)
+    int tc_ok;                // the model qualifies for the f32 tensor-core J^T J (f32, workspace in shared memory)
     int tc;                   // set by the launcher: tensor cores in use
 };
 
 // ---------------------------------------------------------------------------------------------
-// 5th-generation tensor cores (tcgen05) for the J^T J accumulation of the f32 kernel
+// tensor cores for the J^T J accumulation of the f32 kernel; bulk asynchronous copies
 // ---------------------------------------------------------------------------------------------
-// The Jacobian tile is kept transposed, X[i][k] = Jf[k][i] (i: free variable, k: residual row of the tile), in
-// the canonical K-major no-swizzle operand layout (8 x 16-byte core matrices), split into a TF32 "hi" part and
-// a TF32 "lo" remainder.  A = sum over tiles of (hi hi^T + lo hi^T + hi lo^T) accumulates in tensor memory at
-// close to fp32 accuracy (3xTF32) while the threads already assemble the next tile.
+// A warp computes one 16x16 block of the upper triangle of Jf^T Jf over the rows of a tile with mma.sync m16n8k8 on
+// TF32 operands.  Every Jacobian value is split into a TF32 "hi" part and a TF32 "lo" remainder;
+// hi hi^T goes to one register accumulator, lo hi^T + hi lo^T + lo lo^T to another, and their sum is added to A
+// on the CUDA cores once per tile: close to fp32 accuracy (3xTF32), and the tensor core's truncating additions only
+// ever span the rows of one tile.
 constexpr int kMaxDepth = 16;         // deepest kinematic chain the tree walk unrolls (checked at model creation)
 constexpr int kDR = 28;              // floats per joint in dRl: three 3x3 derivative matrices (27) padded to 16-byte vectors
 constexpr int kM3 = 12;              // floats per padded 3x3 matrix (MtR per slot, Loc per marker vertex) and per joint in u (3 x 4)
-constexpr int kTcM = 128;            // UMMA M: free variables, zero/garbage padded (rows >= n are never read back)
-constexpr int kTcCols = 512;         // tensor-memory columns: hi*hi accumulators at 0 and 128 (alternating K steps), cross terms at 256
-M2_HD int tc_xidx(int i, int k, int kt) {        // float index of X[i][k] inside a [kTcM][kt] operand buffer
-    return (i >> 3) * (kt >> 2) * 32 + (k >> 2) * 32 + (i & 7) * 4 + (k & 3);
-}
 #if M2_GPU
 namespace tc {
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ float to_tf32(float v) { uint32_t r; asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v)); return __uint_as_float(r); }
-// shared-memory matrix descriptor, K-major, no swizzle: LBO = byte distance of the two core matrices along K,
-// SBO = byte distance of consecutive 8-row groups; version field 1 (sm_100)
-__device__ __forceinline__ uint64_t smem_desc(uint32_t addr, uint32_t lbo, uint32_t sbo) {
-    return uint64_t((addr & 0x3FFFF) >> 4) | (uint64_t((lbo >> 4) & 0x3FFF) << 16) | (uint64_t((sbo >> 4) & 0x3FFF) << 32) | (uint64_t(1) << 46);
+__device__ __forceinline__ uint32_t to_tf32(float v) { uint32_t r; asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v)); return r; }
+// D += A B, one warp: A 16x8 (row), B 8x8 (col), D 16x8 f32 (g = lane / 4, t = lane % 4: a = A[g, g+8, g, g+8][t, t, t+4, t+4],
+// b = B[t, t+4][g], d = D[g, g, g+8, g+8][2t, 2t+1, 2t, 2t+1])
+__device__ __forceinline__ void mma_tf32_m16n8k8(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-// instruction descriptor: D f32, A and B tf32, both K-major, M x N
-__device__ __forceinline__ uint32_t idesc_tf32(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | (uint32_t(N >> 3) << 17) | (uint32_t(M >> 4) << 24);
-}
-__device__ __forceinline__ void mma_tf32(uint32_t d_tmem, uint64_t a, uint64_t b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                 "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n"
-                 :: "r"(d_tmem), "l"(a), "l"(b), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void commit(uint32_t mbar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" :: "r"(mbar) : "memory");
+// One warp: block (rows i0.., columns j0..) of J^T J over `rows` rows of the row-major tile J (row length ld; columns
+// >= cols read as zero).  hh[nj] / cr[nj]: the 16x8 accumulators of columns j0 + 8 nj.. (hi hi^T, and the cross terms).
+__device__ __forceinline__ void jtj_block_tf32(const float *J, int ld, int rows, int cols, int i0, int j0,
+                                               float (&hh)[2][4], float (&cr)[2][4]) {
+    const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+    const int ca0 = i0 + g, ca1 = i0 + 8 + g, cb0 = j0 + g, cb1 = j0 + 8 + g;
+    for (int k0 = 0; k0 < rows; k0 += 8) {
+        const int k1 = k0 + t, k2 = k0 + t + 4;
+        const float *r1 = J + (k1 < rows ? k1 : 0) * ld, *r2 = J + (k2 < rows ? k2 : 0) * ld;
+        const bool in1 = k1 < rows, in2 = k2 < rows;
+        // A[i][k] = J[k][i], B[k][j] = J[k][j]
+        const float av[4] = {(in1 && ca0 < cols) ? r1[ca0] : 0.f, (in1 && ca1 < cols) ? r1[ca1] : 0.f,
+                             (in2 && ca0 < cols) ? r2[ca0] : 0.f, (in2 && ca1 < cols) ? r2[ca1] : 0.f};
+        const float bv[2][2] = {{(in1 && cb0 < cols) ? r1[cb0] : 0.f, (in2 && cb0 < cols) ? r2[cb0] : 0.f},
+                                {(in1 && cb1 < cols) ? r1[cb1] : 0.f, (in2 && cb1 < cols) ? r2[cb1] : 0.f}};
+        uint32_t ahi[4], alo[4], bhi[2][2], blo[2][2];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) { ahi[q] = to_tf32(av[q]); alo[q] = to_tf32(av[q] - __uint_as_float(ahi[q])); }
+#pragma unroll
+        for (int nj = 0; nj < 2; ++nj)
+#pragma unroll
+            for (int q = 0; q < 2; ++q) { bhi[nj][q] = to_tf32(bv[nj][q]); blo[nj][q] = to_tf32(bv[nj][q] - __uint_as_float(bhi[nj][q])); }
+#pragma unroll
+        for (int nj = 0; nj < 2; ++nj) {
+            mma_tf32_m16n8k8(hh[nj], ahi, bhi[nj][0], bhi[nj][1]);
+            mma_tf32_m16n8k8(cr[nj], alo, bhi[nj][0], bhi[nj][1]);
+            mma_tf32_m16n8k8(cr[nj], ahi, blo[nj][0], blo[nj][1]);
+            mma_tf32_m16n8k8(cr[nj], alo, blo[nj][0], blo[nj][1]);
+        }
+    }
 }
 __device__ __forceinline__ void mbar_init(uint32_t mbar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(mbar), "r"(count) : "memory");
@@ -456,25 +468,6 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void *src, uin
                  :: "r"(dst_smem), "l"(src), "r"(bytes), "r"(mbar) : "memory");
 }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_dst), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float *v) {       // 16 consecutive columns of this thread's lane
-    uint32_t r[16];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                   "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
 }  // namespace tc
 #endif
 
@@ -529,28 +522,17 @@ M2_HD void carve(Work<real, BIG> &w, const Dims &d, const Model<real> &m, Arena 
     // The Cholesky factor is alive only inside gauss_newton(); the Jacobian tiles and the other scratch of build()
     // (and the pose-blend partial sums of eval(), which live in Jt) are dead there, so they share its storage.
     // A and the Cholesky factor Lm are adjacent.  The factor is alive only inside gauss_newton(); the scratch of
-    // build() (and the pose-blend partial sums of eval(), which live in Jt) is dead there and is laid over it.  In
-    // tensor-core mode the operand tiles X start at A (idle until the accumulator is read back at the end of
-    // build()) and may run on into the factor's storage; the Jacobian tile Jf is not needed at all.
+    // build() (and the pose-blend partial sums of eval(), which live in Jt) is dead there and is laid over it.
     {
-        const bool tc_ok = sizeof(real) == 4 && !BIG && d.n2 <= kTcM && !m.dev_no_tc;
-        const size_t x_bytes = sizeof(float) * size_t(2) * kTcM * 4 * d.tmk;   // hi and lo tiles, 4 rows per marker (3 + 1 zero)
         w.A.ofs = B.take<real>(size_t(d.n2) * d.lda);
-        w.Xhi.ofs = w.A.ofs;
-        w.Xlo.ofs = w.A.ofs + uint32_t(x_bytes / 2);
-        w.tc_ok = tc_ok ? 1 : 0;
+        w.tc_ok = (sizeof(real) == 4 && !BIG && !m.dev_no_tc) ? 1 : 0;
         w.tc = 0;
         const size_t mark_b = B.off;
         w.Lm.ofs = B.take<real>(size_t(d.n2 + 1) * d.ld);
         const size_t end_b = B.off;
         B.off = mark_b;
-        if (tc_ok && w.A.ofs + x_bytes > B.off) B.off = w.A.ofs + x_bytes;
         w.Jt.ofs = B.take<real>(d.jt_size);
-#ifdef MOSH2_TC_CHECK
-        w.Jf.ofs = B.take<real>(3 * d.tmk * d.npad);      // development check: the plain tile is kept next to the operand tiles
-#else
-        w.Jf.ofs = tc_ok ? w.Jt.ofs : B.take<real>(3 * d.tmk * d.npad);
-#endif
+        w.Jf.ofs = B.take<real>(3 * d.tmk * d.npad);
         if (!BIG) {
             w.Loc.ofs = S.take<real>(3 * kM3 * d.M); w.MtR.ofs = S.take<real>(kM3 * d.S);
             w.u.ofs = S.take<real>(kM3 * d.nJ); w.dtg.ofs = S.take<real>(3 * d.nJ * d.nd + 1);
@@ -569,7 +551,7 @@ M2_HD void carve(Work<real, BIG> &w, const Dims &d, const Model<real> &m, Arena 
     w.colmap.ofs = S.take<int>(d.NX); w.colsrc.ofs = S.take<int>(d.n2); w.jlist.ofs = S.take<int>(d.nJ); w.isc.ofs = S.take<int>(8);
     w.st_colmap.ofs = S.take<int>(2 * d.NX); w.st_colsrc.ofs = S.take<int>(2 * d.n2); w.st_jlist.ofs = S.take<int>(2 * d.nJ); w.st_meta.ofs = S.take<int>(4);
     w.prof.ofs = S.take<long long>(32);
-    w.mbar.ofs = S.take<unsigned long long>(2); w.tmem_slot.ofs = S.take<unsigned int>(2);   // mbar[0]: tensor-core tiles, mbar[1]: table staging
+    w.mbar.ofs = S.take<unsigned long long>(1);
     w.vis.ofs = S.take<uint8_t>(d.M);
     // small per-model tables are always staged in shared memory (a dependent global load costs ~600 cycles and the
     // kinematic-tree walk chains three of them per level); the larger ones stay in global memory / L2.  The tables that
@@ -641,8 +623,6 @@ struct Solver {
     bool fwd_has_prior = false;   // ... including the prior products
     bool resuming = false;    // boundary repair: the chunk continues from emitted rows (run_chunk)
     real resume_diff = 0;     // ... and how far the frame just solved is from the row it replaces
-    unsigned int tc_tmem = 0, tc_phase = 0;   // tensor-memory base address, parity of the MMA completion barrier
-    int tc_kt = 0;            // rows per Jacobian tile (K extent of one tile's MMAs)
     int lin_f = -1;           // linearise mode: the frame this block works on (else -1)
 
     M2_D Solver(const Model<real> &m_, const Job<real> &j_, const Work<real, BIG> &w_, const Dims &d_, Cta c_)
@@ -1110,29 +1090,10 @@ struct Solver {
         }
     }
 
-    // ---- the three residual rows of marker `ml` of the tile (already weighted) in free-variable column `col`.
-    //      Tensor-core mode keeps the tile transposed and split (see tc_xidx): one marker's rows are one 16-byte
-    //      vector of the hi and of the lo operand (4th row zero).
+    // ---- the three residual rows of marker `ml` of the tile (already weighted) in free-variable column `col`
     M2_D void jf_store3(int ml, int col, real v0, real v1, real v2) {
-#if M2_GPU
-        if (w.tc) {
-            const float h0 = tc::to_tf32(float(v0)), h1 = tc::to_tf32(float(v1)), h2 = tc::to_tf32(float(v2));
-            const int q = tc_xidx(col, 4 * ml, tc_kt);
-            *reinterpret_cast<float4 *>(w.Xhi + q) = make_float4(h0, h1, h2, 0.f);
-            *reinterpret_cast<float4 *>(w.Xlo + q) = make_float4(tc::to_tf32(float(v0) - h0), tc::to_tf32(float(v1) - h1), tc::to_tf32(float(v2) - h2), 0.f);
-#ifndef MOSH2_TC_CHECK
-            return;
-#endif
-        }
-#endif
         real *J = w.Jf + 3 * ml * d.npad + col;
         J[0] = v0; J[d.npad] = v1; J[2 * d.npad] = v2;
-    }
-    M2_D real jf_load(int ml, int r, int col) const {
-#if M2_GPU
-        if (w.tc) { const int q = tc_xidx(col, 4 * ml + r, tc_kt); return real(w.Xhi[q] + w.Xlo[q]); }
-#endif
-        return w.Jf[(3 * ml + r) * d.npad + col];
     }
 
     // ---- a finished 3x3 block of T1: body joints go straight to their free columns of the tile (weighted and
@@ -1173,7 +1134,7 @@ struct Solver {
             else mat3_vec(w.Rg + 9 * par, om, uo);
         }
         CTA_FOR(mi, d.M) marker_local_jacobian(mi);
-        if (!w.tc) CTA_FOR(i, n * ld) w.A[i] = 0;      // (tensor-core mode: A's storage holds the operand tiles for now)
+        CTA_FOR(i, n * ld) w.A[i] = 0;
         CTA_FOR(i, n) w.g[i] = 0;
         if (d.nd) {
             // d tg_j / d delta_i = d tg_par + Rg_par (Jd_j - Jd_par): every (joint, coefficient) item sums down the joint's own
@@ -1380,10 +1341,7 @@ struct Solver {
                 const real v = w.vis[t0 + ml] ? wd : real(0);
                 if (col >= 0) jf_store3(ml, col, q == 0 ? v : real(0), q == 1 ? v : real(0), q == 2 ? v : real(0));
             }
-            if (w.tc) {
-                // short last tile: the markers that are not there must not contribute
-                CTA_FOR(idx, n * (d.tmk - tm)) jf_store3(tm + idx / n, idx % n, real(0), real(0), real(0));
-            } else {
+            {
                 const int npadc = d.npad - n;
                 CTA_FOR(idx, trows * npadc) w.Jf[(idx / npadc) * d.npad + n + idx % npadc] = 0;
             }
@@ -1432,51 +1390,13 @@ struct Solver {
                     }
                 }
             }
-#if M2_GPU
-            if (w.tc) tc::fence_async_smem();                // this thread's operand stores -> visible to the async proxy
-#endif
             M2_SYNC();
-#ifdef MOSH2_TC_CHECK
-            if (w.tc) {
-                CTA_FOR(idx, tm * 3 * n) {
-                    const int cc = idx % n, row = idx / n, ml = row / 3, r = row - 3 * ml;
-                    const int q = tc_xidx(cc, 4 * ml + r, tc_kt);
-                    const float xv = w.Xhi[q] + w.Xlo[q], jv = float(w.Jf[row * d.npad + cc]);
-                    if (fabsf(xv - jv) > 1e-4f * (fabsf(jv) + 1e-3f)) printf("X MISMATCH build %d n %d tile %d ml %d r %d col %d: X %g Jf %g\n", n_build, n, t0, ml, r, cc, xv, jv);
-                }
-                __syncthreads();
-            }
-#endif
             M2_TACC(8);
-            if (lin_f >= 0 && job.lin_J && !w.tc) {       // linearise mode: the finished rows of the tile go out as they are
+            if (lin_f >= 0 && job.lin_J) {       // linearise mode: the finished rows of the tile go out as they are
                 real *Jo = job.lin_J + (size_t(lin_f) * 3 * d.M + 3 * t0) * n;
                 CTA_FOR(idx, trows * n) { const int row = idx / n, cc = idx - row * n; Jo[idx] = w.Jf[row * d.npad + cc]; }
             }
             // T3: A += Jf^T Jf, g -= Jf^T r
-#if M2_GPU
-            if (w.tc) {
-                // tensor cores: one thread issues the tile's MMAs (hi hi^T + lo hi^T + hi lo^T per K step of 8 rows);
-                // they accumulate in tensor memory while the other threads go on with g
-                if (cta.tid == 0) {
-                    tc::fence_after();
-                    const uint32_t lbo = 128, sbo = uint32_t(tc_kt >> 2) * 128;
-                    const uint32_t ahi = tc::smem_u32(w.Xhi), alo = tc::smem_u32(w.Xlo);
-                    const uint32_t idesc = tc::idesc_tf32(kTcM, (n + 15) & ~15);
-                    // The tensor core adds every K step into the accumulator with a truncation, so the error grows
-                    // with the number of steps into one accumulator and with its magnitude: the dominant hi*hi term
-                    // alternates between two accumulators, the (2^-11 smaller) cross terms have their own.
-                    for (int ks = 0; ks < (tc_kt >> 3); ++ks) {
-                        const uint64_t dhi = tc::smem_desc(ahi + ks * 2 * lbo, lbo, sbo), dlo = tc::smem_desc(alo + ks * 2 * lbo, lbo, sbo);
-                        const bool first = t0 == 0 && ks == 0, second = t0 == 0 && ks == 1;
-                        tc::mma_tf32(tc_tmem + 128 * (ks & 1), dhi, dhi, idesc, (first || second) ? 0u : 1u);
-                        tc::mma_tf32(tc_tmem + 256, dlo, dhi, idesc, first ? 0u : 1u);
-                        tc::mma_tf32(tc_tmem + 256, dhi, dlo, idesc, 1u);
-                        tc::mma_tf32(tc_tmem + 256, dlo, dlo, idesc, 1u);
-                    }
-                    tc::commit(tc::smem_u32(w.mbar));
-                }
-            } else
-#endif
 #if M2_GPU
             if constexpr (sizeof(real) == 8) {
                 // float64: J^T J on the tensor cores as well -- mma.sync m8n8k4 (DMMA), a warp per 16x16 block of the upper
@@ -1531,6 +1451,42 @@ struct Solver {
                                 }
                             }
                 }
+            } else if (w.tc) {
+                // float32: split TF32 on the tensor cores (tc::jtj_block_tf32), a warp per 16x16 block of the upper
+                // triangle; A += (hi hi^T + cross terms), mirrored like the float64 blocks above
+                const int lane = cta.tid & 31, warp = cta.tid >> 5, nwarp = cta.nthr >> 5;
+                const int g = lane >> 2, tq = lane & 3;
+                const int nb16 = (n + 15) >> 4, ntile = nb16 * (nb16 + 1) / 2;
+                for (int tile = warp; tile < ntile; tile += nwarp) {
+                    int ti = 0, rem = tile;
+                    while (rem >= nb16 - ti) { rem -= nb16 - ti; ++ti; }
+                    const int tj = ti + rem, i0 = 16 * ti, j0 = 16 * tj;
+                    float hh[2][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}}, cr[2][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}};
+                    tc::jtj_block_tf32(w.Jf, d.npad, trows, d.npad, i0, j0, hh, cr);
+                    real old[2][2][2];
+#pragma unroll
+                    for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+                        for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                const int i = i0 + 8 * mi + g, j = j0 + 8 * ni + 2 * tq + e;
+                                old[mi][ni][e] = (j < n && i <= j) ? w.A[i * ld + j] : real(0);
+                            }
+#pragma unroll
+                    for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+                        for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                const int i = i0 + 8 * mi + g, j = j0 + 8 * ni + 2 * tq + e;
+                                if (j < n && i <= j) {
+                                    const real v = old[mi][ni][e] + (hh[ni][2 * mi + e] + cr[ni][2 * mi + e]);
+                                    w.A[i * ld + j] = v;
+                                    if (i < j) w.A[j * ld + i] = v;
+                                }
+                            }
+                }
             } else
 #endif
             {
@@ -1575,28 +1531,6 @@ struct Solver {
                         }
                 }
             }
-#if M2_GPU
-            if (w.tc) {
-                // g -= J^T r straight from the operand tiles: a marker's three rows are one 16-byte vector of the hi and of
-                // the lo operand (scalar loads with their index arithmetic kept the four warps of the columns busy for 3k
-                // cycles per tile, longer than the tile's MMAs).  Same products in the same order as the scalar loop: the
-                // ill-conditioned hand-only fits take another dog-leg path on ANY other rounding of g -- measured with
-                // three partial sums per column, in float32 and in float64.
-                CTA_FOR(cc, n) {
-                    const int xb = (cc >> 3) * (tc_kt >> 2) * 32 + (cc & 7) * 4;
-                    const float *xh = w.Xhi + xb, *xl = w.Xlo + xb;
-                    real sacc = 0;
-                    for (int ml = 0; ml < tm; ++ml) {
-                        const float4 a = *reinterpret_cast<const float4 *>(xh + 32 * ml), b = *reinterpret_cast<const float4 *>(xl + 32 * ml);
-                        const real *rp = w.rm + 3 * (t0 + ml);
-                        sacc += real(a.x + b.x) * rp[0];
-                        sacc += real(a.y + b.y) * rp[1];
-                        sacc += real(a.z + b.z) * rp[2];
-                    }
-                    w.g[cc] -= sacc;
-                }
-            } else
-#endif
             CTA_FOR(cc, n) {                                 // (six rows in flight, for the same reason; same order of the sum)
                 real s = 0;
                 for (int row = 0; row < trows; row += 6) {
@@ -1608,46 +1542,9 @@ struct Solver {
                 }
                 w.g[cc] -= s;
             }
-#if M2_GPU
-            if (w.tc) {                                      // the tile buffers may be rewritten once its MMAs are done
-                tc::mbar_wait(tc::smem_u32(w.mbar), tc_phase);
-                tc_phase ^= 1;
-            }
-#endif
             M2_SYNC();
             M2_TACC(9);
         }
-#if M2_GPU
-        if (w.tc) {
-            // accumulator (tensor memory, row i = lane i) -> A, mirrored from the upper triangle so that A is exactly
-            // symmetric; warps 0..3 own the four lane quarters
-            tc::fence_after();
-            {
-                // a warp reads the lane quarter (warp mod 4) of tensor memory; the groups of four warps share the columns
-                const int warp = cta.tid >> 5, lane = cta.tid & 31, ngrp = cta.nthr >> 7, grp = warp >> 2;
-                const int i = 32 * (warp & 3) + lane, nc = (n + 15) & ~15;
-                const uint32_t tbase = tc_tmem + (uint32_t(32 * (warp & 3)) << 16);
-                if (grp < ngrp)
-                for (int c0 = 16 * grp; c0 < nc; c0 += 16 * ngrp) {
-                    float v[16], v1[16], v2[16];
-                    tc::tmem_ld16(tbase + c0, v);
-                    tc::tmem_ld16(tbase + 128 + c0, v1);
-                    tc::tmem_ld16(tbase + 256 + c0, v2);
-#pragma unroll
-                    for (int q = 0; q < 16; ++q) v[q] = (v[q] + v1[q]) + v2[q];
-                    if (i < n) {
-#pragma unroll
-                        for (int q = 0; q < 16; ++q) {
-                            const int j = c0 + q;
-                            if (j >= i && j < n) { w.A[i * ld + j] = real(v[q]); w.A[j * ld + i] = real(v[q]); }
-                        }
-                    }
-                }
-            }
-            tc::fence_before();
-            __syncthreads();
-        }
-#endif
         // closed-form terms
         if (c.wp > real(0)) {
             const int D = d.D, ks = w.isc[0];
@@ -2541,7 +2438,7 @@ struct Solver {
         // the per-model tables: one bulk asynchronous copy of the host-built image (see carve()), waited for below
 #if M2_GPU
         {
-            const uint32_t bar = tc::smem_u32(static_cast<unsigned long long *>(w.mbar) + 1);
+            const uint32_t bar = tc::smem_u32(static_cast<unsigned long long *>(w.mbar));
             if (cta.tid == 0) tc::mbar_init(bar, 1);
             __syncthreads();
             if (cta.tid == 0) {

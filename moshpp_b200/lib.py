@@ -95,7 +95,7 @@ def load_library(path: Optional[str] = None):
         return _LIB
     p = path or default_library_path()
     if not os.path.exists(p):
-        raise Mosh2Error(f'{p} not found: build it with `python -m moshpp_b200.build` (nvcc, sm_100a). '
+        raise Mosh2Error(f'{p} not found: build it with `python -m moshpp_b200.build` (nvcc, sm_90a). '
                          'moshpp_b200 has no CPU solver.')
     lib = C.CDLL(p)
     vp = C.c_void_p

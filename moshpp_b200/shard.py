@@ -124,9 +124,10 @@ class GpuRankSolver:
     never straddle a sequence.  Different subjects get a job each, on their own streams."""
 
     def __init__(self, packs: Dict[int, object], options, frame_counts: Dict[int, int], device: int, *,
-                 chunk_warmup: int, warmup_full: int, sm_budget: int = 148, precision=None):
+                 chunk_warmup: int, warmup_full: int, sm_budget: Optional[int] = None, precision=None):
         from . import lib
-        from .chmosh import first_chunk_extra, plan_chunk_len
+        from .chmosh import NUM_SMS, first_chunk_extra, plan_chunk_len
+        sm_budget = NUM_SMS if sm_budget is None else sm_budget
         self.device = device
         prec = lib.MOSH2_F32 if precision is None else precision
         extra = first_chunk_extra(chunk_warmup, warmup_full)

@@ -1,4 +1,4 @@
-"""``mosh_stagei`` -- Stage I of MoSh++ (shape, latent markers, the poses of the picked frames) on libmosh2.so (B200).
+"""``mosh_stagei`` -- Stage I of MoSh++ (shape, latent markers, the poses of the picked frames) on libmosh2.so (H100).
 
 Reference: src/moshpp/chmosh.py:83-455 (SURVEY.md 8(f-2)).  Same inputs (``stagei_frames``: one ``{label: xyz}`` dictionary
 per picked frame, ``cfg``, ``betas_fname``, ``v_template_fname``) and the same return dictionary (chmosh.py:436-455).  The
@@ -567,7 +567,7 @@ class StageI:
 
 def mosh_stagei(stagei_frames: List[Dict[str, np.ndarray]], cfg, betas_fname=None, v_template_fname=None, *, marker_meta=None,
                 device: int = 0, backend=None) -> dict:
-    """Stage I of MoSh++ on one B200.  Positional arguments as in the reference (chmosh.py:83-85).  The marker layout is read
+    """Stage I of MoSh++ on one H100.  Positional arguments as in the reference (chmosh.py:83-85).  The marker layout is read
     from ``cfg.dirs.marker_layout.fname`` like the reference does (chmosh.py:120-125), or handed over loaded as ``marker_meta``."""
     if marker_meta is None:                                                                      # chmosh.py:120-125
         mc = cfg.mocap

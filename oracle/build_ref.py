@@ -5,7 +5,8 @@
               3-vector / 3x3 container; Eigen is not installed, so it compiles against the stand-in oracle/eigen_shim.
               (The reference's own build -- Cython + CGAL for the AABB tree of psbody.mesh -- is not runnable here.)
 
-    python -m oracle.build_ref            # needs /root/reference; the GPU box uses the prebuilt file
+    python -m oracle.build_ref            # needs the reference sources
+tests/golden/make_reference_vectors.py stores what the header computes (ref_s2m.npz); the tests read only that.
 """
 import os
 import subprocess

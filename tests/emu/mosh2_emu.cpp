@@ -2,7 +2,7 @@
 //
 // Compiles the device source with MOSH2_EMU: one "thread" (tid 0 of 1), barriers are no-ops.  The CPU
 // test-suite runs it against the oracle to validate index math and control flow of the exact code that
-// nvcc compiles for sm_100a.  It is never linked into libmosh2.so and never loaded by moshpp_b200.
+// nvcc compiles for sm_90a.  It is never linked into libmosh2.so and never loaded by moshpp_b200.
 #define MOSH2_EMU 1
 #include "../../include/mosh2.h"
 #include "../../moshpp_b200/csrc/mosh2_device.cuh"
@@ -168,8 +168,8 @@ int run(const mosh2_model_desc *desc, const mosh2_options *opt, int n_frames, co
             mosh2::Arena Sa{mosh2::kSmemHeader}, Ga{0};
             mosh2::carve<real, false>(ww, dd, hm.m, Sa, Ga);
             std::fprintf(stderr, "plan: sizeof(real)=%zu tile=%d smem=%zu bytes (limit %d)\n", sizeof(real), tile, Sa.off, 227 * 1024);
-            std::fprintf(stderr, "      A=%u Lm=%u Xhi=%u Xlo=%u Jt=%u Jf=%u Loc=%u MtR=%u u=%u dtg=%u Linv=%u tc_ok=%d\n", ww.A.ofs, ww.Lm.ofs, ww.Xhi.ofs,
-                         ww.Xlo.ofs, ww.Jt.ofs, ww.Jf.ofs, ww.Loc.ofs, ww.MtR.ofs, ww.u.ofs, ww.dtg.ofs, ww.Linv.ofs, ww.tc_ok);
+            std::fprintf(stderr, "      A=%u Lm=%u Jt=%u Jf=%u Loc=%u MtR=%u u=%u dtg=%u Linv=%u tc_ok=%d\n", ww.A.ofs, ww.Lm.ofs,
+                         ww.Jt.ofs, ww.Jf.ofs, ww.Loc.ofs, ww.MtR.ofs, ww.u.ofs, ww.dtg.ofs, ww.Linv.ofs, ww.tc_ok);
         }
         hm.m.tile_markers = 20;
         hm.m.dev_no_tc = 1;

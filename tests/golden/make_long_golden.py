@@ -6,7 +6,9 @@ frame-serial numpy solve.
     python tests/golden/make_long_golden.py KEY [KEY ...]       # keys: see LONG below
 
 Poses / translations are stored as float32 (rounding 6e-8, four orders below the tolerances they are
-compared at); per-frame data SSE and frame ids as float64 / int32.
+compared at); per-frame data SSE and frame ids as float64 / int32.  The 4000-frame sequences keep the pose (and dmpl)
+rows of their first POSE_FRAMES solved frames only, so that every fixture stays below 1 MB; translations, data SSE
+and frame ids cover every frame.
 """
 import os
 import sys
@@ -36,6 +38,12 @@ LONG = {
     # occlusion gap straddling a chunk boundary (ADVICE r1): built by the test from C2 with frames 90..139 blanked
     'GAP': ('C2', dict(frames=240)),
 }
+POSE_FRAMES = 2000      # pose / dmpl rows stored per fixture (a contiguous run from the first solved frame)
+
+
+def shrink(arrs):
+    """The stored subset: pose and dmpl rows of the first POSE_FRAMES solved frames."""
+    return {k: (v[:POSE_FRAMES] if k in ('pose', 'dmpls') else v) for k, v in arrs.items()}
 
 
 def blank_gap(case):
@@ -68,7 +76,7 @@ def main():
             arrs['dmpls'] = out['dmpls'].astype(np.float32)
         if key in ('C2', 'GAP'):
             arrs['markers_sim'] = np.concatenate(dbg['markers_sim']).astype(np.float32)
-        np.savez_compressed(os.path.join(HERE, f'long_{key}.npz'), **arrs)
+        np.savez_compressed(os.path.join(HERE, f'long_{key}.npz'), **shrink(arrs))
         print(key, out['fullpose'].shape, st, 'written', flush=True)
 
 

@@ -166,6 +166,39 @@ def prior_and_marker_vectors():
     print('ref_lms.npz:', {k: v.shape for k, v in cases.items() if k.startswith('closest')})
 
 
+S2M_KINDS = ((0, 1.0), (1, 1.0), (2, 0.05), (2, 0.5))     # (oracle.mesh_distance KIND_*, sigma)
+
+
+def s2m_vectors():
+    """scan2mesh/mesh_distance/sample2meshdist.h, UNMODIFIED, through oracle/_ref/libs2m.so (oracle/build_ref.py): value and
+    the four gradients of one sample against one triangle, for every part and robustifier, on 40 random cases
+    -> ref_s2m.npz."""
+    import ctypes as C
+    from oracle import build_ref
+    lib = C.CDLL(build_ref.build(force=True))
+    dp = C.POINTER(C.c_double)
+    lib.s2m_tri.restype = C.c_double
+    lib.s2m_tri.argtypes = [C.c_int, C.c_double, C.c_int, dp, dp, dp, dp, dp, dp, dp, dp]
+    rng = np.random.default_rng(7)
+    xabc = np.zeros((40, 4, 3))
+    val = np.zeros((40, len(S2M_KINDS), 7))
+    grad = np.zeros((40, len(S2M_KINDS), 7, 4, 3))
+    for trial in range(40):
+        a, b, c = rng.normal(0, 0.3, (3, 3))
+        x = (a + b + c) / 3 + rng.normal(0, 0.2, 3)
+        xabc[trial] = x, a, b, c
+        args = [np.ascontiguousarray(v) for v in (x, a, b, c)]
+        for ki, (kind, sigma) in enumerate(S2M_KINDS):
+            for part in range(7):
+                bufs = [np.zeros(3) for _ in range(4)]
+                val[trial, ki, part] = lib.s2m_tri(kind, sigma, part, *[v.ctypes.data_as(dp) for v in args],
+                                                   *[v.ctypes.data_as(dp) for v in bufs])
+                grad[trial, ki, part] = bufs
+    np.savez_compressed(os.path.join(HERE, 'ref_s2m.npz'), xabc=xabc, kinds=np.array(S2M_KINDS), value=val, grad=grad)
+    print('ref_s2m.npz:', val.shape)
+
+
 if __name__ == '__main__':
     main()
     prior_and_marker_vectors()
+    s2m_vectors()

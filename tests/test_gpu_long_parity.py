@@ -28,9 +28,11 @@ def _full_case(cases, key):
 
 
 def _report(tag, pose, trans, sse, gold, body_dof, tol_body=TOL_BODY):
-    """Per-frame deviations from the fixture; returns the dict the assertions use and prints the summary."""
+    """Per-frame deviations from the fixture; returns the dict the assertions use and prints the summary.  (The
+    fixtures of the 4000-frame sequences hold the poses of their first solved frames only: make_long_golden.POSE_FRAMES.)"""
     fid = gold['frame_ids']
-    dp = np.abs(pose - gold['pose'].astype(np.float64))
+    npose = len(gold['pose'])
+    dp = np.abs(pose[:npose] - gold['pose'].astype(np.float64))
     bd = min(body_dof, 66)
     body = dp[:, :bd].max(1)
     finger = dp[:, bd:].max(1) if dp.shape[1] > bd else np.zeros(len(dp))
@@ -77,7 +79,7 @@ def _excursions(over):
 # therefore per frame for >= 99 % of the frames plus bounded, short excursions, and the exact mode (float64) covers all.
 @pytest.mark.parametrize('key,kw,tol_body,max_over', [
     ('C2', {}, TOL_BODY, 0.0),                       # BASELINE configs[1]: 500 frames -> chunks of 4
-    ('NS', {}, TOL_BODY, 0.01),                      # north-star target: 4000-frame SMPL-H -> chunks of 28
+    ('NS', {}, TOL_BODY, 0.01),                      # north-star target: 4000-frame SMPL-H -> chunks of 30
     ('C3', dict(chunk_len=28), 1e-4, 0.0),           # 640-frame window of configs[2], cut with the chunk length of 4000 frames
     ('C3F', {}, 1e-4, 0.0),                          # configs[2] in full: SMPL-X + DMPL, 4000 frames (default: the exact preset)
     ('C4L', {}, 5e-3, 0.01),                         # configs[3]: hand-only model, the wrist is weakly observed (BASELINE.md 4)
@@ -99,7 +101,7 @@ def test_default_product_path_vs_sequential_oracle(cases, key, kw, tol_body, max
                   b['pose_reduced'], out['trans'], out['stageii_debug_details']['stageii_errs']['data'], gold,
                   case['pack'].body_dof, tol_body)
     if 'dmpls' in gold.files:
-        dd = np.abs(out['dmpls'] - gold['dmpls']).max(1)
+        dd = np.abs(out['dmpls'][:len(gold['dmpls'])] - gold['dmpls']).max(1)
         print(f'    dmpl coefficients max {dd.max():.2e}, frames over 1e-2: {(dd > 1e-2).sum()}')
     st = b['status']
     assert not (st & (lib.ST_GN_FALLBACK | lib.ST_MAXITER)).any()
@@ -107,9 +109,9 @@ def test_default_product_path_vs_sequential_oracle(cases, key, kw, tol_body, max
     # branches of the reference's own decision); such chunks stay flagged
     assert bc['unverified_chunks'] <= max(1, 0.05 * b['chunks'])
     assert int(((st & lib.ST_SHORT_WARMUP) != 0).sum()) <= bc['unverified_chunks'] * b['chunk_len']
-    n = len(rep['body'])
     for name, tol in (('body', tol_body), ('finger', TOL_FINGER), ('trans', TOL_TRANS), ('sse', TOL_SSE)):
         over = rep[name] > tol
+        n = len(over)
         runs = _excursions(over)
         assert over.sum() <= max_over * n, (name, int(over.sum()), n)
         assert np.sqrt((rep[name] ** 2).mean()) <= tol, name                       # typical frame: well inside

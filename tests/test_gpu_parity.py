@@ -1,4 +1,4 @@
-"""Parity tests proper: the CUDA library (through the C-ABI) against the float64 oracle on a B200."""
+"""Parity tests proper: the CUDA library (through the C-ABI) against the float64 oracle on an H100."""
 import numpy as np
 import pytest
 
@@ -183,9 +183,10 @@ def test_library_is_the_cuda_build():
     assert 'libmosh2.so' in maps
 
 
-def test_tcgen05_jtj_building_block():
+def test_tf32_jtj_building_block():
     """Stand-alone kernel (tests/tc): J^T J on the tensor cores with the split-TF32 / separate-accumulator scheme the
-    Stage-II kernel uses, against a float64 product, for the operand shapes of all model families (incl. N = 16)."""
+    Stage-II kernel uses (its own device function), against a float64 product, for the operand shapes of all model
+    families."""
     import subprocess
     from moshpp_b200 import build
     exe = build.build_tc_test()

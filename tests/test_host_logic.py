@@ -45,7 +45,7 @@ def test_result_assembly_matches_reference_layout(cases, emu):
 
 
 def test_auto_chunk_len():
-    assert chmosh.auto_chunk_len(500) == 4 and chmosh.auto_chunk_len(4000) == 28 and chmosh.auto_chunk_len(12) == 4
+    assert chmosh.auto_chunk_len(500) == 4 and chmosh.auto_chunk_len(4000) == 31 and chmosh.auto_chunk_len(12) == 4
     assert chmosh.auto_chunk_len(4000, sm_budget=37) == 109
 
 
@@ -65,10 +65,11 @@ def test_planned_schedule_counts_chunks_like_the_chunk_table():
             for E in (0, 3, 52):
                 assert chmosh.count_chunks(F, L, E) == brute(F, L, E), (F, L, E)
     assert chmosh.first_chunk_extra(64, 48) == 52 and chmosh.first_chunk_extra(256, -1) == 256 and chmosh.first_chunk_extra(0, 0) == 0
-    L = chmosh.plan_chunk_len([4000], 148, 64, 48, first_extra=52)
-    assert L == 27 and chmosh.count_chunks(4000, L, 52) <= 148 < chmosh.count_chunks(4000, L - 1, 52)
-    L5 = chmosh.plan_chunk_len([4000] * 32, 148, 64, 48, first_extra=52)
-    assert sum(chmosh.count_chunks(4000, L5, 52) for _ in range(32)) <= 2 * 148
+    S = chmosh.NUM_SMS
+    L = chmosh.plan_chunk_len([4000], S, 64, 48, first_extra=52)
+    assert L == 30 and chmosh.count_chunks(4000, L, 52) <= S < chmosh.count_chunks(4000, L - 1, 52)
+    L5 = chmosh.plan_chunk_len([4000] * 32, S, 64, 48, first_extra=52)
+    assert sum(chmosh.count_chunks(4000, L5, 52) for _ in range(32)) <= 2 * S
 
 
 def test_options_follow_the_config(cases):

@@ -1,4 +1,4 @@
-"""Measures the BASELINE.json configurations on one B200 (development / reporting tool, not the product):
+"""Measures the BASELINE.json configurations on one H100 (development / reporting tool, not the product):
 C1..C4 at full size through the C-ABI job calls, a C5 shard (4 sequences x 4000 frames on one GPU, jobs on
 separate streams), and optionally the CPU oracle in reference-cost mode on the first frames of each config.
 
@@ -27,7 +27,7 @@ def load(name, d, frames=None, seq_idx=0, hand_side='left'):
     return case, pk, opts, obs, vis
 
 
-def run_jobs(items, reps=3, warmup=chmosh.DEFAULT_WARMUP, precision=lib.MOSH2_F32, sm_budget=148):
+def run_jobs(items, reps=3, warmup=chmosh.DEFAULT_WARMUP, precision=lib.MOSH2_F32, sm_budget=chmosh.NUM_SMS):
     """items: list of (pk, opts, obs, vis).  All jobs are launched back to back on their own streams."""
     models = [lib.Model(pk) for pk, _, _, _ in items]
     jobs = []

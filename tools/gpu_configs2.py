@@ -1,6 +1,6 @@
 """Reporting tool (GPU): the BASELINE.json configurations C1..C4 at full size through the drop-in callable
 (chmosh.mosh_stageii, default fast mode: verified time-parallel schedule), device time = sum of the launches of the call.
-    python tools/gpu_configs2.py > gpurun_out/r02_configs.jsonl"""
+    python tools/gpu_configs2.py > configs.jsonl"""
 import json, os, sys, tempfile, time
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -1,4 +1,4 @@
-"""Development tool (GPU): solve one small case once (for compute-sanitizer).  Usage: python tools/gpu_one.py C4 f32"""
+"""Development tool (GPU): solve one small case once.  Usage: python tools/gpu_one.py C4 f32"""
 import os
 import sys
 import tempfile

@@ -1,4 +1,4 @@
-"""Development tool (GPU): a small chunked + verified + repaired solve (used under compute-sanitizer)."""
+"""Development tool (GPU): a small chunked + verified + repaired solve."""
 import os, sys, tempfile
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -1,6 +1,6 @@
 """Development tool (CPU): how well-conditioned is the REFERENCE's own result?  Runs the float64 oracle on a window of the
 north-star sequence twice -- once as is, once with the observations perturbed by N(0, eps) (eps << the 1 mm marker noise) --
-and prints the pose difference per frame.  Output of this script: profiles/r02_oracle_sensitivity.txt."""
+and prints the pose difference per frame."""
 import sys, tempfile, time
 import os
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
