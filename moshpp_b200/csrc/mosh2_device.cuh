@@ -275,6 +275,13 @@ M2_HD void cross3(const real *a, const real *b, real *o) {
     o[1] = a[2] * b[0] - a[0] * b[2];
     o[2] = a[0] * b[1] - a[1] * b[0];
 }
+// block (bi, bj), bi <= bj, of the upper triangle of an nb x nb grid of blocks that are numbered row by row
+M2_HD void upper_block(int idx, int nb, int &bi, int &bj) {
+    int ti = 0, rem = idx;
+    while (rem >= nb - ti) { rem -= nb - ti; ++ti; }
+    bi = ti;
+    bj = ti + rem;
+}
 
 // R = exp([w]x) and dR[k] = dR/dw_k (cv2.Rodrigues convention), cancellation-free near 0.
 // `only_k` >= 0: this caller writes only dR[only_k] (and R when only_k == 0) -- three threads share a joint.
@@ -1025,22 +1032,30 @@ struct Solver {
         }
     }
 
-    // ---- pose-blend vectors of slot (marker mi, vertex t) for joint a: p[3 e + c] (nine 16-byte loads, issued together)
-    M2_D void t1_load(int mi, int a, int t, real *p) {
-        const size_t es = size_t(d.S) * 4;
-        const real *P = m.pd4 + size_t(a >= 1 ? a - 1 : 0) * 9 * es + size_t(3 * mi + t) * 4;
-#pragma unroll
-        for (int e = 0; e < 9; ++e) {
-            const Vec4<real> v = ld4(P + e * es);
-            p[3 * e] = v.x; p[3 * e + 1] = v.y; p[3 * e + 2] = v.z;
-        }
+    // ---- the padded 3x3 matrices of slot sl in registers: MtR (pose-blend part of T1) and Loc (rigid part)
+    M2_D void slot_mats(int sl, real (&Mt)[9], real (&Lc)[9]) {
+        const real *Mp = w.MtR + kM3 * sl, *Lp = w.Loc + kM3 * sl;
+        const Vec4<real> m0 = ld4(Mp), m1 = ld4(Mp + 4), m2 = ld4(Mp + 8), l0 = ld4(Lp), l1 = ld4(Lp + 4), l2 = ld4(Lp + 8);
+        Mt[0] = m0.x; Mt[1] = m0.y; Mt[2] = m0.z; Mt[3] = m0.w; Mt[4] = m1.x; Mt[5] = m1.y; Mt[6] = m1.z; Mt[7] = m1.w; Mt[8] = m2.x;
+        Lc[0] = l0.x; Lc[1] = l0.y; Lc[2] = l0.z; Lc[3] = l0.w; Lc[4] = l1.x; Lc[5] = l1.y; Lc[6] = l1.z; Lc[7] = l1.w; Lc[8] = l2.x;
     }
 
-    // ---- contribution of slot (marker mi, vertex t) to the 3x3 Jacobian block of joint a:  blk[r*3+k] +=
-    M2_D void t1_compute(int mi, int a, int t, const real *p, real *blk) {
-        const int s = 3 * mi + t;
+    // ---- T1: the part of slot sl (marker sl / 3, vertex sl % 3) in the 3x3 Jacobian block of joint a, blk[3 r + k] (row r,
+    //      rotation axis k).  Mt, Lc: slot_mats(sl); Pslot: the slot's pose-blend vectors, m.pd4 + 4 sl.
+    M2_D void slot_pose_block(int sl, int a, const real (&Mt)[9], const real (&Lc)[9], const real *Pslot, real (&blk)[9]) {
+        const int mask = w.c_amask[sl * d.nJ + a];          // the slot's skinning joints in the subtree of a
+#pragma unroll
+        for (int q = 0; q < 9; ++q) blk[q] = 0;
         if (a >= 1) {
-            // pose-blend part: E[c][k] = sum_e Pd[c][e] dR_k[e], then blk += (Loc_t Rsk_s) E
+            // pose-blend part: E[c][k] = sum_e Pd[c][e] dR_k[e], then blk = (Loc_t Rsk_s) E
+            // (requesting the NEXT joint's vectors here, right after E has consumed the current ones, was
+            // measured slower: the loop is bound by instruction issue -- about 500 warp instructions per
+            // joint, a quarter of them FMAs -- not by the latency of these loads)
+            const size_t es = size_t(d.S) * 4;
+            const real *P = Pslot + size_t(a - 1) * 9 * es;
+            Vec4<real> pv[9];
+#pragma unroll
+            for (int e = 0; e < 9; ++e) pv[e] = ld4(P + e * es);
             const real *dR = w.dRl + kDR * a;
             real dr[kDR];
 #pragma unroll
@@ -1052,32 +1067,39 @@ struct Solver {
 #pragma unroll
             for (int e = 0; e < 9; ++e) {
                 const real q0 = dr[e], q1 = dr[9 + e], q2 = dr[18 + e];
-                E[0] += p[3 * e] * q0; E[1] += p[3 * e] * q1; E[2] += p[3 * e] * q2;
-                E[3] += p[3 * e + 1] * q0; E[4] += p[3 * e + 1] * q1; E[5] += p[3 * e + 1] * q2;
-                E[6] += p[3 * e + 2] * q0; E[7] += p[3 * e + 2] * q1; E[8] += p[3 * e + 2] * q2;
+                E[0] += pv[e].x * q0; E[1] += pv[e].x * q1; E[2] += pv[e].x * q2;
+                E[3] += pv[e].y * q0; E[4] += pv[e].y * q1; E[5] += pv[e].y * q2;
+                E[6] += pv[e].z * q0; E[7] += pv[e].z * q1; E[8] += pv[e].z * q2;
             }
-            const real *Mp = w.MtR + kM3 * s;
-            const Vec4<real> m0 = ld4(Mp), m1 = ld4(Mp + 4), m2 = ld4(Mp + 8);
-            const real Mt[9] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w, m2.x};
 #pragma unroll
             for (int r = 0; r < 3; ++r)
 #pragma unroll
                 for (int k = 0; k < 3; ++k)
-                    blk[3 * r + k] += Mt[3 * r] * E[k] + Mt[3 * r + 1] * E[3 + k] + Mt[3 * r + 2] * E[6 + k];
+                    blk[3 * r + k] = Mt[3 * r] * E[k] + Mt[3 * r + 1] * E[3 + k] + Mt[3 * r + 2] * E[6 + k];
         }
         // rigid part: the slot's skinning joints below a turn about a:  d v / d omega_{a,k} = u_{a,k} x q
-        const int mask = w.c_amask[s * d.nJ + a];
         if (mask) {
             real q[3] = {0, 0, 0};
-            for (int i = 0; i < d.kw; ++i)
-                if ((mask >> i) & 1) {
-                    const real wt = w.c_wv[s * d.kw + i];
-                    const real *pp = w.pj + 3 * (s * d.kw + i);
-                    for (int r = 0; r < 3; ++r) q[r] += wt * (pp[r] - w.tg[3 * a + r]);
-                }
-            const real *Lp = w.Loc + kM3 * s;
-            const Vec4<real> l0 = ld4(Lp), l1 = ld4(Lp + 4), l2 = ld4(Lp + 8);
-            const real L[9] = {l0.x, l0.y, l0.z, l0.w, l1.x, l1.y, l1.z, l1.w, l2.x};
+            if (d.kw == 4) {
+                // four skinning joints per slot (every released model): weights and joint-relative positions
+                // of the slot as four 16-byte vectors, the subtree mask applied to the weights -- no branches
+                const Vec4<real> wv = ld4(w.c_wv + 4 * sl);
+                const real *pp = w.pj + 12 * sl;
+                const Vec4<real> a0 = ld4(pp), a1 = ld4(pp + 4), a2 = ld4(pp + 8);
+                const real g0 = w.tg[3 * a], g1 = w.tg[3 * a + 1], g2 = w.tg[3 * a + 2];
+                const real w0 = (mask & 1) ? wv.x : real(0), w1 = (mask & 2) ? wv.y : real(0);
+                const real w2 = (mask & 4) ? wv.z : real(0), w3 = (mask & 8) ? wv.w : real(0);
+                q[0] = w0 * (a0.x - g0); q[1] = w0 * (a0.y - g1); q[2] = w0 * (a0.z - g2);
+                q[0] += w1 * (a0.w - g0); q[1] += w1 * (a1.x - g1); q[2] += w1 * (a1.y - g2);
+                q[0] += w2 * (a1.z - g0); q[1] += w2 * (a1.w - g1); q[2] += w2 * (a2.x - g2);
+                q[0] += w3 * (a2.y - g0); q[1] += w3 * (a2.z - g1); q[2] += w3 * (a2.w - g2);
+            } else
+                for (int i = 0; i < d.kw; ++i)
+                    if ((mask >> i) & 1) {
+                        const real wt = w.c_wv[sl * d.kw + i];
+                        const real *pp = w.pj + 3 * (sl * d.kw + i);
+                        for (int r = 0; r < 3; ++r) q[r] += wt * (pp[r] - w.tg[3 * a + r]);
+                    }
 #pragma unroll
             for (int k = 0; k < 3; ++k) {
                 const Vec4<real> uk = ld4(w.u + kM3 * a + 4 * k);
@@ -1085,7 +1107,7 @@ struct Solver {
                 real cr[3];
                 cross3(uv, q, cr);
 #pragma unroll
-                for (int r = 0; r < 3; ++r) blk[3 * r + k] += L[3 * r] * cr[0] + L[3 * r + 1] * cr[1] + L[3 * r + 2] * cr[2];
+                for (int r = 0; r < 3; ++r) blk[3 * r + k] += Lc[3 * r] * cr[0] + Lc[3 * r + 1] * cr[1] + Lc[3 * r + 2] * cr[2];
             }
         }
     }
@@ -1096,31 +1118,21 @@ struct Solver {
         J[0] = v0; J[d.npad] = v1; J[2 * d.npad] = v2;
     }
 
-    // ---- a finished 3x3 block of T1: body joints go straight to their free columns of the tile (weighted and
-    //      masked); hand joints go to the full-pose tile for the PCA chain (T2b)
-    M2_D void t1_store(int ml, int mi, int a, const real *blk) {
+    // ---- column k (rows b0, b1, b2) of the finished 3x3 T1 block of marker `ml` of the tile and joint a: body joints go
+    //      straight to their free column of the tile, weighted by sc (wd, or 0 for an invisible marker); hand joints go to
+    //      the full-pose tile for the PCA chain (T2b)
+    M2_D void pose_col_store(int ml, int a, int k, real sc, real b0, real b1, real b2) {
         if (3 * a < m.body_dof) {
-            const real sc = w.vis[mi] ? wd : real(0);
-#pragma unroll
-            for (int k = 0; k < 3; ++k) {
-                const int col = w.colmap[3 + 3 * a + k];
-                if (col >= 0) jf_store3(ml, col, blk[k] * sc, blk[3 + k] * sc, blk[6 + k] * sc);
-            }
+            const int col = w.colmap[3 + 3 * a + k];
+            if (col >= 0) jf_store3(ml, col, b0 * sc, b1 * sc, b2 * sc);
         } else {
-#pragma unroll
-            for (int r = 0; r < 3; ++r)
-#pragma unroll
-                for (int k = 0; k < 3; ++k) w.Jt[(3 * ml + r) * d.NCt + (3 * a - m.body_dof) + k] = blk[3 * r + k];
+            real *Jr = w.Jt + 3 * ml * d.NCt + (3 * a - m.body_dof) + k;
+            Jr[0] = b0; Jr[d.NCt] = b1; Jr[2 * d.NCt] = b2;
         }
     }
 
-    // ---- normal equations at the state of the latest eval():  A = J^T J (full symmetric), g = -J^T r
-    M2_D void build(const real *xs, const StepCfg<real> &c) {
-        ++n_build;
-        M2_T0();
-        const real *th = xs + 3;
-        const real *dl = xs + 3 + d.PR;
-        const int n = c.n, ld = d.lda;
+    // ---- u_{a,k} = Rg_par(a) vee(dR_{a,k} R_a^T), the rotation axes of the rigid part of T1
+    M2_D void joint_axes() {
         CTA_FOR(idx, 3 * d.nJ) {
             const int a = idx / 3, k = idx - 3 * a;
             const real *D = w.dRl + kDR * a + 9 * k, *R = w.Rl + 9 * a;
@@ -1133,419 +1145,331 @@ struct Solver {
             if (par < 0) { for (int q = 0; q < 3; ++q) uo[q] = om[q]; }
             else mat3_vec(w.Rg + 9 * par, om, uo);
         }
-        CTA_FOR(mi, d.M) marker_local_jacobian(mi);
-        CTA_FOR(i, n * ld) w.A[i] = 0;
-        CTA_FOR(i, n) w.g[i] = 0;
-        if (d.nd) {
-            // d tg_j / d delta_i = d tg_par + Rg_par (Jd_j - Jd_par): every (joint, coefficient) item sums down the joint's own
-            // ancestor chain (root first, the order of the level-wise recursion), so there is no barrier per tree level
-            CTA_FOR(q, d.nJ * d.nd) {
-                const int j = q / d.nd, i = q - j * d.nd;
-                uint32_t cw[kMaxDepth / 4];
+    }
+
+    // ---- d tg_j / d delta_i = d tg_par + Rg_par (Jd_j - Jd_par): every (joint, coefficient) item sums down the joint's own
+    //      ancestor chain (root first, the order of the level-wise recursion), so there is no barrier per tree level
+    M2_D void dtg_chains() {
+        if (!d.nd) return;
+        CTA_FOR(q, d.nJ * d.nd) {
+            const int j = q / d.nd, i = q - j * d.nd;
+            uint32_t cw[kMaxDepth / 4];
 #pragma unroll
-                for (int u = 0; u < kMaxDepth / 4; ++u) cw[u] = w.c_chain[j * (kMaxDepth / 4) + u];
-                int prev = int(cw[0] & 255u);
-                real acc[3];
-                for (int r = 0; r < 3; ++r) acc[r] = w.c_jd[(3 * prev + r) * d.nd + i];
-                for (int k = 1; k < kMaxDepth; ++k) {
-                    const int cj = int((cw[k >> 2] >> (8 * (k & 3))) & 255u);
-                    if (cj == 255) break;
-                    real dj[3], t[3];
-                    for (int r = 0; r < 3; ++r) dj[r] = w.c_jd[(3 * cj + r) * d.nd + i] - w.c_jd[(3 * prev + r) * d.nd + i];
-                    mat3_vec(w.Rg + 9 * prev, dj, t);
-                    for (int r = 0; r < 3; ++r) acc[r] = acc[r] + t[r];
-                    prev = cj;
-                }
-                real *o = w.dtg + 3 * (j * d.nd + i);
-                for (int r = 0; r < 3; ++r) o[r] = acc[r];
+            for (int u = 0; u < kMaxDepth / 4; ++u) cw[u] = w.c_chain[j * (kMaxDepth / 4) + u];
+            int prev = int(cw[0] & 255u);
+            real acc[3];
+            for (int r = 0; r < 3; ++r) acc[r] = w.c_jd[(3 * prev + r) * d.nd + i];
+            for (int k = 1; k < kMaxDepth; ++k) {
+                const int cj = int((cw[k >> 2] >> (8 * (k & 3))) & 255u);
+                if (cj == 255) break;
+                real dj[3], t[3];
+                for (int r = 0; r < 3; ++r) dj[r] = w.c_jd[(3 * cj + r) * d.nd + i] - w.c_jd[(3 * prev + r) * d.nd + i];
+                mat3_vec(w.Rg + 9 * prev, dj, t);
+                for (int r = 0; r < 3; ++r) acc[r] = acc[r] + t[r];
+                prev = cj;
             }
+            real *o = w.dtg + 3 * (j * d.nd + i);
+            for (int r = 0; r < 3; ++r) o[r] = acc[r];
         }
-        M2_SYNC();
-        CTA_FOR(s, d.S) mat3_mul(w.Loc + kM3 * s, w.Rsk + 9 * s, w.MtR + kM3 * s);
-        M2_SYNC();
-        M2_TACC(6);
-        for (int t0 = 0; t0 < d.M; t0 += d.tmk) {
-            const int tm = (d.M - t0 < d.tmk) ? d.M - t0 : d.tmk;
-            // T1: full-pose 3x3 Jacobian blocks (marker, joint) for the joints this step needs.  A block is the sum
-            // over the marker's three slots; on the GPU three adjacent lanes take one slot each (their pose-blend
-            // vectors are adjacent in memory) and are summed with two shuffles.
-            {
+    }
+
+    // ---- T1: full-pose 3x3 Jacobian blocks (marker, joint) of the tile's tm markers from t0 on, for the joints this step
+    //      needs.  A block is the sum over the marker's three slots; on the GPU three adjacent lanes take one slot each (their
+    //      pose-blend vectors are adjacent in memory) and are summed with two shuffles.
+    M2_D void tile_pose_columns(int t0, int tm) {
 #if M2_GPU
-                // A warp owns up to ten markers of the tile (lane = marker vertex: 30 lanes) and walks a strided share
-                // of the joints, so everything that belongs to the slot stays in registers.  The three partial 3x3
-                // blocks of a marker are summed by rotation -- lane t ends up with column t -- and every lane stores
-                // its own column.
-                const int lane = cta.tid & 31, warp = cta.tid >> 5, nwarp = cta.nthr >> 5;
-                const int t = lane % 3, grp = lane / 3;
-                const int nmg = (tm + 9) / 10, nch = nwarp / nmg;         // marker groups, joint shares
-                const int mg = warp % nmg, ch = warp / nmg;
-                const int ml = mg * 10 + grp;
-                const bool valid = lane < 30 && ml < tm;
-                if (ch < nch) {
-                    const int mi = t0 + (valid ? ml : 0), sl = 3 * mi + t;
-                    const real sc = (valid && w.vis[mi]) ? wd : real(0);
-                    // slot constants
-                    real Mt[9], Lc[9];
-                    {
-                        const real *Mp = w.MtR + kM3 * sl, *Lp = w.Loc + kM3 * sl;
-                        const Vec4<real> m0 = ld4(Mp), m1 = ld4(Mp + 4), m2 = ld4(Mp + 8), l0 = ld4(Lp), l1 = ld4(Lp + 4), l2 = ld4(Lp + 8);
-                        Mt[0] = m0.x; Mt[1] = m0.y; Mt[2] = m0.z; Mt[3] = m0.w; Mt[4] = m1.x; Mt[5] = m1.y; Mt[6] = m1.z; Mt[7] = m1.w; Mt[8] = m2.x;
-                        Lc[0] = l0.x; Lc[1] = l0.y; Lc[2] = l0.z; Lc[3] = l0.w; Lc[4] = l1.x; Lc[5] = l1.y; Lc[6] = l1.z; Lc[7] = l1.w; Lc[8] = l2.x;
-                    }
-                    const size_t es = size_t(d.S) * 4;
-                    const real *Pslot = m.pd4 + size_t(sl) * 4;
-                    const uint8_t *mrow = w.c_amask + sl * d.nJ;
-                    const int src1 = lane - t + (t + 2) % 3, src2 = lane - t + (t + 1) % 3;   // lanes whose t is t-1, t-2 (mod 3)
+        // A warp owns up to ten markers of the tile (lane = marker vertex: 30 lanes) and walks a strided share
+        // of the joints, so everything that belongs to the slot stays in registers.  The three partial 3x3
+        // blocks of a marker are summed by rotation -- lane t ends up with column t -- and every lane stores
+        // its own column.
+        const int lane = cta.tid & 31, warp = cta.tid >> 5, nwarp = cta.nthr >> 5;
+        const int t = lane % 3, grp = lane / 3;
+        const int nmg = (tm + 9) / 10, nch = nwarp / nmg;         // marker groups, joint shares
+        const int mg = warp % nmg, ch = warp / nmg;
+        const int ml = mg * 10 + grp;
+        const bool valid = lane < 30 && ml < tm;
+        if (ch < nch) {
+            const int mi = t0 + (valid ? ml : 0), sl = 3 * mi + t;
+            const real sc = (valid && w.vis[mi]) ? wd : real(0);
+            real Mt[9], Lc[9];
+            slot_mats(sl, Mt, Lc);
+            const real *Pslot = m.pd4 + size_t(sl) * 4;
+            const int src1 = lane - t + (t + 2) % 3, src2 = lane - t + (t + 1) % 3;   // lanes whose t is t-1, t-2 (mod 3)
 #pragma unroll 1
-                    for (int ji = ch; ji < njl; ji += nch) {
-                        const int a = w.jlist[ji];
-                        real blk[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-                        if (a >= 1) {
-                            // (requesting the NEXT joint's vectors here, right after E has consumed the current ones, was
-                            // measured slower: the loop is bound by instruction issue -- about 500 warp instructions per
-                            // joint, a quarter of them FMAs -- not by the latency of these loads)
-                            const real *P = Pslot + size_t(a - 1) * 9 * es;
-                            Vec4<real> pv[9];
+            for (int ji = ch; ji < njl; ji += nch) {
+                const int a = w.jlist[ji];
+                real blk[9];
+                slot_pose_block(sl, a, Mt, Lc, Pslot, blk);
+                // lane t collects column t of the marker's block: own part + the parts of the two other vertices
+                real col3[3];
 #pragma unroll
-                            for (int e = 0; e < 9; ++e) pv[e] = ld4(P + e * es);
-                            const real *dR = w.dRl + kDR * a;
-                            real dr[kDR];
-#pragma unroll
-                            for (int v = 0; v < kDR / 4; ++v) {
-                                const Vec4<real> q4 = ld4(dR + 4 * v);
-                                dr[4 * v] = q4.x; dr[4 * v + 1] = q4.y; dr[4 * v + 2] = q4.z; dr[4 * v + 3] = q4.w;
-                            }
-                            real E[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-#pragma unroll
-                            for (int e = 0; e < 9; ++e) {
-                                const real q0 = dr[e], q1 = dr[9 + e], q2 = dr[18 + e];
-                                E[0] += pv[e].x * q0; E[1] += pv[e].x * q1; E[2] += pv[e].x * q2;
-                                E[3] += pv[e].y * q0; E[4] += pv[e].y * q1; E[5] += pv[e].y * q2;
-                                E[6] += pv[e].z * q0; E[7] += pv[e].z * q1; E[8] += pv[e].z * q2;
-                            }
-#pragma unroll
-                            for (int r = 0; r < 3; ++r)
-#pragma unroll
-                                for (int k = 0; k < 3; ++k)
-                                    blk[3 * r + k] = Mt[3 * r] * E[k] + Mt[3 * r + 1] * E[3 + k] + Mt[3 * r + 2] * E[6 + k];
-                        }
-                        const int mask = mrow[a];
-                        if (mask) {                                  // rigid part: u_{a,k} x q
-                            real q[3] = {0, 0, 0};
-#if 1
-                            if (d.kw == 4) {
-                                // four skinning joints per slot (every released model): weights and joint-relative positions
-                                // of the slot as four 16-byte vectors, the subtree mask applied to the weights -- no branches
-                                const Vec4<real> wv = ld4(w.c_wv + 4 * sl);
-                                const real *pp = w.pj + 12 * sl;
-                                const Vec4<real> a0 = ld4(pp), a1 = ld4(pp + 4), a2 = ld4(pp + 8);
-                                const real g0 = w.tg[3 * a], g1 = w.tg[3 * a + 1], g2 = w.tg[3 * a + 2];
-                                const real w0 = (mask & 1) ? wv.x : real(0), w1 = (mask & 2) ? wv.y : real(0);
-                                const real w2 = (mask & 4) ? wv.z : real(0), w3 = (mask & 8) ? wv.w : real(0);
-                                q[0] = w0 * (a0.x - g0); q[1] = w0 * (a0.y - g1); q[2] = w0 * (a0.z - g2);
-                                q[0] += w1 * (a0.w - g0); q[1] += w1 * (a1.x - g1); q[2] += w1 * (a1.y - g2);
-                                q[0] += w2 * (a1.z - g0); q[1] += w2 * (a1.w - g1); q[2] += w2 * (a2.x - g2);
-                                q[0] += w3 * (a2.y - g0); q[1] += w3 * (a2.z - g1); q[2] += w3 * (a2.w - g2);
-                            } else
-#endif
-                            for (int i = 0; i < d.kw; ++i)
-                                if ((mask >> i) & 1) {
-                                    const real wt = w.c_wv[sl * d.kw + i];
-                                    const real *pp = w.pj + 3 * (sl * d.kw + i);
-                                    for (int r = 0; r < 3; ++r) q[r] += wt * (pp[r] - w.tg[3 * a + r]);
-                                }
-#pragma unroll
-                            for (int k = 0; k < 3; ++k) {
-                                const Vec4<real> uk = ld4(w.u + kM3 * a + 4 * k);
-                                const real uv[3] = {uk.x, uk.y, uk.z};
-                                real cr[3];
-                                cross3(uv, q, cr);
-#pragma unroll
-                                for (int r = 0; r < 3; ++r) blk[3 * r + k] += Lc[3 * r] * cr[0] + Lc[3 * r + 1] * cr[1] + Lc[3 * r + 2] * cr[2];
-                            }
-                        }
-                        // lane t collects column t of the marker's block: own part + the parts of the two other vertices
-                        real col3[3];
-#pragma unroll
-                        for (int r = 0; r < 3; ++r) {
-                            const real b0 = blk[3 * r], b1 = blk[3 * r + 1], b2 = blk[3 * r + 2];
-#if 1
-                            // (two selects each; written as nested conditionals the compiler turned them into three divergent
-                            // branches per row -- every warp holds all three values of t)
-                            const real own = sel3(t, b0, b1, b2);
-                            const real to1 = sel3(t, b1, b2, b0);
-                            const real to2 = sel3(t, b2, b0, b1);
-#else
-                            const real own = t == 0 ? b0 : (t == 1 ? b1 : b2);
-                            const real to1 = t == 0 ? b1 : (t == 1 ? b2 : b0);   // what the lane with t+1 wants: column t+1
-                            const real to2 = t == 0 ? b2 : (t == 1 ? b0 : b1);   // column t+2
-#endif
-                            col3[r] = own + __shfl_sync(0xffffffffu, to1, src1) + __shfl_sync(0xffffffffu, to2, src2);
-                        }
-                        if (valid) {
-                            if (3 * a < m.body_dof) {
-                                const int col = w.colmap[3 + 3 * a + t];
-                                if (col >= 0) jf_store3(ml, col, col3[0] * sc, col3[1] * sc, col3[2] * sc);
-                            } else {
-                                real *Jr = w.Jt + 3 * ml * d.NCt + (3 * a - m.body_dof) + t;
-                                Jr[0] = col3[0]; Jr[d.NCt] = col3[1]; Jr[2 * d.NCt] = col3[2];
-                            }
-                        }
-                    }
+                for (int r = 0; r < 3; ++r) {
+                    const real b0 = blk[3 * r], b1 = blk[3 * r + 1], b2 = blk[3 * r + 2];
+                    // (two selects each; written as nested conditionals the compiler turned them into three divergent
+                    // branches per row -- every warp holds all three values of t)
+                    const real own = sel3(t, b0, b1, b2);
+                    const real to1 = sel3(t, b1, b2, b0);
+                    const real to2 = sel3(t, b2, b0, b1);
+                    col3[r] = own + __shfl_sync(0xffffffffu, to1, src1) + __shfl_sync(0xffffffffu, to2, src2);
                 }
-#else
-                const int ngroups = tm * njl;
-                for (int gi = 0; gi < ngroups; ++gi) {
-                    const int ml = gi % tm, a = w.jlist[gi / tm];
-                    real blk[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-                    for (int t = 0; t < 3; ++t) {
-                        real part[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-                        real pv[27];
-                        t1_load(t0 + ml, a, t, pv);
-                        t1_compute(t0 + ml, a, t, pv, part);
-                        for (int q = 0; q < 9; ++q) blk[q] += part[q];
-                    }
-                    t1_store(ml, t0 + ml, a, blk);
-                }
-#endif
+                if (valid) pose_col_store(ml, a, t, sc, col3[0], col3[1], col3[2]);
             }
-            CTA_FOR(it, tm * d.nd) {
-                const int ml = it / d.nd, i = it - ml * d.nd, mi = t0 + ml;
-                real val[3] = {0, 0, 0};
-                real sdv[9];                              // the nine (L2) loads of the item, issued together
-#pragma unroll
-                for (int u = 0; u < 9; ++u) sdv[u] = m.sd[(9 * mi + u) * d.nd + i];
-                for (int t = 0; t < 3; ++t) {
-                    const int s = 3 * mi + t;
-                    real dv[3] = {0, 0, 0};
-                    for (int kk = 0; kk < d.kw; ++kk) {
-                        const int j = w.c_wj[s * d.kw + kk];
-                        if (j < 0) continue;
-                        const real wt = w.c_wv[s * d.kw + kk];
-                        real df[3], o[3];
-                        for (int r = 0; r < 3; ++r) df[r] = sdv[3 * t + r] - w.c_jd[(3 * j + r) * d.nd + i];
-                        mat3_vec(w.Rg + 9 * j, df, o);
-                        for (int r = 0; r < 3; ++r) dv[r] += wt * (o[r] + w.dtg[3 * (j * d.nd + i) + r]);
-                    }
-                    const real *L = w.Loc + kM3 * s;
-                    for (int r = 0; r < 3; ++r) val[r] += L[3 * r] * dv[0] + L[3 * r + 1] * dv[1] + L[3 * r + 2] * dv[2];
-                }
-                const int col = w.colmap[3 + d.PR + i];
-                const real sc = w.vis[mi] ? wd : real(0);
-                if (col >= 0) jf_store3(ml, col, val[0] * sc, val[1] * sc, val[2] * sc);
-            }
-            // translation columns (identity); zero padding of the tile
-            const int trows = 3 * tm;
-            CTA_FOR(idx, tm * 3) {
-                const int ml = idx / 3, q = idx - 3 * ml, col = w.colmap[q];
-                const real v = w.vis[t0 + ml] ? wd : real(0);
-                if (col >= 0) jf_store3(ml, col, q == 0 ? v : real(0), q == 1 ? v : real(0), q == 2 ? v : real(0));
-            }
-            {
-                const int npadc = d.npad - n;
-                CTA_FOR(idx, trows * npadc) w.Jf[(idx / npadc) * d.npad + n + idx % npadc] = 0;
-            }
-            M2_SYNC();
-            M2_TACC(7);
-            // T2b: hand columns = Jt[:, hand block] * C^T as a register-tiled product (one marker's 3 rows x 4 outputs)
-            if (hand_free) {
-                int ngt = 0;                                  // output groups of 4 over all blocks
-                for (int b = 0; b < m.hb_n; ++b) ngt += m.hb[b].rw4 / 4;
-                CTA_FOR(it, tm * ngt) {
-                    const int ml = it / ngt;
-                    int rg = it - ml * ngt, b = 0;
-                    while (rg >= m.hb[b].rw4 / 4) { rg -= m.hb[b].rw4 / 4; ++b; }
-                    const HandBlock hb = m.hb[b];
-                    const int nq = hb.q1 - hb.q0;
-                    const real *J0 = w.Jt + 3 * ml * d.NCt + hb.q0, *J1 = J0 + d.NCt, *J2 = J1 + d.NCt;
-                    const real *ct = w.hct + hb.ct_off + 4 * rg;
-                    real acc[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-                    // (global-workspace layout: the full-pose tile lives in L2 -- five columns in flight; same order of the sums)
-                    constexpr int U = BIG ? 5 : 1;
-                    for (int q = 0; q < nq; q += U) {
-                        real j0[U], j1[U], j2[U];
-                        Vec4<real> cv[U];
-#pragma unroll
-                        for (int u = 0; u < U; ++u) {
-                            const int qq = q + u < nq ? q + u : nq - 1;
-                            j0[u] = J0[qq]; j1[u] = J1[qq]; j2[u] = J2[qq];
-                            cv[u] = ld4(ct + qq * hb.rw4);
-                        }
-#pragma unroll
-                        for (int u = 0; u < U; ++u)
-                            if (q + u < nq) {
-                                acc[0] += j0[u] * cv[u].x; acc[1] += j0[u] * cv[u].y; acc[2] += j0[u] * cv[u].z; acc[3] += j0[u] * cv[u].w;
-                                acc[4] += j1[u] * cv[u].x; acc[5] += j1[u] * cv[u].y; acc[6] += j1[u] * cv[u].z; acc[7] += j1[u] * cv[u].w;
-                                acc[8] += j2[u] * cv[u].x; acc[9] += j2[u] * cv[u].y; acc[10] += j2[u] * cv[u].z; acc[11] += j2[u] * cv[u].w;
-                            }
-                    }
-                    const real sc = w.vis[t0 + ml] ? wd : real(0);
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const int r = hb.r0 + 4 * rg + e;
-                        if (r < hb.r1) {
-                            const int col = w.colmap[3 + m.body_dof + r];
-                            if (col >= 0) jf_store3(ml, col, acc[e] * sc, acc[4 + e] * sc, acc[8 + e] * sc);
-                        }
-                    }
-                }
-            }
-            M2_SYNC();
-            M2_TACC(8);
-            if (lin_f >= 0 && job.lin_J) {       // linearise mode: the finished rows of the tile go out as they are
-                real *Jo = job.lin_J + (size_t(lin_f) * 3 * d.M + 3 * t0) * n;
-                CTA_FOR(idx, trows * n) { const int row = idx / n, cc = idx - row * n; Jo[idx] = w.Jf[row * d.npad + cc]; }
-            }
-            // T3: A += Jf^T Jf, g -= Jf^T r
-#if M2_GPU
-            if constexpr (sizeof(real) == 8) {
-                // float64: J^T J on the tensor cores as well -- mma.sync m8n8k4 (DMMA), a warp per 16x16 block of the upper
-                // triangle, K = the tile's rows in steps of four.  The FP64 pipe of the CUDA cores issues one warp
-                // instruction per ~25 cycles and SM sub-partition here: the register-tile product below took half of the
-                // float64 kernel's time (measured; 8x8 register tiles, i.e. half the operand bytes, took twice as long).
-                const int lane = cta.tid & 31, warp = cta.tid >> 5, nwarp = cta.nthr >> 5;
-                const int g = lane >> 2, tq = lane & 3;
-                const int nb16 = (n + 15) >> 4, ntile = nb16 * (nb16 + 1) / 2;
-                for (int tile = warp; tile < ntile; tile += nwarp) {
-                    int ti = 0, rem = tile;
-                    while (rem >= nb16 - ti) { rem -= nb16 - ti; ++ti; }
-                    const int tj = ti + rem, i0 = 16 * ti, j0 = 16 * tj;
-                    double c[2][2][2] = {{{0, 0}, {0, 0}}, {{0, 0}, {0, 0}}};
-                    // operand columns of this lane (beyond the padded row length: nothing to read)
-                    const int ca0 = i0 + g, ca1 = i0 + 8 + g, cb0 = j0 + g, cb1 = j0 + 8 + g;
-                    for (int k0 = 0; k0 < trows; k0 += 4) {
-                        const int k = k0 + tq;
-                        const bool kin = k < trows;
-                        const real *Jr = w.Jf + (kin ? k : 0) * d.npad;
-                        const double a0 = (kin && ca0 < d.npad) ? double(Jr[ca0]) : 0.0, a1 = (kin && ca1 < d.npad) ? double(Jr[ca1]) : 0.0;
-                        const double b0 = (kin && cb0 < d.npad) ? double(Jr[cb0]) : 0.0, b1 = (kin && cb1 < d.npad) ? double(Jr[cb1]) : 0.0;
-                        dmma_m8n8k4(c[0][0][0], c[0][0][1], a0, b0);
-                        dmma_m8n8k4(c[0][1][0], c[0][1][1], a0, b1);
-                        dmma_m8n8k4(c[1][0][0], c[1][0][1], a1, b0);
-                        dmma_m8n8k4(c[1][1][0], c[1][1][1], a1, b1);
-                    }
-                    // A += block, mirrored.  The old values are fetched together (in the global-workspace layout A lives in L2,
-                    // and sixteen read-modify-writes one after the other cost a launch's worth of latency per tile: that, not the
-                    // product, was the phase); the mirror entry receives the same sum -- it has received the same terms.
-                    real old[2][2][2];
-#pragma unroll
-                    for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-                        for (int ni = 0; ni < 2; ++ni)
-#pragma unroll
-                            for (int e = 0; e < 2; ++e) {
-                                const int i = i0 + 8 * mi + g, j = j0 + 8 * ni + 2 * tq + e;
-                                old[mi][ni][e] = (j < n && i <= j) ? w.A[i * ld + j] : real(0);
-                            }
-#pragma unroll
-                    for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-                        for (int ni = 0; ni < 2; ++ni)
-#pragma unroll
-                            for (int e = 0; e < 2; ++e) {
-                                const int i = i0 + 8 * mi + g, j = j0 + 8 * ni + 2 * tq + e;
-                                if (j < n && i <= j) {
-                                    const real v = old[mi][ni][e] + real(c[mi][ni][e]);
-                                    w.A[i * ld + j] = v;
-                                    if (i < j) w.A[j * ld + i] = v;
-                                }
-                            }
-                }
-            } else if (w.tc) {
-                // float32: split TF32 on the tensor cores (tc::jtj_block_tf32), a warp per 16x16 block of the upper
-                // triangle; A += (hi hi^T + cross terms), mirrored like the float64 blocks above
-                const int lane = cta.tid & 31, warp = cta.tid >> 5, nwarp = cta.nthr >> 5;
-                const int g = lane >> 2, tq = lane & 3;
-                const int nb16 = (n + 15) >> 4, ntile = nb16 * (nb16 + 1) / 2;
-                for (int tile = warp; tile < ntile; tile += nwarp) {
-                    int ti = 0, rem = tile;
-                    while (rem >= nb16 - ti) { rem -= nb16 - ti; ++ti; }
-                    const int tj = ti + rem, i0 = 16 * ti, j0 = 16 * tj;
-                    float hh[2][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}}, cr[2][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}};
-                    tc::jtj_block_tf32(w.Jf, d.npad, trows, d.npad, i0, j0, hh, cr);
-                    real old[2][2][2];
-#pragma unroll
-                    for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-                        for (int ni = 0; ni < 2; ++ni)
-#pragma unroll
-                            for (int e = 0; e < 2; ++e) {
-                                const int i = i0 + 8 * mi + g, j = j0 + 8 * ni + 2 * tq + e;
-                                old[mi][ni][e] = (j < n && i <= j) ? w.A[i * ld + j] : real(0);
-                            }
-#pragma unroll
-                    for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-                        for (int ni = 0; ni < 2; ++ni)
-#pragma unroll
-                            for (int e = 0; e < 2; ++e) {
-                                const int i = i0 + 8 * mi + g, j = j0 + 8 * ni + 2 * tq + e;
-                                if (j < n && i <= j) {
-                                    const real v = old[mi][ni][e] + (hh[ni][2 * mi + e] + cr[ni][2 * mi + e]);
-                                    w.A[i * ld + j] = v;
-                                    if (i < j) w.A[j * ld + i] = v;
-                                }
-                            }
-                }
-            } else
-#endif
-            {
-                const int nb = (n + kBS - 1) / kBS, nblk = nb * (nb + 1) / 2;
-                CTA_FOR(b, nblk) {
-                    int bi = 0, rem = b;
-                    while (rem >= nb - bi) { rem -= nb - bi; ++bi; }
-                    const int bj = bi + rem;
-                    real acc[kBS * kBS];
-#pragma unroll
-                    for (int q = 0; q < kBS * kBS; ++q) acc[q] = 0;
-                    // four rows in flight: in the float64 / oversized layout the tile lives in the global workspace (L2), and a
-                    // loop that waits for every row's two loads before its sixteen FMAs ran at a fourteenth of the FP64 rate
-                    // (half of the float64 kernel's time).  Same products in the same order.
-                    for (int row = 0; row < trows; row += 4) {
-                        Vec4<real> av[4], bv[4];
-#pragma unroll
-                        for (int u = 0; u < 4; ++u) {
-                            const real *Jr = w.Jf + (row + u < trows ? row + u : trows - 1) * d.npad;
-                            av[u] = ld4(Jr + bi * kBS);
-                            bv[u] = ld4(Jr + bj * kBS);
-                        }
-#pragma unroll
-                        for (int u = 0; u < 4; ++u)
-                            if (row + u < trows) {
-                                const real ai[4] = {av[u].x, av[u].y, av[u].z, av[u].w}, bjv[4] = {bv[u].x, bv[u].y, bv[u].z, bv[u].w};
-#pragma unroll
-                                for (int p = 0; p < kBS; ++p)
-#pragma unroll
-                                    for (int q = 0; q < kBS; ++q) acc[p * kBS + q] += ai[p] * bjv[q];
-                            }
-                    }
-#pragma unroll
-                    for (int p = 0; p < kBS; ++p)
-#pragma unroll
-                        for (int q = 0; q < kBS; ++q) {
-                            const int i = bi * kBS + p, j = bj * kBS + q;
-                            if (j < n && i <= j) {
-                                w.A[i * ld + j] += acc[p * kBS + q];
-                                if (i < j) w.A[j * ld + i] += acc[p * kBS + q];
-                            }
-                        }
-                }
-            }
-            CTA_FOR(cc, n) {                                 // (six rows in flight, for the same reason; same order of the sum)
-                real s = 0;
-                for (int row = 0; row < trows; row += 6) {
-                    real jv[6];
-#pragma unroll
-                    for (int u = 0; u < 6; ++u) jv[u] = w.Jf[(row + u < trows ? row + u : trows - 1) * d.npad + cc];
-#pragma unroll
-                    for (int u = 0; u < 6; ++u) if (row + u < trows) s += jv[u] * w.rm[3 * t0 + row + u];
-                }
-                w.g[cc] -= s;
-            }
-            M2_SYNC();
-            M2_TACC(9);
         }
-        // closed-form terms
+#else
+        for (int gi = 0; gi < tm * njl; ++gi) {
+            const int ml = gi % tm, a = w.jlist[gi / tm], mi = t0 + ml;
+            real blk[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+            for (int t = 0; t < 3; ++t) {
+                const int sl = 3 * mi + t;
+                real Mt[9], Lc[9], part[9];
+                slot_mats(sl, Mt, Lc);
+                slot_pose_block(sl, a, Mt, Lc, m.pd4 + size_t(sl) * 4, part);
+                for (int q = 0; q < 9; ++q) blk[q] += part[q];
+            }
+            const real sc = w.vis[mi] ? wd : real(0);
+            for (int k = 0; k < 3; ++k) pose_col_store(ml, a, k, sc, blk[k], blk[3 + k], blk[6 + k]);
+        }
+#endif
+    }
+
+    // ---- linear-block (DMPL / expression) columns of the tile, from the vertex directions `sd` and the joint-position
+    //      derivatives of dtg_chains()
+    M2_D void tile_linear_columns(int t0, int tm) {
+        CTA_FOR(it, tm * d.nd) {
+            const int ml = it / d.nd, i = it - ml * d.nd, mi = t0 + ml;
+            real val[3] = {0, 0, 0};
+            real sdv[9];                              // the nine (L2) loads of the item, issued together
+#pragma unroll
+            for (int u = 0; u < 9; ++u) sdv[u] = m.sd[(9 * mi + u) * d.nd + i];
+            for (int t = 0; t < 3; ++t) {
+                const int s = 3 * mi + t;
+                real dv[3] = {0, 0, 0};
+                for (int kk = 0; kk < d.kw; ++kk) {
+                    const int j = w.c_wj[s * d.kw + kk];
+                    if (j < 0) continue;
+                    const real wt = w.c_wv[s * d.kw + kk];
+                    real df[3], o[3];
+                    for (int r = 0; r < 3; ++r) df[r] = sdv[3 * t + r] - w.c_jd[(3 * j + r) * d.nd + i];
+                    mat3_vec(w.Rg + 9 * j, df, o);
+                    for (int r = 0; r < 3; ++r) dv[r] += wt * (o[r] + w.dtg[3 * (j * d.nd + i) + r]);
+                }
+                const real *L = w.Loc + kM3 * s;
+                for (int r = 0; r < 3; ++r) val[r] += L[3 * r] * dv[0] + L[3 * r + 1] * dv[1] + L[3 * r + 2] * dv[2];
+            }
+            const int col = w.colmap[3 + d.PR + i];
+            const real sc = w.vis[mi] ? wd : real(0);
+            if (col >= 0) jf_store3(ml, col, val[0] * sc, val[1] * sc, val[2] * sc);
+        }
+    }
+
+    // ---- translation columns of the tile (identity) and the zero padding of its rows beyond the n free columns
+    M2_D void tile_translation_columns(int t0, int tm, int n) {
+        CTA_FOR(idx, tm * 3) {
+            const int ml = idx / 3, q = idx - 3 * ml, col = w.colmap[q];
+            const real v = w.vis[t0 + ml] ? wd : real(0);
+            if (col >= 0) jf_store3(ml, col, q == 0 ? v : real(0), q == 1 ? v : real(0), q == 2 ? v : real(0));
+        }
+        const int npadc = d.npad - n;
+        CTA_FOR(idx, 3 * tm * npadc) w.Jf[(idx / npadc) * d.npad + n + idx % npadc] = 0;
+    }
+
+    // ---- T2b: hand columns = Jt[:, hand block] * C^T as a register-tiled product (one marker's 3 rows x 4 outputs)
+    M2_D void tile_hand_columns(int t0, int tm) {
+        if (!hand_free) return;
+        int ngt = 0;                                  // output groups of 4 over all blocks
+        for (int b = 0; b < m.hb_n; ++b) ngt += m.hb[b].rw4 / 4;
+        CTA_FOR(it, tm * ngt) {
+            const int ml = it / ngt;
+            int rg = it - ml * ngt, b = 0;
+            while (rg >= m.hb[b].rw4 / 4) { rg -= m.hb[b].rw4 / 4; ++b; }
+            const HandBlock hb = m.hb[b];
+            const int nq = hb.q1 - hb.q0;
+            const real *J0 = w.Jt + 3 * ml * d.NCt + hb.q0, *J1 = J0 + d.NCt, *J2 = J1 + d.NCt;
+            const real *ct = w.hct + hb.ct_off + 4 * rg;
+            real acc[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+            // (global-workspace layout: the full-pose tile lives in L2 -- five columns in flight; same order of the sums)
+            constexpr int U = BIG ? 5 : 1;
+            for (int q = 0; q < nq; q += U) {
+                real j0[U], j1[U], j2[U];
+                Vec4<real> cv[U];
+#pragma unroll
+                for (int u = 0; u < U; ++u) {
+                    const int qq = q + u < nq ? q + u : nq - 1;
+                    j0[u] = J0[qq]; j1[u] = J1[qq]; j2[u] = J2[qq];
+                    cv[u] = ld4(ct + qq * hb.rw4);
+                }
+#pragma unroll
+                for (int u = 0; u < U; ++u)
+                    if (q + u < nq) {
+                        acc[0] += j0[u] * cv[u].x; acc[1] += j0[u] * cv[u].y; acc[2] += j0[u] * cv[u].z; acc[3] += j0[u] * cv[u].w;
+                        acc[4] += j1[u] * cv[u].x; acc[5] += j1[u] * cv[u].y; acc[6] += j1[u] * cv[u].z; acc[7] += j1[u] * cv[u].w;
+                        acc[8] += j2[u] * cv[u].x; acc[9] += j2[u] * cv[u].y; acc[10] += j2[u] * cv[u].z; acc[11] += j2[u] * cv[u].w;
+                    }
+            }
+            const real sc = w.vis[t0 + ml] ? wd : real(0);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int r = hb.r0 + 4 * rg + e;
+                if (r < hb.r1) {
+                    const int col = w.colmap[3 + m.body_dof + r];
+                    if (col >= 0) jf_store3(ml, col, acc[e] * sc, acc[4 + e] * sc, acc[8 + e] * sc);
+                }
+            }
+        }
+    }
+
+#if M2_GPU
+    // ---- A += the 16x16 block at (i0, j0) of the upper triangle that the calling warp holds in the layout of the mma
+    //      accumulators: c[mi][ni][e] is entry (i0 + 8 mi + g, j0 + 8 ni + 2 tq + e), g = lane / 4, tq = lane % 4.  The old
+    //      values are fetched together (in the global-workspace layout A lives in L2, and sixteen read-modify-writes one
+    //      after the other cost a launch's worth of latency per tile: that, not the product, was the phase); the mirror
+    //      entry receives the same sum -- it has received the same terms.
+    M2_D void add_upper_block16(int i0, int j0, int n, const real (&c)[2][2][2]) {
+        const int lane = cta.tid & 31, g = lane >> 2, tq = lane & 3, ld = d.lda;
+        real old[2][2][2];
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+            for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int i = i0 + 8 * mi + g, j = j0 + 8 * ni + 2 * tq + e;
+                    old[mi][ni][e] = (j < n && i <= j) ? w.A[i * ld + j] : real(0);
+                }
+#pragma unroll
+        for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+            for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int i = i0 + 8 * mi + g, j = j0 + 8 * ni + 2 * tq + e;
+                    if (j < n && i <= j) {
+                        const real v = old[mi][ni][e] + c[mi][ni][e];
+                        w.A[i * ld + j] = v;
+                        if (i < j) w.A[j * ld + i] = v;
+                    }
+                }
+    }
+#endif
+
+    // ---- T3: A += Jf^T Jf, g -= Jf^T r over the tile's rows; in linearise mode the finished rows go out first, as they are
+    M2_D void tile_normal_equations(int t0, int tm, int n) {
+        const int trows = 3 * tm, ld = d.lda;
+        if (lin_f >= 0 && job.lin_J) {
+            real *Jo = job.lin_J + (size_t(lin_f) * 3 * d.M + 3 * t0) * n;
+            CTA_FOR(idx, trows * n) { const int row = idx / n, cc = idx - row * n; Jo[idx] = w.Jf[row * d.npad + cc]; }
+        }
+#if M2_GPU
+        if constexpr (sizeof(real) == 8) {
+            // float64: J^T J on the tensor cores as well -- mma.sync m8n8k4 (DMMA), a warp per 16x16 block of the upper
+            // triangle, K = the tile's rows in steps of four.  The FP64 pipe of the CUDA cores issues one warp
+            // instruction per ~25 cycles and SM sub-partition here: the register-tile product below took half of the
+            // float64 kernel's time (measured; 8x8 register tiles, i.e. half the operand bytes, took twice as long).
+            const int lane = cta.tid & 31, warp = cta.tid >> 5, nwarp = cta.nthr >> 5;
+            const int g = lane >> 2, tq = lane & 3;
+            const int nb16 = (n + 15) >> 4, ntile = nb16 * (nb16 + 1) / 2;
+            for (int tile = warp; tile < ntile; tile += nwarp) {
+                int ti, tj;
+                upper_block(tile, nb16, ti, tj);
+                const int i0 = 16 * ti, j0 = 16 * tj;
+                double c[2][2][2] = {{{0, 0}, {0, 0}}, {{0, 0}, {0, 0}}};
+                // operand columns of this lane (beyond the padded row length: nothing to read)
+                const int ca0 = i0 + g, ca1 = i0 + 8 + g, cb0 = j0 + g, cb1 = j0 + 8 + g;
+                for (int k0 = 0; k0 < trows; k0 += 4) {
+                    const int k = k0 + tq;
+                    const bool kin = k < trows;
+                    const real *Jr = w.Jf + (kin ? k : 0) * d.npad;
+                    const double a0 = (kin && ca0 < d.npad) ? double(Jr[ca0]) : 0.0, a1 = (kin && ca1 < d.npad) ? double(Jr[ca1]) : 0.0;
+                    const double b0 = (kin && cb0 < d.npad) ? double(Jr[cb0]) : 0.0, b1 = (kin && cb1 < d.npad) ? double(Jr[cb1]) : 0.0;
+                    dmma_m8n8k4(c[0][0][0], c[0][0][1], a0, b0);
+                    dmma_m8n8k4(c[0][1][0], c[0][1][1], a0, b1);
+                    dmma_m8n8k4(c[1][0][0], c[1][0][1], a1, b0);
+                    dmma_m8n8k4(c[1][1][0], c[1][1][1], a1, b1);
+                }
+                add_upper_block16(i0, j0, n, c);
+            }
+        } else if (w.tc) {
+            // float32: split TF32 on the tensor cores (tc::jtj_block_tf32), a warp per 16x16 block of the upper
+            // triangle; A += (hi hi^T + cross terms)
+            const int warp = cta.tid >> 5, nwarp = cta.nthr >> 5;
+            const int nb16 = (n + 15) >> 4, ntile = nb16 * (nb16 + 1) / 2;
+            for (int tile = warp; tile < ntile; tile += nwarp) {
+                int ti, tj;
+                upper_block(tile, nb16, ti, tj);
+                const int i0 = 16 * ti, j0 = 16 * tj;
+                float hh[2][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}}, cr[2][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}};
+                tc::jtj_block_tf32(w.Jf, d.npad, trows, d.npad, i0, j0, hh, cr);
+                real c[2][2][2];
+#pragma unroll
+                for (int mi = 0; mi < 2; ++mi)
+#pragma unroll
+                    for (int ni = 0; ni < 2; ++ni)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) c[mi][ni][e] = hh[ni][2 * mi + e] + cr[ni][2 * mi + e];
+                add_upper_block16(i0, j0, n, c);
+            }
+        } else
+#endif
+        {
+            const int nb = (n + kBS - 1) / kBS, nblk = nb * (nb + 1) / 2;
+            CTA_FOR(b, nblk) {
+                int bi, bj;
+                upper_block(b, nb, bi, bj);
+                real acc[kBS * kBS];
+#pragma unroll
+                for (int q = 0; q < kBS * kBS; ++q) acc[q] = 0;
+                // four rows in flight: in the float64 / oversized layout the tile lives in the global workspace (L2), and a
+                // loop that waits for every row's two loads before its sixteen FMAs ran at a fourteenth of the FP64 rate
+                // (half of the float64 kernel's time).  Same products in the same order.
+                for (int row = 0; row < trows; row += 4) {
+                    Vec4<real> av[4], bv[4];
+#pragma unroll
+                    for (int u = 0; u < 4; ++u) {
+                        const real *Jr = w.Jf + (row + u < trows ? row + u : trows - 1) * d.npad;
+                        av[u] = ld4(Jr + bi * kBS);
+                        bv[u] = ld4(Jr + bj * kBS);
+                    }
+#pragma unroll
+                    for (int u = 0; u < 4; ++u)
+                        if (row + u < trows) {
+                            const real ai[4] = {av[u].x, av[u].y, av[u].z, av[u].w}, bjv[4] = {bv[u].x, bv[u].y, bv[u].z, bv[u].w};
+#pragma unroll
+                            for (int p = 0; p < kBS; ++p)
+#pragma unroll
+                                for (int q = 0; q < kBS; ++q) acc[p * kBS + q] += ai[p] * bjv[q];
+                        }
+                }
+#pragma unroll
+                for (int p = 0; p < kBS; ++p)
+#pragma unroll
+                    for (int q = 0; q < kBS; ++q) {
+                        const int i = bi * kBS + p, j = bj * kBS + q;
+                        if (j < n && i <= j) {
+                            w.A[i * ld + j] += acc[p * kBS + q];
+                            if (i < j) w.A[j * ld + i] += acc[p * kBS + q];
+                        }
+                    }
+            }
+        }
+        CTA_FOR(cc, n) {                                 // (six rows in flight, for the same reason; same order of the sum)
+            real s = 0;
+            for (int row = 0; row < trows; row += 6) {
+                real jv[6];
+#pragma unroll
+                for (int u = 0; u < 6; ++u) jv[u] = w.Jf[(row + u < trows ? row + u : trows - 1) * d.npad + cc];
+#pragma unroll
+                for (int u = 0; u < 6; ++u) if (row + u < trows) s += jv[u] * w.rm[3 * t0 + row + u];
+            }
+            w.g[cc] -= s;
+        }
+    }
+
+    // ---- closed-form terms at state xs: the prior block, the diagonals of the velocity, finger, face and linear-block
+    //      terms, the joint angles of the horse model
+    M2_D void closed_form_terms(const real *xs, const StepCfg<real> &c) {
+        const real *th = xs + 3;
+        const real *dl = xs + 3 + d.PR;
+        const int n = c.n, ld = d.lda;
         if (c.wp > real(0)) {
             const int D = d.D, ks = w.isc[0];
             const real w2 = c.wp * c.wp;
@@ -1623,6 +1547,38 @@ struct Solver {
                 }
             }
         }
+    }
+
+    // ---- normal equations at the state of the latest eval():  A = J^T J (full symmetric), g = -J^T r, built marker tile by
+    //      marker tile (DESIGN.md, "Per linearisation")
+    M2_D void build(const real *xs, const StepCfg<real> &c) {
+        ++n_build;
+        M2_T0();
+        const int n = c.n;
+        joint_axes();
+        CTA_FOR(mi, d.M) marker_local_jacobian(mi);
+        CTA_FOR(i, n * d.lda) w.A[i] = 0;
+        CTA_FOR(i, n) w.g[i] = 0;
+        dtg_chains();
+        M2_SYNC();
+        CTA_FOR(s, d.S) mat3_mul(w.Loc + kM3 * s, w.Rsk + 9 * s, w.MtR + kM3 * s);
+        M2_SYNC();
+        M2_TACC(6);
+        for (int t0 = 0; t0 < d.M; t0 += d.tmk) {
+            const int tm = (d.M - t0 < d.tmk) ? d.M - t0 : d.tmk;
+            tile_pose_columns(t0, tm);
+            tile_linear_columns(t0, tm);
+            tile_translation_columns(t0, tm, n);
+            M2_SYNC();
+            M2_TACC(7);
+            tile_hand_columns(t0, tm);
+            M2_SYNC();
+            M2_TACC(8);
+            tile_normal_equations(t0, tm, n);
+            M2_SYNC();
+            M2_TACC(9);
+        }
+        closed_form_terms(xs, c);
         M2_SYNC();
         M2_TACC(10);
     }

@@ -27,9 +27,9 @@ __global__ void __launch_bounds__(384, 1) jtj_kernel(const float *J, int rows, i
         }
         __syncthreads();
         for (int t = warp; t < ntile; t += nwarp) {
-            int ti = 0, rem = t;
-            while (rem >= nb16 - ti) { rem -= nb16 - ti; ++ti; }
-            const int i0 = 16 * ti, j0 = 16 * (ti + rem);
+            int ti, tj;
+            mosh2::upper_block(t, nb16, ti, tj);
+            const int i0 = 16 * ti, j0 = 16 * tj;
             float hh[2][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}}, cr[2][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}};
             mosh2::tc::jtj_block_tf32(tile, npad, tr, npad, i0, j0, hh, cr);
             for (int mi = 0; mi < 2; ++mi)

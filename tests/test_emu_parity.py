@@ -3,6 +3,8 @@
 This validates index math and control flow of the exact code nvcc compiles; the numbers that count are
 the `-m gpu` twins in test_gpu_parity.py, which call the CUDA library through the C-ABI.
 """
+import dataclasses
+
 import numpy as np
 import pytest
 
@@ -10,9 +12,16 @@ from conftest import run_oracle
 from moshpp_b200 import lib
 
 
-@pytest.mark.parametrize('name', ['C1', 'C2', 'C3', 'C4', 'CF', 'CH'])
+@pytest.mark.parametrize('name', ['C1', 'C2', 'C3', 'C4', 'CF', 'CH', 'C2-kw5'])
 def test_f64_device_source_equals_oracle(cases, emu, name):
-    case = cases(name)
+    case = cases(name.split('-')[0])
+    if name.endswith('-kw5'):
+        # the same model with an empty fifth skinning column (joint -1, weight 0): the Jacobian takes the generic
+        # per-joint skinning loop instead of the four-joint vector path of the released models
+        pk = case['pack']
+        assert pk.kw == 4
+        case = dict(case, pack=dataclasses.replace(pk, kw=5, w_joint=np.pad(pk.w_joint, ((0, 0), (0, 1)), constant_values=-1),
+                                                   w_val=np.pad(pk.w_val, ((0, 0), (0, 1)))))
     out = run_oracle(case)
     res = emu(case, precision=lib.MOSH2_F64)
     dbg = out['stageii_debug_details']
