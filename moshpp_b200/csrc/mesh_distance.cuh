@@ -51,6 +51,37 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t
                  :: "r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 
+// A triangle whose sides are parallel to within 1e-5 rad (|ab x ac|^2 <= 1e-10 |ab|^2 |ac|^2, far above the float32
+// rounding of the cross product) has no plane to speak of: the Voronoi tests below can fall through to the interior
+// with va + vb + vc at round-off level, and the plane distance of such a triangle is 0 / 0.
+__device__ __forceinline__ bool degenerate(const float ab[3], const float ac[3]) {
+    const float n0 = ab[1] * ac[2] - ab[2] * ac[1], n1 = ab[2] * ac[0] - ab[0] * ac[2], n2 = ab[0] * ac[1] - ab[1] * ac[0];
+    const float l2 = (ab[0] * ab[0] + ab[1] * ab[1] + ab[2] * ab[2]) * (ac[0] * ac[0] + ac[1] * ac[1] + ac[2] * ac[2]);
+    return !(n0 * n0 + n1 * n1 + n2 * n2 > 1e-10f * l2);
+}
+
+// squared distance from p to the closest of the three edges of a degenerate triangle, as edge (1..3) or, where the
+// closest point is an end of the edge, vertex (4..6) part
+__device__ __noinline__ float closest_on_edges(const float p[3], const float *__restrict__ tri, int *part) {
+    float best = 3.0e38f;
+    int bp = 4;
+    for (int e = 0; e < 3; ++e) {
+        const float *u = tri + 3 * e, *v = tri + 3 * ((e + 1) % 3);
+        const float uv[3] = {v[0] - u[0], v[1] - u[1], v[2] - u[2]}, up[3] = {p[0] - u[0], p[1] - u[1], p[2] - u[2]};
+        const float l2 = uv[0] * uv[0] + uv[1] * uv[1] + uv[2] * uv[2], t = up[0] * uv[0] + up[1] * uv[1] + up[2] * uv[2];
+        float s;
+        int pt;
+        if (t <= 0.f || !(l2 > 0.f)) { s = 0.f; pt = 4 + e; }
+        else if (t >= l2) { s = 1.f; pt = 4 + (e + 1) % 3; }
+        else { s = t / l2; pt = 1 + e; }
+        float d = 0.f;
+        for (int k = 0; k < 3; ++k) { const float qk = up[k] - s * uv[k]; d += qk * qk; }
+        if (d < best) { best = d; bp = pt; }
+    }
+    *part = bp;
+    return best;
+}
+
 // squared distance from p to triangle (a, b, c) and the part the closest point lies on: 0 interior, 1..3 the edges
 // ab / bc / ca, 4..6 the vertices a / b / c (Voronoi regions of the triangle)
 __device__ __forceinline__ float closest_part(const float p[3], const float *__restrict__ tri, int *part) {
@@ -83,6 +114,8 @@ __device__ __forceinline__ float closest_part(const float p[3], const float *__r
                 const float w = (d4 - d3) / ((d4 - d3) + (d5 - d6));
                 pt = 2;
                 for (int k = 0; k < 3; ++k) q[k] = bp[k] - w * (tri[6 + k] - tri[3 + k]);
+            } else if (degenerate(ab, ac)) {
+                return closest_on_edges(p, tri, part);
             } else {
                 const float den = 1.f / (va + vb + vc), v = vb * den, w = vc * den;
                 pt = 0;

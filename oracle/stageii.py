@@ -330,41 +330,63 @@ class StageIISolver:
         if self.nd:
             self.betas[self.lin_ids] = 0.0
 
+    def frame_terms(self, n_visible: int, velo_target=None, dmpl_target=None):
+        """The objective of one frame (chmosh.py:596-626, 681-699) as a list of [name, payload] terms: the Step-2 list, of
+        which Step 1 minimises the first ``n_step1``.  ``n_visible`` (markers seen in the frame) sets the weights;
+        ``velo_target`` (2 pose[t-1] - pose[t-2]) and ``dmpl_target`` switch the velocity and DMPL-extrapolation terms
+        on.  Returns (terms, n_step1)."""
+        w = self.wts
+        M = self.n_markers
+        n_missing = float(M - n_visible)
+        anneal = 1.0
+        if n_missing > 0:
+            anneal = anneal + (n_missing / M) * w['stageii_wt_annealing']
+        wt_data = w['stageii_wt_data'] * (NUM_TRAIN_MARKERS / n_visible)
+        wt_pose = w['stageii_wt_poseB'] * anneal
+
+        terms = [['data', wt_data]]
+        if len(self.body_ids):
+            terms.append(['poseB', wt_pose])
+            if self.model.model_type == 'animal_horse':
+                terms.append(['poseB_jangles', wt_pose * 2.])                                    # lines 615-617
+        if velo_target is not None:
+            terms.append(['velo', (w['stageii_wt_velo'], velo_target)])                          # line 626
+        n_step1 = len(terms)
+        if self.optimize_fingers:
+            terms.append(['poseH', w['stageii_wt_poseH'] * anneal])
+        if self.optimize_face and len(self.face_ids):
+            terms.append(['poseF', w['stageii_wt_poseF'] * anneal])
+            terms.append(['expr', w['stageii_wt_expr']])
+        if self.optimize_dynamics:
+            if dmpl_target is not None:
+                terms.append(['extrap_dmpl', (6.0, dmpl_target)])                                # line 697 (App. B-1)
+            terms.append(['dmpl', w['stageii_wt_dmpl']])
+        return terms, n_step1
+
     def solve_range(self, obs_frames: List[Optional[Tuple[np.ndarray, np.ndarray]]], emit_from: int = 0,
                     light_until: int = 0, on_frame=None):
         """The frame loop chmosh.py:584-724 over ``obs_frames`` (each ``(vis_idx, obs m x 3)`` or None for a
         frame without visible markers).  Frames before ``emit_from`` are solved but not reported.  Device-schedule
         emulation only (not reference behaviour): frames before ``light_until`` other than the first solved one are
         tracked with a single dog-leg iteration of the Step-2 problem (DESIGN.md section 4)."""
-        w = self.wts
-        M = self.n_markers
         pose_prev = None
-        dmpl_prev = None
         first = True
         out = []
         for fi, fr in enumerate(obs_frames):
             if fr is None:                                                                       # lines 586-588
                 continue
             vis, obs = fr
-            n_missing = float(M - len(vis))
-            anneal = 1.0
-            if n_missing > 0:
-                anneal = anneal + (n_missing / M) * w['stageii_wt_annealing']
-            wt_data = w['stageii_wt_data'] * (NUM_TRAIN_MARKERS / obs.shape[0])
-            wt_pose = w['stageii_wt_poseB'] * anneal
-            wt_poseH = w['stageii_wt_poseH'] * anneal
-            wt_poseF = w['stageii_wt_poseF'] * anneal
-            wt_expr = w['stageii_wt_expr']
-            wt_dmpl = w['stageii_wt_dmpl']
-            wt_velo = w['stageii_wt_velo']
-
-            terms = [['data', wt_data]]
-            if len(self.body_ids):
-                terms.append(['poseB', wt_pose])
-                if self.model.model_type == 'animal_horse':
-                    terms.append(['poseB_jangles', wt_pose * 2.])                                # lines 615-617
-            if pose_prev is not None:
-                terms.append(['velo', (wt_velo, self.pose + (self.pose - pose_prev))])           # line 626
+            velo_target = None if pose_prev is None else self.pose + (self.pose - pose_prev)     # line 626
+            dmpl_target = None
+            if not first:
+                pose_prev = self.pose.copy()                                                     # lines 656-659
+                if self.optimize_dynamics:
+                    # line 697 (App. B-1); Step 1 leaves the coefficients where they are, so the target is known here
+                    dmpl_prev = self.betas[self.dmpl_ids].copy()
+                    cur = self.betas[self.dmpl_ids]
+                    dmpl_target = cur + (cur - dmpl_prev)
+            terms, n_step1 = self.frame_terms(len(vis), velo_target, dmpl_target)
+            step1 = terms[:n_step1]                     # (the same [name, payload] lists: Step 1 sees the schedule below)
 
             was_first = first
             if first:
@@ -372,32 +394,20 @@ class StageIISolver:
                 rv, T = perform_rigid_adjustment(sim, obs)                                       # line 634
                 self.pose[:3] = rv
                 self.trans[:] = T
-                for wt_first in [10. * wt_pose, 5. * wt_pose, wt_pose]:
+                wt_pose = terms[1][1] if len(self.body_ids) else None
+                for scale in (10., 5., 1.):
                     if len(self.body_ids):
+                        wt_first = scale * wt_pose
                         terms[1][1] = wt_first
                         if self.model.model_type == 'animal_horse':
                             terms[2][1] = wt_first * 2.                                          # lines 640-643
-                    self._minimize(_Objective(self, obs, vis, terms, self.step1_ids, False), 1e-3)
+                    self._minimize(_Objective(self, obs, vis, step1, self.step1_ids, False), 1e-3)
                 first = False
-            else:
-                pose_prev = self.pose.copy()                                                     # lines 656-659
-                if self.optimize_dynamics:
-                    dmpl_prev = self.betas[self.dmpl_ids].copy()
 
             light = (not was_first) and fi < light_until
             if not light:
-                self._minimize(_Objective(self, obs, vis, terms, self.step1_ids, False), 1e-2)    # Step 1
+                self._minimize(_Objective(self, obs, vis, step1, self.step1_ids, False), 1e-2)    # Step 1
 
-            if self.optimize_fingers:
-                terms.append(['poseH', wt_poseH])
-            if self.optimize_face and len(self.face_ids):
-                terms.append(['poseF', wt_poseF])
-                terms.append(['expr', wt_expr])
-            if self.optimize_dynamics:
-                if dmpl_prev is not None:
-                    cur = self.betas[self.dmpl_ids]
-                    terms.append(['extrap_dmpl', (6.0, cur + (cur - dmpl_prev))])                # line 697 (App. B-1)
-                terms.append(['dmpl', wt_dmpl])
             obj2 = _Objective(self, obs, vis, terms, self.step2_ids, self.nd > 0)
             self._minimize(obj2, 1e-2, maxiter=1 if light else None)                             # Step 2
 
