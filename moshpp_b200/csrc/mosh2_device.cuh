@@ -2459,8 +2459,9 @@ struct Solver {
         const Options &o = job.opt;
         // Linearise mode (Stage I, Job::lin_mode): the block's "chunk" is the single frame `chunk`, taken at the state the
         // caller gives and left after its first evaluation / linearisation.  The frame's own terms are the Stage-II ones
-        // without the temporal coupling -- data, pose prior (+ joint angles), with lin_step == 2 the finger term -- under
-        // the weights of the options as they are (no per-frame visibility scaling: chmosh.py:327,350).  It runs through the
+        // without the temporal coupling -- data, pose prior (+ joint angles), with lin_step == 2 the finger term and, with
+        // optimize_face, the jaw (poseF) and expression terms -- under the weights of the options as they are (no per-frame
+        // visibility scaling: chmosh.py:327,350; the expression weight is never visibility-scaled).  It runs through the
         // same frame loop and the same solve_frame call as a chunk (one call site each: instruction cache, DESIGN.md 3).
         const bool lin = job.lin_mode != 0;
         // chunk table (host-built, mosh2_host::chunk_table): the chunk emits frames [f_emit, f_end) of the sequence that
@@ -2575,8 +2576,8 @@ struct Solver {
                 if (f >= f_emit && cta.tid == 0) job.status[f] = ST_SKIPPED;
                 continue;
             }
-            real anneal = 1;
-            if (nvis < d.M) anneal += real(d.M - nvis) / real(d.M) * real(o.wt_annealing);
+            real anneal = 1;                                   // (none in linearise mode: wp_frame, wH and wF stay the options')
+            if (nvis < d.M && !lin) anneal += real(d.M - nvis) / real(d.M) * real(o.wt_annealing);
             wd = real(o.wt_data) * (real(o.num_train_markers) / real(nvis));
             wp_frame = has_prior ? real(o.wt_poseB) * anneal : real(0);
             wH = real(o.wt_poseH) * anneal;

@@ -20,6 +20,12 @@ There is no CPU evaluation of the body model per frame: without libmosh2.so or a
 The canonical body ``can_model.r`` (zero reduced pose: with ``use_hands_mean`` the hands are in their mean pose) is an affine
 function of the shape coefficients -- rotations fixed, joints and vertices linear in betas -- so it is expanded once:
 can(betas) = can_0 + C betas[:num_betas] (``CanonicalBody``).
+
+``moshpp.optimize_face`` (SMPL-X with face markers, the shape given and ``optimize_betas`` off; chmosh.py:103-151,283-295):
+every picked frame's model carries the given shape plus its own expressions ``betas[es:es + ne]``; the canonical body keeps
+zero expressions.  The device's linear block then holds the expression directions instead of the shape's, and in the two
+detailed steps the jaw and the expressions are private unknowns of each frame, with the poseF / expr terms.  The expressions
+are returned in the debug details as ``opt_models_expression``.
 """
 from __future__ import annotations
 
@@ -256,6 +262,29 @@ class DeviceBackend:
 # ---------------------------------------------------------------------------------------------------------------------
 # the solver
 # ---------------------------------------------------------------------------------------------------------------------
+def face_flag(cfg, marker_meta, avail_labels) -> bool:
+    """Whether Stage I fits the jaw and the expressions (``moshpp.optimize_face``), by the reference's rules, without changing
+    ``cfg``: off with a free shape when the face markers are excluded (chmosh.py:103-118), off without a face-type marker in the
+    layout or without a face label in the picked frames (chmosh.py:127-137), ignored for models other than SMPL-X (only SMPL-X has
+    a jaw and expression components), and NotImplementedError with a free shape on SMPL-X (chmosh.py:287-291)."""
+    sm, mp = cfg.surface_model, cfg.moshpp
+    if not bool(_get(mp, 'optimize_face', False)):
+        return False
+    free_betas = bool(mp.optimize_betas)
+    if sm.type == 'smplx' and free_betas and 'face' in (_get(cfg.mocap, 'exclude_marker_types', None) or []):
+        return False
+    if not np.any(['face' in t for t in marker_meta['marker_type_mask'].keys()]):
+        return False
+    if not np.any([('face' in t) and l in avail_labels for l, t in marker_meta['marker_type'].items()]):
+        return False
+    if sm.type != 'smplx':
+        return False
+    if free_betas:
+        raise NotImplementedError('optimize_face with optimize_betas: Stage I fits per-frame expressions only for a given shape '
+                                  '(betas_fname or v_template_fname) with optimize_betas off (chmosh.py:287-291)')
+    return True
+
+
 class StageI:
     def __init__(self, stagei_frames, cfg, marker_meta, betas=None, v_template=None, backend=None):
         sm, mp = cfg.surface_model, cfg.moshpp
@@ -271,9 +300,8 @@ class StageI:
                 self.fingers = False
             elif not np.any([('finger' in t) and l in avail for l, t in marker_meta['marker_type'].items()]):
                 self.fingers = False
-        if bool(_get(mp, 'optimize_face', False)):
-            raise NotImplementedError('optimize_face in Stage I (chmosh.py:283-295) is outside this build; run it with the face '
-                                      'markers excluded and optimize_face off, as the reference itself advises (chmosh.py:103-118)')
+        self.free_betas = bool(mp.optimize_betas)
+        self.face = face_flag(cfg, marker_meta, avail)
         if _get(mp, 'head_marker_corr_fname', None) is not None:
             raise NotImplementedError('moshpp.head_marker_corr_fname (chmosh.py:250-264,364-372) is outside this build')
         self.model = model = _pack.load_surface_model(sm.fname, pose_hand_prior_fname=_get(mp, 'pose_hand_prior_fname'),
@@ -289,7 +317,6 @@ class StageI:
         elif pf and model.model_type != 'mano':
             self.prior = _pack.create_gmm_body_prior(pf, exclude_hands=model.model_type in ('smplh', 'smplx'))
         self.nb = int(sm.num_betas)
-        self.free_betas = bool(mp.optimize_betas)
         self.betas = np.zeros(model.shapedirs.shape[-1])
         if betas is not None:
             self.betas[:self.nb] = np.asarray(betas)[:self.nb]                                   # chmosh.py:169-172
@@ -297,6 +324,10 @@ class StageI:
         self.jd_lin = np.einsum('jv,vcd->jcd', model.J_regressor, model.shapedirs[:, :, :self.nb])    # joint directions of the shape block
         self.pose = np.zeros((F, model.p_red))
         self.trans = np.zeros((F, 3))
+        # optimize_face: each picked frame's expression coefficients, betas[es:es + ne] of its own model (chmosh.py:136-151,292-294)
+        self.es = int(_get(sm, 'betas_expr_start_id', 0) or 0) if self.face else 0
+        self.ne = int(_get(sm, 'num_expressions', 0) or 0) if self.face else 0
+        self.expr = np.zeros((F, self.ne))
 
         can_v = self.can(self.betas[:self.nb])                                                   # chmosh.py:57-82
         vn = vertex_normals(can_v, self.faces)
@@ -318,9 +349,15 @@ class StageI:
     # ---- device pack of the current (betas, latent markers): the Stage-II constants with the shape directions as linear block
     def pack_for(self, detailed: bool, can_v=None):
         sm, mp = self.cfg.surface_model, self.cfg.moshpp
+        toes = bool(_get(mp, 'optimize_toes', False))
+        if self.face:
+            # the shape is given: the linear block is the expression directions alone, and Step 2 frees the jaw and them
+            return _pack.build_pack(self.model, self.betas, self.ml, num_betas=self.nb, prior=self.prior,
+                                    optimize_fingers=self.fingers, optimize_toes=toes, optimize_face=True,
+                                    expr_start=self.es, num_expressions=self.ne, can_verts=can_v)
         pk = _pack.build_pack(self.model, self.betas, self.ml, num_betas=self.nb, prior=self.prior,
                               dmpl_dirs=self.model.shapedirs[:, :, :self.nb], num_dmpls=self.nb,
-                              optimize_fingers=self.fingers, optimize_toes=bool(_get(mp, 'optimize_toes', False)),
+                              optimize_fingers=self.fingers, optimize_toes=toes,
                               can_verts=can_v, jd_lin=self.jd_lin)
         lin = [3 + pk.p_red + i for i in range(self.nb)] if self.free_betas else []
         s1 = [int(i) for i in pk.free_step1 if i < 3 + pk.p_red]
@@ -339,6 +376,8 @@ class StageI:
             except (KeyError, AttributeError):
                 base = w['stagei_wt_init']
             out['init'][k] = base * anneal
+        if self.face:                                                                               # chmosh.py:322-324
+            out['poseF'], out['expr'] = w['stagei_wt_poseF'] * anneal, w['stagei_wt_expr'] * anneal
         return out
 
     # ---- one evaluation of the whole objective; with want_jac also its block-arrow normal equations ---------------------
@@ -354,14 +393,22 @@ class StageI:
         n_p = n_f - nb
         x = np.zeros((F, pk.nx))
         x[:, :3], x[:, 3:3 + pk.p_red] = self.trans, self.pose
-        opts = _lib.make_options(None, optimize_fingers=detailed and self.fingers and pk.finger_hi > pk.finger_lo)
+        if self.face:
+            x[:, 3 + pk.p_red:] = self.expr
+        opts = _lib.make_options(None, optimize_fingers=detailed and self.fingers and pk.finger_hi > pk.finger_lo,
+                                 optimize_face=detailed and self.face)
         opts.wt_data, opts.wt_poseB, opts.wt_poseH = float(wts['data']), float(wts['poseB']), float(wts['poseH'])
+        if self.face:
+            opts.wt_poseF, opts.wt_expr = float(wts['poseF']), float(wts['expr'])
         dev = self.backend.linearize(pk, opts, self.obs, self.vis, x, step, want_jac)
         sse = {'data': float(dev['errs'][:, 0].sum())}
         if pk.prior_k:
             sse['poseB'] = float(dev['errs'][:, 1].sum())
         if detailed and self.fingers:
             sse['poseH'] = float(dev['errs'][:, 3].sum())
+        if detailed and self.face:
+            sse['poseF'] = float(dev['errs'][:, 6].sum())
+            sse['expr'] = float(dev['errs'][:, 7].sum())
 
         # init: the latent markers against the initial guess riding on the current canonical body (chmosh.py:185-186,362)
         init, dinit_dv = marker_points(can_v[self.closest0], self.k0)
@@ -395,7 +442,8 @@ class StageI:
         if not want_jac:
             return total, sse, dev
 
-        # ---------------- normal equations, unknowns [betas (nb) | latent markers (3M) | frame 0 (n_p) | frame 1 | ...]
+        # ---------------- normal equations, unknowns [betas (nb) | latent markers (3M) | frame 0 (n_p) | frame 1 | ...];
+        # a frame's private block is [trans | pose ids | expressions (optimize_face, detailed steps)], the free list's order
         ns = nb + 3 * M
         n = ns + F * n_p
         A = np.zeros((n, n))
@@ -467,13 +515,13 @@ class StageI:
         return total, sse, dev, A, g, (pk, free, n_p)
 
     # ---- state <-> unknown vector -------------------------------------------------------------------------------------
-    def get_x(self, pose_ids, nb):
+    def get_x(self, pose_ids, nb, ne=0):
         parts = [self.betas[:nb], self.ml.reshape(-1)]
         for f in range(self.F):
-            parts += [self.trans[f], self.pose[f, pose_ids]]
+            parts += [self.trans[f], self.pose[f, pose_ids], self.expr[f, :ne]]
         return np.concatenate(parts)
 
-    def set_x(self, x, pose_ids, nb):
+    def set_x(self, x, pose_ids, nb, ne=0):
         M, npi = self.M, len(pose_ids)
         self.betas[:nb] = x[:nb]
         self.ml = x[nb:nb + 3 * M].reshape(M, 3).copy()
@@ -481,14 +529,16 @@ class StageI:
         for f in range(self.F):
             self.trans[f] = x[o:o + 3]
             self.pose[f, pose_ids] = x[o + 3:o + 3 + npi]
-            o += 3 + npi
+            self.expr[f, :ne] = x[o + 3 + npi:o + 3 + npi + ne]
+            o += 3 + npi + ne
 
     # ---- chumpy's dog-leg (SURVEY.md A.6; the control flow of csrc/mosh2_device.cuh solve_frame on dense float64 arrays) --
     def minimize(self, wts, detailed, e_3, maxiter, delta_0=0.5, e_1=1e-15, e_2=1e-15):
         nb = self.nb if self.free_betas else 0
         _, _, _, A, g, (pk, free, n_p) = self.evaluate(True, wts, detailed)[:6]
-        pose_ids = np.asarray([int(i) - 3 for i in free[3:n_p]], dtype=np.int64)
-        p = self.get_x(pose_ids, nb)
+        pose_ids = np.asarray([int(i) - 3 for i in free[3:n_p] if i < 3 + pk.p_red], dtype=np.int64)
+        ne = n_p - 3 - len(pose_ids)                     # the expression columns follow the pose ids (optimize_face, Step 2)
+        p = self.get_x(pose_ids, nb, ne)
         sse0 = self._last_total
         delta = delta_0
         done = np.linalg.norm(g, np.inf) < e_1
@@ -517,7 +567,7 @@ class StageI:
                 if np.linalg.norm(d_dl) <= e_2 * np.linalg.norm(p):
                     done = True
                 else:
-                    self.set_x(p + d_dl, pose_ids, nb)
+                    self.set_x(p + d_dl, pose_ids, nb, ne)
                     sse1 = self.evaluate(False, wts, detailed)[0]
                     rho = sse0 - sse1
                     if rho > 0:
@@ -543,7 +593,7 @@ class StageI:
                     break
             if not done and it >= maxiter:
                 done = True
-        self.set_x(p, pose_ids, nb)
+        self.set_x(p, pose_ids, nb, ne)
         self.stats['minimisations'] += 1
 
     def run(self):
@@ -592,6 +642,8 @@ def mosh_stagei(stagei_frames: List[Dict[str, np.ndarray]], cfg, betas_fname=Non
            'stagei_markers_sim_all': sims_all, 'stagei_markers_sim': [sims_all[f][s.vis[f]] for f in range(s.F)],
            'stagei_markers_obs': [s.obs[f][s.vis[f]] for f in range(s.F)], 'stagei_labels_obs': labels_obs,
            'b200': dict(s.stats)}
+    if s.face:
+        dbg['opt_models_expression'] = [e.copy() for e in s.expr]    # betas[es:es + ne] of each picked frame's model
     out = {'betas': s.betas.copy(), 'markers_latent': s.ml.copy(), 'latent_labels': s.labels, 'marker_meta': marker_meta,
            'markers_latent_vids': {l: int(v) for l, v in zip(s.labels, vids)}, 'stagei_debug_details': dbg}
     if v_template_fname is not None:
