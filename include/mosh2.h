@@ -163,15 +163,18 @@ int mosh2_job_upload_markers(mosh2_job *j, const double *markers, int32_t n_file
 /* ---- Stage I building block (chmosh.py:83-455; SURVEY.md 8(f-2)) ------------------------------------------------------------
  * Linearise mode: the frames of the job are INDEPENDENT problems (the twelve frames of Stage I), each evaluated by one
  * thread block at a state the caller gives -- x [F][3 + p_red + n_dmpl] = trans | reduced pose | linear coefficients.  The
- * frame's own terms are data, the pose prior (+ joint-angle term) and, with step == 2, the finger term and (optimize_face)
- * the jaw and expression terms, under opt's wt_data / wt_poseB / wt_poseH / wt_poseF / wt_expr taken as they are (Stage I's
- * annealed weights; no visibility scaling).  step 1 / 2 picks the
+ * frame's own terms are data, the pose prior (+ joint-angle term) and, with step == 2, the finger term, (optimize_face)
+ * the jaw and expression terms and (optimize_dynamics of the job's options, at the job's wt_dmpl) the DMPL term, under opt's
+ * wt_data / wt_poseB / wt_poseH / wt_poseF / wt_expr taken as they are (Stage I's annealed weights; no visibility
+ * scaling).  step 1 / 2 picks the
  * free-variable list free1 / free2 of the model description (n columns).  Outputs (host, float64, any pointer may be NULL):
  *   errs [F][8] SSE per term, markers_sim [F][M][3], r [F][3M] weighted data residual (sim - obs) wt_data (0 where invisible),
  *   vp [F][3M][3] posed attachment vertices; with build != 0 also A [F][n][n], g [F][n] (normal equations of the frame's own
  *   terms, g = -J^T r) and J [F][3M][n] (the weighted data rows d r / d x_free).
  * With the shape directions (or, with optimize_face and a given shape, the expression directions) as the model's linear
- * block these are all per-frame quantities the joint shape / latent-marker solve needs (moshpp_b200/stagei.py).  Float64 jobs of one-frame chunks only (chunk_len = 1).  Synchronous. */
+ * block these are all per-frame quantities the joint shape / latent-marker solve needs (moshpp_b200/stagei.py).  Jobs of
+ * one-frame chunks only (chunk_len = 1).  A float32 job rounds x to float32 and computes in float32; its outputs are widened
+ * to the float64 buffers.  Synchronous. */
 typedef struct mosh2_lin_out {
     double *errs, *markers_sim, *r, *vp, *A, *g, *J;
 } mosh2_lin_out;

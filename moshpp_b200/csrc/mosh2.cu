@@ -499,6 +499,52 @@ void plan_workspace(mosh2::Model<real> &m, size_t *smem, size_t *gws, int *big) 
     }
 }
 
+// mosh2_job_linearize in the job's compute type: the caller's float64 states are rounded to `real` on the way in, every
+// output is widened to the float64 buffers of mosh2_lin_out on the way out
+template <class real>
+int linearize(mosh2_job *j, const mosh2::Model<real> &m, int32_t step, int32_t build, const double *x, const mosh2_lin_out *out) {
+    const size_t F = j->n_frames, M = j->model->n_markers, NX = 3 + j->model->p_red + j->model->n_dmpl;
+    const size_t n = step == 2 ? m.n2 : m.n1, n2 = m.n2 > m.n1 ? m.n2 : m.n1;
+    const size_t words = F * (NX + n2 * n2 + n2 + 3 * M * n2 + 3 * M + 9 * M);
+    if (words * sizeof(real) > j->lin_bytes) {
+        g_blocks.put(j->model->device, j->d_lin);
+        j->d_lin = nullptr; j->lin_bytes = 0;
+        CU(g_blocks.get(j->model->device, words * sizeof(real), &j->d_lin));
+        j->lin_bytes = words * sizeof(real);
+    }
+    const std::vector<real> xr(x, x + F * NX);      // (alive until the stream is synchronised below)
+    CU(cudaMemcpyAsync(j->d_lin, xr.data(), F * NX * sizeof(real), cudaMemcpyHostToDevice, j->stream));
+    CU(cudaMemsetAsync(j->d_out, 0, j->n_out * j->esz, j->stream));
+    j->lin_mode = build ? 2 : 1;
+    j->lin_step = step;
+    j->subset = false;
+    j->launch_blocks = int(F);
+    const int rc = launch<real>(j, m);
+    j->lin_mode = 0;
+    j->launch_blocks = j->n_chunks;
+    if (rc) return rc;
+    const real *p = static_cast<const real *>(j->d_lin) + F * NX;
+    const real *dA = p; p += F * n * n;
+    const real *dg = p; p += F * n;
+    const real *dJ = p; p += F * 3 * M * n;
+    const real *dr = p; p += F * 3 * M;
+    const real *dvp = p;
+    const real *dout = static_cast<const real *>(j->d_out);
+    struct Back { double *dst; const real *src; size_t cnt; std::vector<real> h; };
+    Back b[7] = {{out->r, dr, F * 3 * M, {}}, {out->vp, dvp, F * 9 * M, {}}, {out->errs, dout + j->o_errs, F * mosh2::N_ERR, {}},
+                 {out->markers_sim, dout + j->o_mk, F * 3 * M, {}}, {build ? out->A : nullptr, dA, F * n * n, {}},
+                 {build ? out->g : nullptr, dg, F * n, {}}, {build ? out->J : nullptr, dJ, F * 3 * M * n, {}}};
+    for (Back &e : b) {
+        if (!e.dst) continue;
+        e.h.resize(e.cnt);
+        CU(cudaMemcpyAsync(e.h.data(), e.src, e.cnt * sizeof(real), cudaMemcpyDeviceToHost, j->stream));
+    }
+    CU(cudaStreamSynchronize(j->stream));
+    for (const Back &e : b)
+        if (e.dst) for (size_t i = 0; i < e.cnt; ++i) e.dst[i] = double(e.h[i]);
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -723,48 +769,14 @@ int mosh2_job_upload_markers(mosh2_job *j, const double *markers, int32_t n_file
 
 int mosh2_job_linearize(mosh2_job *j, const mosh2_options *opt, int32_t step, int32_t build, const double *x, const mosh2_lin_out *out) {
     if (!j || !x || !out || (step != 1 && step != 2)) return fail(MOSH2_E_INVALID, "bad argument");
-    if (j->precision != MOSH2_F64) return fail(MOSH2_E_INVALID, "mosh2_job_linearize needs a float64 job");
     if (j->n_chunks < j->n_frames) return fail(MOSH2_E_INVALID, "mosh2_job_linearize needs a job of one-frame chunks (chunk_len = 1)");
     CU(cudaSetDevice(j->model->device));
-    const mosh2::Model<double> &m = j->model->f64.m;
-    const size_t F = j->n_frames, M = j->model->n_markers, NX = 3 + j->model->p_red + j->model->n_dmpl;
-    const size_t n = step == 2 ? m.n2 : m.n1, n2 = m.n2 > m.n1 ? m.n2 : m.n1;
-    const size_t words = F * (NX + n2 * n2 + n2 + 3 * M * n2 + 3 * M + 9 * M);
-    if (words * sizeof(double) > j->lin_bytes) {
-        g_blocks.put(j->model->device, j->d_lin);
-        j->d_lin = nullptr; j->lin_bytes = 0;
-        CU(g_blocks.get(j->model->device, words * sizeof(double), &j->d_lin));
-        j->lin_bytes = words * sizeof(double);
-    }
     if (opt) {      // the weights of this evaluation (Stage I anneals them between minimisations)
         mosh2::Options &o = j->opt;
         o.wt_data = opt->wt_data; o.wt_poseB = opt->wt_poseB; o.wt_poseH = opt->wt_poseH; o.optimize_fingers = opt->optimize_fingers;
     }
-    CU(cudaMemcpyAsync(j->d_lin, x, F * NX * sizeof(double), cudaMemcpyHostToDevice, j->stream));
-    CU(cudaMemsetAsync(j->d_out, 0, j->n_out * j->esz, j->stream));
-    j->lin_mode = build ? 2 : 1;
-    j->lin_step = step;
-    j->subset = false;
-    j->launch_blocks = int(F);
-    const int rc = launch<double>(j, m);
-    j->lin_mode = 0;
-    j->launch_blocks = j->n_chunks;
-    if (rc) return rc;
-    const double *p = static_cast<const double *>(j->d_lin) + F * NX;
-    const double *dA = p; p += F * n * n;
-    const double *dg = p; p += F * n;
-    const double *dJ = p; p += F * 3 * M * n;
-    const double *dr = p; p += F * 3 * M;
-    const double *dvp = p;
-    const double *dout = static_cast<const double *>(j->d_out);
-    auto back = [&](double *dst, const double *src, size_t cnt) { return dst ? cudaMemcpyAsync(dst, src, cnt * sizeof(double), cudaMemcpyDeviceToHost, j->stream) : cudaSuccess; };
-    if (build) { CU(back(out->A, dA, F * n * n)); CU(back(out->g, dg, F * n)); CU(back(out->J, dJ, F * 3 * M * n)); }
-    CU(back(out->r, dr, F * 3 * M));
-    CU(back(out->vp, dvp, F * 9 * M));
-    CU(back(out->errs, dout + j->o_errs, F * mosh2::N_ERR));
-    CU(back(out->markers_sim, dout + j->o_mk, F * 3 * M));
-    CU(cudaStreamSynchronize(j->stream));
-    return 0;
+    if (j->precision == MOSH2_F64) return linearize<double>(j, j->model->f64.m, step, build, x, out);
+    return linearize<float>(j, j->model->f32.m, step, build, x, out);
 }
 
 int mosh2_job_launch(mosh2_job *j) {

@@ -326,7 +326,8 @@ class Job:
 
     def linearize(self, x: np.ndarray, options: Options, step: int, build: bool) -> Dict[str, np.ndarray]:
         """mosh2_job_linearize: every frame of the job evaluated (and, with ``build``, linearised) at its row of ``x``
-        [F, 3 + p_red + n_dmpl]; see include/mosh2.h.  Needs a float64 job of one-frame chunks and uploaded observations."""
+        [F, 3 + p_red + n_dmpl]; see include/mosh2.h.  Needs a job of one-frame chunks and uploaded observations.  A float32
+        job evaluates at ``x`` rounded to float32 and returns its float32 results as float64 arrays."""
         pk = self.model.pk
         F, M = self.n_frames, pk.n_markers
         n = len(pk.free_step2) if step == 2 else len(pk.free_step1)

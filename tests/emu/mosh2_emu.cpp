@@ -206,24 +206,26 @@ int run(const mosh2_model_desc *desc, const mosh2_options *opt, int n_frames, co
     return 0;
 }
 
-// linearise mode (mosh2_job_linearize): every frame evaluated / linearised at the caller's state, float64
+// linearise mode (mosh2_job_linearize): every frame evaluated / linearised at the caller's state; observations and states
+// rounded to `real` and the outputs widened to float64, as the library does
+template <class real>
 int run_lin(const mosh2_model_desc *desc, const mosh2_options *opt, int n_frames, const double *obs, const uint8_t *vis,
             int step, int build, const double *x, const mosh2_lin_out *out) {
-    typedef double real;
     HostModel<real> hm;
     hm.build(*desc);
     const size_t F = n_frames, M = desc->n_markers, PF = size_t(3) * desc->n_joints, PR = desc->p_red, nd = desc->n_dmpl;
     const size_t NX = 3 + PR + nd, n = step == 2 ? desc->n_free2 : desc->n_free1;
     std::vector<real> fullpose(F * PF), pose(F * PR), trans(F * 3), dmpls(F * nd + 1), mk(F * M * 3), errs(F * mosh2::N_ERR);
     std::vector<real> A(F * n * n), g(F * n), J(F * 3 * M * n), r(F * 3 * M), vp(F * 9 * M);
+    const std::vector<real> o(obs, obs + F * M * 3), xr(x, x + F * NX);
     mosh2::Job<real> job{};
     job.n_frames = n_frames; job.n_chunks = n_frames;
-    job.obs = obs; job.vis = vis;
+    job.obs = o.data(); job.vis = vis;
     job.fullpose = fullpose.data(); job.pose = pose.data(); job.trans = trans.data();
     job.dmpls = nd ? dmpls.data() : nullptr; job.markers_sim = mk.data(); job.errs = errs.data();
     std::vector<int> status(F, 0), counters(F * 4, 0);
     job.status = status.data(); job.counters = counters.data();
-    job.lin_mode = build ? 2 : 1; job.lin_step = step; job.lin_x = x;
+    job.lin_mode = build ? 2 : 1; job.lin_step = step; job.lin_x = xr.data();
     job.lin_A = A.data(); job.lin_g = g.data(); job.lin_J = J.data(); job.lin_r = r.data(); job.lin_vp = vp.data();
     mosh2::Options &q = job.opt;
     q.wt_data = opt->wt_data; q.wt_poseB = opt->wt_poseB; q.wt_poseH = opt->wt_poseH; q.wt_velo = opt->wt_velo;
@@ -246,7 +248,7 @@ int run_lin(const mosh2_model_desc *desc, const mosh2_options *opt, int n_frames
         mosh2::Solver<real, false> s(hm.m, job, w, d, cta);
         s.run_chunk(f);
     }
-    auto back = [](double *dst, const std::vector<real> &src) { if (dst) std::memcpy(dst, src.data(), src.size() * sizeof(double)); };
+    auto back = [](double *dst, const std::vector<real> &src) { if (dst) for (size_t i = 0; i < src.size(); ++i) dst[i] = double(src[i]); };
     back(out->errs, errs); back(out->markers_sim, mk); back(out->r, r); back(out->vp, vp);
     if (build) { back(out->A, A); back(out->g, g); back(out->J, J); }
     return 0;
@@ -254,9 +256,17 @@ int run_lin(const mosh2_model_desc *desc, const mosh2_options *opt, int n_frames
 
 }  // namespace
 
+extern "C" int mosh2_emu_linearize_precision(const mosh2_model_desc *desc, const mosh2_options *opt, int32_t n_frames, const double *obs,
+                                             const uint8_t *vis, int32_t step, int32_t build, const double *x, int32_t precision,
+                                             const mosh2_lin_out *out) {
+    if (precision == MOSH2_F64) return run_lin<double>(desc, opt, n_frames, obs, vis, step, build, x, out);
+    return run_lin<float>(desc, opt, n_frames, obs, vis, step, build, x, out);
+}
+
+// float64, the Stage-I back end of the tests (conftest.EmuStageIBackend)
 extern "C" int mosh2_emu_linearize(const mosh2_model_desc *desc, const mosh2_options *opt, int32_t n_frames, const double *obs,
                                    const uint8_t *vis, int32_t step, int32_t build, const double *x, const mosh2_lin_out *out) {
-    return run_lin(desc, opt, n_frames, obs, vis, step, build, x, out);
+    return run_lin<double>(desc, opt, n_frames, obs, vis, step, build, x, out);
 }
 
 extern "C" int mosh2_emu_solve(const mosh2_model_desc *desc, const mosh2_options *opt, int32_t n_frames,
