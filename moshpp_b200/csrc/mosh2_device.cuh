@@ -1617,8 +1617,9 @@ struct Solver {
 #endif
     }
 
-    // ---- factor and invert the 8x8 diagonal block at k0 (GPU: the calling warp, all 32 lanes; host: one thread)
-    M2_D void chol_diag(int k0, int n) {
+    // ---- factor and invert the 8x8 diagonal block at k0 (GPU: the calling warp, all 32 lanes; host: one thread).
+    //      Returns false if a pivot is not above pivot_eps (GPU: in every lane of the warp; host: also clears w.isc[3]).
+    M2_D bool chol_diag(int k0, int n) {
         const int ld = d.ld;
         constexpr int NB = kCholNB;
         const int kb = (n - k0 < NB) ? n - k0 : NB;
@@ -1698,7 +1699,7 @@ struct Solver {
                         }
                     }
             }
-            if (!ok && lane == 0) w.isc[3] = 0;
+            return ok;
                 }
 #else
         {
@@ -1733,6 +1734,7 @@ struct Solver {
                 for (int cc = 0; cc < NB; ++cc)
                     if (r >= kb || cc >= kb) Li[r * NB + cc] = (r == cc) ? real(1) : real(0);
             if (!ok) w.isc[3] = 0;
+            return ok;
                 }
 #endif
     }
@@ -1827,7 +1829,6 @@ struct Solver {
             const real a = w.A[i * d.lda + i];
             w.ds[i] = (a > real(0)) ? real(1) / r_sqrt(a) : real(0);
         }
-        if (cta.tid == 0) w.isc[3] = 1;
         M2_SYNC();
 #if M2_GPU
         {
@@ -1848,11 +1849,15 @@ struct Solver {
         // block, the update of that block, its factorisation and inversion -- while the other warps solve the rest of the
         // panel and apply the trailing update; they only wait (named barrier 1) for warp 0's eight panel rows.  One full
         // barrier per block, and a single call site of the diagonal-block factorisation (the pseudo-block k0 = -NB
-        // factors the first one).  (The launcher never starts fewer than 128 threads.)
+        // factors the first one).  (The launcher never starts fewer than 128 threads.)  The block's full barrier also carries
+        // warp 0's verdict on the block it factored: a flag in shared memory would be cleared by warp 0 in its next
+        // chol_diag before a slow warp had read it (warp 0 passes no blocking barrier in between), and that warp would
+        // return one block early while the others wait for it on barrier 1.
         {
             const int nthr = cta.nthr;
 #pragma unroll 1
             for (int k0 = -NB; k0 < n; k0 += NB) {
+                bool ok = true;
                 const int kb = k0 < 0 ? 0 : ((n - k0 < NB) ? n - k0 : NB);
                 const int r0 = k0 < 0 ? 0 : k0 + kb;
                 const real *Li = w.Linv + (k0 < 0 ? 0 : k0 / NB) * NB * NB;
@@ -1887,7 +1892,7 @@ struct Solver {
                         }
                     }
                     M2_TACC(12);
-                    if (r0 < n) chol_diag(r0, n);
+                    if (r0 < n) ok = chol_diag(r0, n);
                     M2_TACC(13);
                 } else {
                     if (k0 >= 0) {
@@ -1900,13 +1905,13 @@ struct Solver {
                         }
                     }
                 }
-                M2_SYNC();
-                if (w.isc[3] == 0) return false;
+                if (__syncthreads_or(!ok)) return false;
             }
             M2_TACC(14);
         }
 #else
         // host build: the same blocked right-looking factorisation, one block after the other
+        w.isc[3] = 1;
         chol_diag(0, n);
         if (w.isc[3] == 0) return false;
         for (int k0 = 0; k0 < n; k0 += NB) {

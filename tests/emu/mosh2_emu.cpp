@@ -7,6 +7,7 @@
 #include "../../include/mosh2.h"
 #include "../../moshpp_b200/csrc/mosh2_device.cuh"
 #include "../../moshpp_b200/csrc/mosh2_host.h"
+#include "../tc/gauss_newton_case.h"
 
 #include <algorithm>
 #include <cstdlib>
@@ -254,7 +255,44 @@ int run_lin(const mosh2_model_desc *desc, const mosh2_options *opt, int n_frames
     return 0;
 }
 
+// one Gauss-Newton solve and A g in the workspace of a model with the dimensions of `desc`: the host twin of gn_run
+// (tests/tc/gauss_newton_test.cu), with the same layout and the same NaN fill
+template <class real, bool BIG>
+int run_gn(const mosh2_model_desc *desc, int n, const double *A, const double *g, double *dgn_out, double *Ag_out, int *ok_out) {
+    mosh2::Model<real> m = gn_case::dims_model<real>(*desc);
+    mosh2::Dims d;
+    mosh2::Work<real, BIG> w;
+    size_t smem = 0, gws_bytes = 0;
+    if (n < 1 || n > m.n2 || !gn_case::layout<real, BIG>(m, d, w, smem, gws_bytes)) return -1;
+    std::vector<char> smem_raw(smem + 32, char(gn_case::kNaN)), gws_raw(gws_bytes + 32, char(gn_case::kNaN));
+    unsigned char *smem_base = reinterpret_cast<unsigned char *>(smem_raw.data() + ((32 - (reinterpret_cast<uintptr_t>(smem_raw.data()) & 31)) & 31));
+    char *gws = gws_raw.data() + ((32 - (reinterpret_cast<uintptr_t>(gws_raw.data()) & 31)) & 31);
+    mosh2::m2_smem_ref() = smem_base;
+    if (BIG) *reinterpret_cast<char **>(smem_base) = gws;
+    real *wA = w.A, *wg = w.g;
+    for (int i = 0; i < n; ++i) {
+        for (int j = 0; j < n; ++j) wA[i * d.lda + j] = real(A[size_t(i) * n + j]);
+        wg[i] = real(g[i]);
+    }
+    const mosh2::Job<real> job{};
+    mosh2::Solver<real, BIG> s(m, job, w, d, mosh2::Cta{0, 1});
+    const bool solved = s.gauss_newton(n);
+    s.symv(w.g, w.Ag, n);
+    for (int i = 0; i < n; ++i) { dgn_out[i] = double(w.dgn[i]); Ag_out[i] = double(w.Ag[i]); }
+    *ok_out = solved ? 1 : 0;
+    return 0;
+}
+
 }  // namespace
+
+// `threads` is accepted for the signature of gn_run and ignored: the host build is one thread
+extern "C" int mosh2_emu_gauss_newton(int32_t precision, int32_t big, int32_t threads, const mosh2_model_desc *desc, int32_t n,
+                                      const double *A, const double *g, double *dgn_out, double *Ag_out, int32_t *ok_out) {
+    (void)threads;
+    if (precision == MOSH2_F64)
+        return big ? run_gn<double, true>(desc, n, A, g, dgn_out, Ag_out, ok_out) : run_gn<double, false>(desc, n, A, g, dgn_out, Ag_out, ok_out);
+    return big ? run_gn<float, true>(desc, n, A, g, dgn_out, Ag_out, ok_out) : run_gn<float, false>(desc, n, A, g, dgn_out, Ag_out, ok_out);
+}
 
 extern "C" int mosh2_emu_linearize_precision(const mosh2_model_desc *desc, const mosh2_options *opt, int32_t n_frames, const double *obs,
                                              const uint8_t *vis, int32_t step, int32_t build, const double *x, int32_t precision,
