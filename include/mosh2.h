@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MOSH2_VERSION 104
+#define MOSH2_VERSION 105
 
 enum {
     MOSH2_OK = 0,
@@ -160,6 +160,14 @@ int mosh2_job_upload(mosh2_job *j, const double *obs, const uint8_t *vis);
  * observations (metres, compute precision) and visibility.  Async on the job's stream; replaces mosh2_job_upload. */
 int mosh2_job_upload_markers(mosh2_job *j, const double *markers, int32_t n_file_frames, int32_t n_cols, const int32_t *col_of_marker,
                              int32_t frame_start, int32_t frame_step, double unit_per_metre, const double *rot3x3);
+/* ... for frames [frame0, frame0 + n) of the job's frame axis only (one capture of a batch job, mosh2_job_create_batch):
+ * job frame frame0 + k is file frame frame_start + k * frame_step of this capture's table.  Every call stages its own rows
+ * (pinned host memory that is not reused before the call's copy and kernel have finished), so the uploads of a subject's
+ * captures can be issued back to back without waiting; the caller's buffers may be freed when the call returns.  Async on
+ * the job's stream. */
+int mosh2_job_upload_markers_range(mosh2_job *j, int32_t frame0, int32_t n, const double *markers, int32_t n_file_frames, int32_t n_cols,
+                                   const int32_t *col_of_marker, int32_t frame_start, int32_t frame_step, double unit_per_metre,
+                                   const double *rot3x3);
 /* ---- Stage I building block (chmosh.py:83-455; SURVEY.md 8(f-2)) ------------------------------------------------------------
  * Linearise mode: the frames of the job are INDEPENDENT problems (the twelve frames of Stage I), each evaluated by one
  * thread block at a state the caller gives -- x [F][3 + p_red + n_dmpl] = trans | reduced pose | linear coefficients.  The

@@ -14,6 +14,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libmosh2.so')
 EMU_SRC = os.path.join(ROOT, 'tests', 'emu', 'mosh2_emu.cpp')
+EMU_ADAPTER_SRC = os.path.join(ROOT, 'tests', 'emu', 'mosh2_emu_adapter.cpp')
 EMU_LIB = os.path.join(ROOT, 'tests', 'emu', '_build', 'libmosh2_emu.so')
 TC_SRC = os.path.join(ROOT, 'tests', 'tc', 'jtj_tf32_test.cu')
 TC_BIN = os.path.join(ROOT, 'tests', 'tc', '_build', 'jtj_test')
@@ -56,10 +57,11 @@ def build_library(force: bool = False, verbose: bool = False) -> str:
 def build_emu(force: bool = False) -> str:
     """TEST-ONLY single-thread host build of the CTA program (see tests/emu/mosh2_emu.cpp)."""
     srcs = [EMU_SRC, os.path.join(CSRC, "mosh2_device.cuh"), os.path.join(CSRC, "mosh2_host.h"), os.path.join(ROOT, 'include', 'mosh2.h'),
-            os.path.join(ROOT, 'tests', 'tc', 'gauss_newton_case.h')]
+            os.path.join(ROOT, 'tests', 'tc', 'gauss_newton_case.h'), EMU_ADAPTER_SRC]
     if force or _stale(EMU_LIB, srcs):
         os.makedirs(os.path.dirname(EMU_LIB), exist_ok=True)
-        cmd = ['g++', '-O2', '-std=c++17', '-shared', '-fPIC', '-o', EMU_LIB, EMU_SRC]
+        units = [EMU_SRC] + ([EMU_ADAPTER_SRC] if os.path.exists(EMU_ADAPTER_SRC) else [])     # (the input adapter's host build)
+        cmd = ['g++', '-O2', '-std=c++17', '-shared', '-fPIC', '-o', EMU_LIB] + units
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError('g++ failed:\n' + r.stdout + r.stderr)

@@ -432,6 +432,31 @@ def download_verified(job, bad, report):
     return res
 
 
+def _select_input(mocap: MocapSession, cfg, latent_labels, device_adapter: bool):
+    """(selected frames, file column of every latent marker or None, obs, vis, number of frames) of one capture.
+
+    Input adapter.  Normally on the device: the raw marker table of the file goes up as it is and one kernel produces the
+    observations and the visibility mask (mosh2_job_upload_markers); the host copy of the same clean-up -- needed for the
+    output dictionary only -- is made behind the solve.  Labels that own several columns, and frame selections that are
+    not a forward range inside the file, take the host path (``frames_for_labels``, obs / vis returned here) in front of
+    the solve."""
+    end = len(mocap) if cfg.mocap.end_fidx == -1 else cfg.mocap.end_fidx
+    selected_frames = range(cfg.mocap.start_fidx, end, cfg.mocap.ds_rate)                         # chmosh.py:539-540
+    raw_cols = mocap.raw_columns_for_labels(list(latent_labels)) if device_adapter else None
+    if raw_cols is not None and not (len(selected_frames) and selected_frames.step > 0 and selected_frames.start >= 0
+                                     and selected_frames[-1] < len(mocap)):
+        raw_cols = None
+    if raw_cols is None:
+        obs, vis = mocap.frames_for_labels(list(latent_labels), selected_frames)
+        F = obs.shape[0]
+    else:
+        obs = vis = None
+        F = len(selected_frames)
+    if F == 0:
+        raise ValueError('no frames selected')
+    return selected_frames, raw_cols, obs, vis, F
+
+
 def mosh_stageii(mocap_fname: str, cfg, markers_latent: np.ndarray, latent_labels: list, betas: np.ndarray,
                  marker_meta: dict, v_template_fname=None, *, device: int = 0, mode: str = 'fast',
                  chunk_len: Optional[int] = None, chunk_warmup: Optional[int] = None, warmup_full: Optional[int] = None,
@@ -481,24 +506,7 @@ def mosh_stageii(mocap_fname: str, cfg, markers_latent: np.ndarray, latent_label
     if boundary_tol is None:
         boundary_tol = tol_def
 
-    end = len(mocap) if cfg.mocap.end_fidx == -1 else cfg.mocap.end_fidx
-    selected_frames = range(cfg.mocap.start_fidx, end, cfg.mocap.ds_rate)                         # chmosh.py:539-540
-    # Input adapter.  Normally on the device: the raw marker table of the file goes up as it is and one kernel produces the
-    # observations and the visibility mask (mosh2_job_upload_markers); the host copy of the same clean-up -- needed for the
-    # output dictionary only -- is made behind the solve.  Labels that own several columns, and frame selections that are
-    # not a forward range inside the file, take the host path (``frames_for_labels``) in front of the solve.
-    raw_cols = mocap.raw_columns_for_labels(list(latent_labels)) if device_adapter else None
-    if raw_cols is not None and not (len(selected_frames) and selected_frames.step > 0 and selected_frames.start >= 0
-                                     and selected_frames[-1] < len(mocap)):
-        raw_cols = None
-    if raw_cols is None:
-        obs, vis = mocap.frames_for_labels(list(latent_labels), selected_frames)
-        F = obs.shape[0]
-    else:
-        obs = vis = None
-        F = len(selected_frames)
-    if F == 0:
-        raise ValueError('no frames selected')
+    selected_frames, raw_cols, obs, vis, F = _select_input(mocap, cfg, latent_labels, device_adapter)
     if first_extra is None:
         first_extra = first_chunk_extra(chunk_warmup, warmup_full)
     if chunk_len is None:
@@ -573,3 +581,131 @@ def mosh_stageii(mocap_fname: str, cfg, markers_latent: np.ndarray, latent_label
     if n_fb:
         logger.warning('%d frames hit a non-positive-definite Gauss-Newton system (Cauchy step used)', n_fb)
     return data
+
+
+class _SeqResult:
+    """Rows [a, b) of a batch job's ResultArrays: the result arrays of one capture."""
+
+    def __init__(self, res: '_lib.ResultArrays', a: int, b: int):
+        for k in ('fullpose', 'pose', 'trans', 'dmpls', 'markers_sim', 'errs', 'status', 'counters'):
+            setattr(self, k, getattr(res, k)[a:b].copy())
+        self.nd = res.nd
+
+
+def mosh_stageii_batch(mocap_fnames, cfg, markers_latent: np.ndarray, latent_labels: list, betas: np.ndarray, marker_meta: dict,
+                       v_template_fname=None, *, device: int = 0, mode: str = 'fast', chunk_len: Optional[int] = None,
+                       chunk_warmup: Optional[int] = None, warmup_full: Optional[int] = None, first_extra: Optional[int] = None,
+                       precision: Optional[str] = None, verify: bool = True, boundary_tol=None, sm_budget: int = NUM_SMS,
+                       labels_map='general', subject_cache: bool = True, device_adapter: bool = True) -> list:
+    """Stage II of several captures of ONE subject (one Stage-I result, one ``cfg`` apart from ``mocap.fname``) in one launch.
+
+    Returns one dictionary per capture, in the order of ``mocap_fnames``: what ``mosh_stageii`` returns for that capture with
+    the same keyword arguments, except ``stageii_debug_details['b200']``.  The captures share one pack (subject cache) and one
+    batch job (mosh2_job_create_batch): their frames lie back to back on the job's frame axis, the chunk length is planned
+    over all their frame counts (``plan_chunk_len``, as ``shard.GpuRankSolver`` does), and one verified launch with its
+    repair rounds (``launch_verified``) and one download serve them all.  Every capture uploads its own raw marker table
+    into its range of the job (mosh2_job_upload_markers_range); a capture whose labels own several columns or whose frame
+    selection is not a forward range takes the host adapter, as in ``mosh_stageii``.  ``b200`` holds the capture's own
+    status / counters / frame ids and, under ``'batch'``, the figures of the whole launch (device time, chunks, boundary
+    check, totals), marked ``'shared': True`` -- the same for every capture of the call."""
+    t0 = time.time()
+    if mode not in BOUNDARY_TOL:
+        raise ValueError(f"mode must be 'fast' or 'exact', not {mode!r}")
+    mocap_fnames = list(mocap_fnames)
+    if not mocap_fnames:
+        raise ValueError('no captures given')
+    only = [cfg.mocap.subject_name] if cfg.mocap.multi_subject else None
+    seqs = []
+    for fn in mocap_fnames:
+        mocap = MocapSession(fn, mocap_unit=cfg.mocap.unit, mocap_rotate=cfg.mocap.rotate, labels_map=labels_map, only_subjects=only)
+        sel, raw_cols, obs, vis, F = _select_input(mocap, cfg, latent_labels, device_adapter)
+        seqs.append(dict(fname=fn, mocap=mocap, sel=sel, raw_cols=raw_cols, obs=obs, vis=vis, F=F))
+    if subject_cache:
+        pk, opts, flags, model, cache_hit = subject_for(cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname, device)
+    else:
+        pk, opts, flags = prepare_stageii(cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname)
+        model, cache_hit = None, False
+    dyn = bool(opts.optimize_dynamics)
+    w_def, wf_def, prec_def, tol_def = default_schedule(pk.model_type, mode, pk.n_dmpl)
+    chunk_warmup = w_def if chunk_warmup is None else int(chunk_warmup)
+    warmup_full = (wf_def if chunk_warmup == w_def else -1) if warmup_full is None else int(warmup_full)
+    precision = precision or prec_def
+    if boundary_tol is None:
+        boundary_tol = tol_def
+    counts = [s['F'] for s in seqs]
+    if first_extra is None:
+        first_extra = first_chunk_extra(chunk_warmup, warmup_full)
+    if chunk_len is None:
+        chunk_len = plan_chunk_len(counts, sm_budget, chunk_warmup, warmup_full if warmup_full >= 0 else chunk_warmup,
+                                   first_extra=first_extra)
+    if chunk_len >= max(counts):
+        chunk_len = 0
+    prec = {'f32': _lib.MOSH2_F32, 'f64': _lib.MOSH2_F64}[precision]
+    labels = list(latent_labels)
+
+    own_model = model is None
+    if own_model:
+        model = _lib.Model(pk, device=device)
+    try:
+        job = model.job(counts, opts, chunk_len=chunk_len, chunk_warmup=chunk_warmup, warmup_full=warmup_full, precision=prec,
+                        first_extra=first_extra)
+        try:
+            offsets = job.seq_offsets
+            if any(s['raw_cols'] is None for s in seqs):
+                # host-adapter captures: one upload of the whole frame axis; the device-adapter ranges are written over it
+                obs = np.zeros((job.n_frames, pk.n_markers, 3))
+                vis = np.zeros((job.n_frames, pk.n_markers), dtype=bool)
+                for k, s in enumerate(seqs):
+                    if s['raw_cols'] is None:
+                        obs[offsets[k]:offsets[k + 1]], vis[offsets[k]:offsets[k + 1]] = s['obs'], s['vis']
+                job.upload(obs, vis)
+            rot = None if cfg.mocap.rotate is None else _rotation_xyz(cfg.mocap.rotate)
+            for k, s in enumerate(seqs):            # issued back to back: every call stages its own rows
+                if s['raw_cols'] is not None:
+                    m = s['mocap']
+                    job.upload_markers_range(int(offsets[k]), s['F'], m.raw, s['raw_cols'], s['sel'].start, s['sel'].step,
+                                             m.unit_per_metre, rot)
+
+            def host_side():                        # the result-independent half of every output, behind the solve
+                for s in seqs:
+                    if s['raw_cols'] is not None:
+                        s['obs'], s['vis'] = s['mocap'].frames_for_labels(labels, s['sel'])
+                    s['lists'] = observation_lists(s['obs'], s['vis'], labels)
+                    s['markers_orig'] = s['mocap'].markers[s['sel']]
+
+            bad, report = launch_verified(job, boundary_tol if verify else None, while_running=host_side)
+            res = download_verified(job, bad, report)
+            kernel_ms = float(sum(report['kernel_ms']))
+            n_chunks = job.num_chunks
+            totals = job.totals()
+        finally:
+            job.close()
+    finally:
+        if own_model:
+            model.close()
+
+    batch = {'shared': True, 'captures': len(seqs), 'frames': int(sum(counts)), 'kernel_ms': kernel_ms, 'wall_s': time.time() - t0,
+             'chunks': n_chunks, 'chunk_len': chunk_len, 'chunk_warmup': chunk_warmup, 'warmup_full': warmup_full,
+             'first_extra': first_extra, 'precision': precision, 'mode': mode, 'boundary_check': report, 'totals': totals,
+             'subject_cache_hit': cache_hit}
+    out = []
+    for k, s in enumerate(seqs):
+        r = _SeqResult(res, int(offsets[k]), int(offsets[k + 1]))
+        data = assemble_stageii_data(r, s['obs'], s['vis'], labels, pk, flags, dyn, s.get('lists'))
+        m = s['mocap']
+        solved = (r.status & _lib.ST_SOLVED) != 0
+        data['stageii_debug_details'].update({
+            'markers_orig': s['markers_orig'] if 'markers_orig' in s else m.markers[s['sel']],
+            'labels_orig': m.labels,
+            'mocap_fname': s['fname'],
+            'mocap_frame_rate': m.frame_rate,
+            'mocap_time_length': m.time_length(),
+            'b200': {'batch': batch, 'batch_index': k, 'frame_offset': int(offsets[k]), 'device_adapter': s['raw_cols'] is not None,
+                     'status': r.status.copy(), 'counters': r.counters.copy(), 'pose_reduced': r.pose[solved],
+                     'frame_ids': np.nonzero(solved)[0]},
+        })
+        out.append(data)
+    n_fb = int(((res.status & _lib.ST_GN_FALLBACK) != 0).sum())
+    if n_fb:
+        logger.warning('%d frames hit a non-positive-definite Gauss-Newton system (Cauchy step used)', n_fb)
+    return out

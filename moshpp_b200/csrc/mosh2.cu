@@ -306,8 +306,8 @@ __global__ void boundary_delta_kernel(const real *__restrict__ warm_x, const int
 
 // Mocap input adapter on the device (tools/mocap_interface.py:186,223-225,254-279; chmosh.py:582-594): from the raw marker
 // table of a capture file [file frame][file column][xyz] (file units, float64) to the job's observations [frame][marker][xyz]
-// (metres, compute precision) and visibility.  A sample is missing when a coordinate is NaN or all three are exactly zero
-// (:277); such samples -- and markers whose label the file does not have (col < 0) -- are invisible and stored as zero.
+// (metres, compute precision) and visibility, per sample by mosh2::gather_marker_sample; markers whose label the file does
+// not have (col < 0) are invisible and stored as zero.  `obs` / `vis` point at the first frame the call writes.
 template <class real>
 __global__ void gather_markers_kernel(const double *__restrict__ raw, int n_cols, const int *__restrict__ col_of_marker, int M,
                                       int n_frames, int frame_step, double unit_per_metre, const double *__restrict__ rot,
@@ -315,22 +315,10 @@ __global__ void gather_markers_kernel(const double *__restrict__ raw, int n_cols
     const size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
     if (i >= size_t(n_frames) * M) return;
     const int f = int(i / M), mk = int(i - size_t(f) * M), col = col_of_marker[mk];
-    double x = 0, y = 0, z = 0;
-    bool ok = false;
-    if (col >= 0) {
-        const double *p = raw + (size_t(f) * frame_step * n_cols + col) * 3;
-        x = p[0]; y = p[1]; z = p[2];
-        ok = !(isnan(x) || isnan(y) || isnan(z)) && !(x == 0.0 && y == 0.0 && z == 0.0);
-    }
-    if (!ok) { x = y = z = 0; }
-    else {
-        if (rot) {      // mocap.rotate: the points turned by Rz Ry Rx before the unit conversion (mocap_interface.py:218-221)
-            const double rx = rot[0] * x + rot[1] * y + rot[2] * z, ry = rot[3] * x + rot[4] * y + rot[5] * z, rz = rot[6] * x + rot[7] * y + rot[8] * z;
-            x = rx; y = ry; z = rz;
-        }
-        x = x / unit_per_metre; y = y / unit_per_metre; z = z / unit_per_metre;
-    }
-    obs[3 * i] = real(x); obs[3 * i + 1] = real(y); obs[3 * i + 2] = real(z);
+    double v[3];
+    const bool ok = mosh2::gather_marker_sample(col >= 0 ? raw + (size_t(f) * frame_step * n_cols + col) * 3 : nullptr,
+                                                unit_per_metre, rot, v);
+    obs[3 * i] = real(v[0]); obs[3 * i + 1] = real(v[1]); obs[3 * i + 2] = real(v[2]);
     vis[i] = ok ? 1 : 0;
 }
 
@@ -417,6 +405,11 @@ struct mosh2_job {
     void *h_raw = nullptr, *d_raw = nullptr;     // raw marker table of mosh2_job_upload_markers (pinned staging, device copy)
     int *d_cols = nullptr;
     size_t raw_bytes = 0;
+    // mosh2_job_upload_markers_range: one staging slot per upload in flight.  A slot holds the table rows, the rotation and
+    // the column map (pinned, and their device copy); `done` is recorded behind the gather kernel that reads them, and a
+    // slot is only refilled once its event has completed, so uploads of several captures can be queued back to back.
+    struct RangeSlot { void *h = nullptr, *d = nullptr; size_t bytes = 0; cudaEvent_t done = nullptr; };
+    std::vector<RangeSlot> range_slots;
     int *h_status = nullptr, *h_counters = nullptr;
     size_t n_obs = 0, n_out = 0;
     size_t o_fullpose = 0, o_pose = 0, o_trans = 0, o_dmpls = 0, o_mk = 0, o_errs = 0;   // element offsets in d_out
@@ -767,6 +760,65 @@ int mosh2_job_upload_markers(mosh2_job *j, const double *markers, int32_t n_file
     return 0;
 }
 
+int mosh2_job_upload_markers_range(mosh2_job *j, int32_t frame0, int32_t nfr, const double *markers, int32_t n_file_frames, int32_t n_cols,
+                                   const int32_t *col_of_marker, int32_t frame_start, int32_t frame_step, double unit_per_metre,
+                                   const double *rot3x3) {
+    if (!j || !markers || !col_of_marker) return fail(MOSH2_E_INVALID, "null argument");
+    if (frame0 < 0 || nfr < 1 || frame0 > j->n_frames - nfr)
+        return fail(MOSH2_E_INVALID, "frame range [%d, %d) outside the job's %d frames", frame0, frame0 + nfr, j->n_frames);
+    const int M = j->model->n_markers;
+    if (n_cols < 1 || frame_step < 1 || frame_start < 0 || !(unit_per_metre > 0) ||
+        size_t(frame_start) + size_t(nfr - 1) * frame_step >= size_t(n_file_frames))
+        return fail(MOSH2_E_INVALID, "frames %d + k*%d (k < %d) do not fit a file of %d frames", frame_start, frame_step, nfr, n_file_frames);
+    for (int i = 0; i < M; ++i)
+        if (col_of_marker[i] >= n_cols) return fail(MOSH2_E_INVALID, "marker %d: column %d of %d", i, col_of_marker[i], n_cols);
+    CU(cudaSetDevice(j->model->device));
+    const int dv = j->model->device;
+    // slot layout: rows [frame_start, last used frame] of the table (all columns) | rotation (9) | column map (M int32)
+    const size_t rows = size_t(nfr - 1) * frame_step + 1, bytes = rows * n_cols * 3 * sizeof(double);
+    const size_t o_cols = bytes + 9 * sizeof(double), total = o_cols + size_t(M) * sizeof(int32_t);
+    mosh2_job::RangeSlot *slot = nullptr, *idle = nullptr;
+    for (auto &s : j->range_slots) {
+        const cudaError_t q = cudaEventQuery(s.done);
+        if (q == cudaErrorNotReady) continue;
+        CU(q);
+        if (s.bytes >= total) { slot = &s; break; }
+        if (!idle) idle = &s;
+    }
+    if (!slot) {
+        if (!idle) {
+            j->range_slots.emplace_back();
+            idle = &j->range_slots.back();
+            CU(cudaEventCreateWithFlags(&idle->done, cudaEventDisableTiming));
+        }
+        slot = idle;
+        g_blocks.put(-1, slot->h); g_blocks.put(dv, slot->d);
+        slot->h = slot->d = nullptr; slot->bytes = 0;
+        CU(g_blocks.get(-1, total, &slot->h));
+        CU(g_blocks.get(dv, total, &slot->d));
+        slot->bytes = total;
+    }
+    char *h = static_cast<char *>(slot->h);
+    memcpy(h, markers + size_t(frame_start) * n_cols * 3, bytes);
+    if (rot3x3) memcpy(h + bytes, rot3x3, 9 * sizeof(double));
+    memcpy(h + o_cols, col_of_marker, size_t(M) * sizeof(int32_t));
+    CU(cudaMemcpyAsync(slot->d, h, total, cudaMemcpyHostToDevice, j->stream));
+    const char *d = static_cast<const char *>(slot->d);
+    const double *d_raw = reinterpret_cast<const double *>(d), *d_rot = rot3x3 ? reinterpret_cast<const double *>(d + bytes) : nullptr;
+    const int *d_cols = reinterpret_cast<const int *>(d + o_cols);
+    const size_t n = size_t(nfr) * M, o0 = size_t(frame0) * M;
+    const int blocks = int((n + 255) / 256);
+    if (j->precision == MOSH2_F64)
+        gather_markers_kernel<double><<<blocks, 256, 0, j->stream>>>(d_raw, n_cols, d_cols, M, nfr, frame_step, unit_per_metre, d_rot,
+                                                                     static_cast<double *>(j->d_obs) + 3 * o0, j->d_vis + o0);
+    else
+        gather_markers_kernel<float><<<blocks, 256, 0, j->stream>>>(d_raw, n_cols, d_cols, M, nfr, frame_step, unit_per_metre, d_rot,
+                                                                    static_cast<float *>(j->d_obs) + 3 * o0, j->d_vis + o0);
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(slot->done, j->stream));
+    return 0;
+}
+
 int mosh2_job_linearize(mosh2_job *j, const mosh2_options *opt, int32_t step, int32_t build, const double *x, const mosh2_lin_out *out) {
     if (!j || !x || !out || (step != 1 && step != 2)) return fail(MOSH2_E_INVALID, "bad argument");
     if (j->n_chunks < j->n_frames) return fail(MOSH2_E_INVALID, "mosh2_job_linearize needs a job of one-frame chunks (chunk_len = 1)");
@@ -992,6 +1044,11 @@ void mosh2_job_destroy(mosh2_job *j) {
     g_blocks.put(dv, j->d_cols);
     for (void *p : {j->h_obs, j->h_out, static_cast<void *>(j->h_vis), static_cast<void *>(j->h_status), static_cast<void *>(j->h_counters), j->h_raw})
         g_blocks.put(-1, p);
+    for (auto &s : j->range_slots) {        // (the stream is idle: every slot's copy and kernel have finished)
+        g_blocks.put(-1, s.h);
+        g_blocks.put(dv, s.d);
+        if (s.done) cudaEventDestroy(s.done);
+    }
     if (j->ev0) cudaEventDestroy(j->ev0);
     if (j->ev1) cudaEventDestroy(j->ev1);
     if (j->ev_in) cudaEventDestroy(j->ev_in);

@@ -67,6 +67,29 @@ inline unsigned char *m2_smem() { return m2_smem_ref(); }
 #endif
 constexpr unsigned kSmemHeader = 16;     // first bytes of the dynamic shared memory: base of the per-CTA global workspace
 
+// One sample of the mocap input adapter (mosh2.cu gather_markers_kernel; tools/mocap_interface.py:186,223-225,254-279):
+// `p` the sample's xyz in file units, or NULL when the file has no column for the marker.  A sample is missing when a
+// coordinate is NaN or all three are exactly zero (:277); a missing sample comes out as zero.  Otherwise it is turned by
+// `rot` (row-major Rz Ry Rx, mocap.rotate, may be NULL) and converted to metres.  Returns the visibility.
+M2_HD bool gather_marker_sample(const double *p, double unit_per_metre, const double *rot, double out[3]) {
+    double x = 0, y = 0, z = 0;
+    bool ok = false;
+    if (p) {
+        x = p[0]; y = p[1]; z = p[2];
+        ok = !(isnan(x) || isnan(y) || isnan(z)) && !(x == 0.0 && y == 0.0 && z == 0.0);
+    }
+    if (!ok) { x = y = z = 0; }
+    else {
+        if (rot) {      // the points turned before the unit conversion (mocap_interface.py:218-221)
+            const double rx = rot[0] * x + rot[1] * y + rot[2] * z, ry = rot[3] * x + rot[4] * y + rot[5] * z, rz = rot[6] * x + rot[7] * y + rot[8] * z;
+            x = rx; y = ry; z = rz;
+        }
+        x = x / unit_per_metre; y = y / unit_per_metre; z = z / unit_per_metre;
+    }
+    out[0] = x; out[1] = y; out[2] = z;
+    return ok;
+}
+
 template <class T>
 struct SPtr {                            // array in shared memory
     uint32_t ofs;

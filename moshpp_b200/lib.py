@@ -13,7 +13,7 @@ import numpy as np
 
 from .pack import StageIIPack
 
-ABI_VERSION = 104          # MOSH2_VERSION of include/mosh2.h that the ctypes structs below encode
+ABI_VERSION = 105          # MOSH2_VERSION of include/mosh2.h that the ctypes structs below encode
 MOSH2_F32, MOSH2_F64 = 0, 1
 ST_SOLVED, ST_SKIPPED, ST_HAS_VELO, ST_HAS_EXTRAP, ST_GN_FALLBACK, ST_MAXITER, ST_SHORT_WARMUP = 1, 2, 4, 8, 16, 32, 64
 ERR_NAMES = ('data', 'poseB', 'velo', 'poseH', 'dmpl', 'extrap_dmpl', 'poseF', 'expr')   # column order of mosh2_result.errs
@@ -119,6 +119,8 @@ def load_library(path: Optional[str] = None):
     lib.mosh2_job_upload.argtypes = [vp, _f64p, _u8p]
     lib.mosh2_job_linearize.argtypes = [vp, C.POINTER(Options), C.c_int32, C.c_int32, _f64p, C.POINTER(LinOut)]
     lib.mosh2_job_upload_markers.argtypes = [vp, _f64p, C.c_int32, C.c_int32, _i32p, C.c_int32, C.c_int32, C.c_double, _f64p]
+    lib.mosh2_job_upload_markers_range.argtypes = [vp, C.c_int32, C.c_int32, _f64p, C.c_int32, C.c_int32, _i32p, C.c_int32, C.c_int32,
+                                                   C.c_double, _f64p]
     lib.mosh2_job_upload_device_range.argtypes = [vp, C.c_int32, C.c_int32, vp, C.c_int32, vp, vp]
     lib.mosh2_job_upload_device.argtypes = [vp, vp, C.c_int32, vp, vp]
     lib.mosh2_job_row_width.argtypes = [vp]
@@ -150,7 +152,7 @@ EXPORTED_SYMBOLS = (
     'mosh2_solve', 'mosh2_job_upload_device', 'mosh2_job_row_width', 'mosh2_job_download_device', 'mosh2_job_span_ms',
     'mosh2_job_create_batch', 'mosh2_job_upload_device_range', 'mosh2_job_warm_states', 'mosh2_job_relaunch_chunks',
     'mosh2_job_boundary_deltas', 'mosh2_release_cached_memory', 'mosh2_mesh_distance', 'mosh2_job_upload_markers', 'mosh2_job_linearize',
-    'mosh2_job_chunk_ranges')
+    'mosh2_job_chunk_ranges', 'mosh2_job_upload_markers_range')
 
 
 def _ptr(a: np.ndarray, typ):
@@ -323,6 +325,20 @@ class Job:
         self.model._check(self.lib.mosh2_job_upload_markers(self.handle, _ptr(raw, _f64p), raw.shape[0], raw.shape[1], _ptr(cols, _i32p),
                                                             int(frame_start), int(frame_step), float(unit_per_metre),
                                                             _ptr(rot, _f64p) if rot is not None else None), 'mosh2_job_upload_markers')
+
+    def upload_markers_range(self, frame0: int, n: int, raw: np.ndarray, col_of_marker, frame_start: int, frame_step: int,
+                             unit_per_metre: float, rot3x3=None):
+        """``upload_markers`` for frames [frame0, frame0 + n) of the job's frame axis: one capture of a batch job
+        (mosh2_job_upload_markers_range).  The library stages the rows it needs before it returns, so the uploads of all
+        captures can be issued back to back."""
+        raw = np.ascontiguousarray(raw, dtype=np.float64)
+        cols = np.ascontiguousarray(col_of_marker, dtype=np.int32)
+        assert raw.ndim == 3 and raw.shape[2] == 3 and cols.shape == (self.model.pk.n_markers,)
+        rot = None if rot3x3 is None else np.ascontiguousarray(rot3x3, dtype=np.float64).reshape(3, 3)
+        self.model._check(self.lib.mosh2_job_upload_markers_range(self.handle, int(frame0), int(n), _ptr(raw, _f64p), raw.shape[0],
+                                                                  raw.shape[1], _ptr(cols, _i32p), int(frame_start), int(frame_step),
+                                                                  float(unit_per_metre), _ptr(rot, _f64p) if rot is not None else None),
+                          'mosh2_job_upload_markers_range')
 
     def linearize(self, x: np.ndarray, options: Options, step: int, build: bool) -> Dict[str, np.ndarray]:
         """mosh2_job_linearize: every frame of the job evaluated (and, with ``build``, linearised) at its row of ``x``

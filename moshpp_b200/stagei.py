@@ -93,6 +93,20 @@ def load_marker_layout(marker_layout_fname: str, labels_map='general', exclude_m
             'surface_model_type': d.get('surface_model_type', 'smplx'), 'marker_layout_fname': marker_layout_fname}
 
 
+def write_marker_layout(fname: str, marker_meta: dict) -> str:
+    """The marker layout json the reference's Stage I reads (marker_layout/edit_tools.py:115-160) from a ``marker_meta``
+    (``marker_layout_write`` without the colours and the viewer files)."""
+    import json
+    sets = []
+    for t, mask in marker_meta['marker_type_mask'].items():
+        labels = [l for l, m in zip(marker_meta['marker_vids'].keys(), np.asarray(mask, dtype=bool)) if m]
+        sets.append({'type': t, 'distance_from_skin': float(marker_meta['m2b_distance'][t]),
+                     'indices': {l: int(marker_meta['marker_vids'][l]) for l in labels}})
+    with open(fname, 'w') as f:
+        json.dump({'surface_model_type': marker_meta['surface_model_type'], 'markersets': sets}, f)
+    return fname
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # small host-side geometry (float64 numpy, O(markers))
 # ---------------------------------------------------------------------------------------------------------------------

@@ -658,14 +658,22 @@ def make_case(out_dir: str, config: str = 'C2', *, frames: Optional[int] = None,
                 gt_markers=mk, obs=obs, vis=vis, model=model, config=c)
 
 
-def write_marker_layout(fname: str, marker_meta: Dict) -> str:
-    """The marker layout json the reference's Stage I reads (marker_layout/edit_tools.py:115-160) from a ``marker_meta``."""
-    import json
-    sets = []
-    for t, mask in marker_meta['marker_type_mask'].items():
-        labels = [l for l, m in zip(marker_meta['marker_vids'].keys(), np.asarray(mask, dtype=bool)) if m]
-        sets.append({'type': t, 'distance_from_skin': float(marker_meta['m2b_distance'][t]),
-                     'indices': {l: int(marker_meta['marker_vids'][l]) for l in labels}})
-    with open(fname, 'w') as f:
-        json.dump({'surface_model_type': marker_meta['surface_model_type'], 'markersets': sets}, f)
-    return fname
+from .stagei import write_marker_layout  # noqa: E402,F401  (re-exported: the fixtures write their layouts with it)
+
+
+def make_subject(out_dir: str, config: str = 'C2', frames=(1000, 2000), **kw):
+    """Several captures of ONE synthetic subject (one shape, one set of latent markers): a case of ``sum(frames)`` frames
+    (``make_case``, npz configurations) whose capture file is cut into consecutive captures of ``frames[k]`` frames.
+    Returns (the case, the capture file names)."""
+    case = make_case(out_dir, config, frames=int(sum(frames)), **kw)
+    if not case['mocap_fname'].endswith('.npz'):
+        raise ValueError(f'{config}: make_subject cuts npz captures only')
+    z = np.load(case['mocap_fname'])
+    stem = os.path.splitext(case['mocap_fname'])[0]
+    fnames, f0 = [], 0
+    for k, F in enumerate(frames):
+        fn = f'{stem}_take{k:02d}_{int(F)}.npz'
+        np.savez(fn, markers=z['markers'][f0:f0 + int(F)], labels=z['labels'], frame_rate=z['frame_rate'])
+        fnames.append(fn)
+        f0 += int(F)
+    return case, fnames
