@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MOSH2_VERSION 105
+#define MOSH2_VERSION 106
 
 enum {
     MOSH2_OK = 0,
@@ -148,6 +148,16 @@ int mosh2_job_create(mosh2_model *m, const mosh2_options *opt, int32_t n_frames,
  * from its own cold start.  All per-frame buffers (obs, vis, results) are indexed by the concatenated frame axis. */
 int mosh2_job_create_batch(mosh2_model *m, const mosh2_options *opt, int32_t n_seq, const int32_t *frame_counts,
                            const mosh2_schedule *sched, int32_t precision, mosh2_job **out);
+/* The same for sequences of SEVERAL subjects: sequence q is solved with models[model_of_seq[q]].  The frame axis and every
+ * other job call are as for mosh2_job_create_batch (mosh2_job_linearize refuses a multi-model job).  All models must be on one
+ * device and have the same kernel shape -- equal n_joints, n_markers, body_dof, p_red, n_hand_red, n_hand_full, n_dmpl, kw,
+ * n_free1, n_free2, finger range, face range, n_expr, n_jangles, prior_k, prior_d and hand-block structure of hand_comps --
+ * so that one workspace plan serves the whole launch; their tables (shape, latent markers, attachment, prior, ...) may
+ * differ, e.g. the male and female model of one family.  A mismatch returns MOSH2_E_INVALID and mosh2_last_error names the
+ * first field that differs.  The models must outlive the job (as the model of any job must). */
+int mosh2_job_create_multi(mosh2_model *const *models, int32_t n_models, const mosh2_options *opt, int32_t n_seq,
+                           const int32_t *frame_counts, const int32_t *model_of_seq, const mosh2_schedule *sched,
+                           int32_t precision, mosh2_job **out);
 /* obs [F*M*3] metres in latent-label order, vis [F*M] 0/1.  Async on the job's stream. */
 int mosh2_job_upload(mosh2_job *j, const double *obs, const uint8_t *vis);
 /* Mocap input adapter on the device -- what the reference does per frame in Python between the capture file and the frame

@@ -709,3 +709,174 @@ def mosh_stageii_batch(mocap_fnames, cfg, markers_latent: np.ndarray, latent_lab
     if n_fb:
         logger.warning('%d frames hit a non-positive-definite Gauss-Newton system (Cauchy step used)', n_fb)
     return out
+
+
+def kernel_shape_key(pk) -> tuple:
+    """What two packs must share to be solved by one multi-model launch (mosh2_job_create_multi): sizes, free-variable
+    counts, finger / face / joint-angle ranges, prior size and the hand-block structure of the hand-PCA matrix (the non-zero
+    column range of every row).  The tables themselves may differ."""
+    hc = np.asarray(pk.hand_comps).reshape(pk.n_hand_red, pk.n_hand_full) if pk.n_hand_red else np.zeros((0, 0))
+    rows = []
+    for r in hc:
+        nz = np.flatnonzero(r)
+        rows.append((int(nz[0]), int(nz[-1]) + 1) if len(nz) else (0, 0))
+    return (pk.n_joints, pk.n_markers, pk.body_dof, pk.p_red, pk.n_hand_red, pk.n_hand_full, pk.n_dmpl, pk.kw, len(pk.free_step1),
+            len(pk.free_step2), pk.finger_lo, pk.finger_hi, pk.n_expr, pk.face_lo, pk.face_hi, len(getattr(pk, 'jangles_ids', ())),
+            pk.prior_k, pk.prior_d, tuple(rows))
+
+
+def subject_launch_key(pk, opts, mode: str = 'fast') -> tuple:
+    """Subjects with equal keys share a launch of ``mosh_stageii_subjects``: one kernel shape (``kernel_shape_key``), equal
+    ``mosh2_options`` and the same default schedule (``default_schedule``: precision, warm-up, boundary tolerance)."""
+    return (kernel_shape_key(pk), tuple(getattr(opts, f) for f, _ in opts._fields_), default_schedule(pk.model_type, mode, pk.n_dmpl))
+
+
+def launch_groups(keys) -> list:
+    """Subjects (by their ``subject_launch_key``) that share a launch: lists of subject indices, in the order of first
+    appearance."""
+    groups = {}
+    for i, k in enumerate(keys):
+        groups.setdefault(k, []).append(i)
+    return list(groups.values())
+
+
+def mosh_stageii_subjects(subjects, *, device: int = 0, mode: str = 'fast', chunk_len: Optional[int] = None,
+                          chunk_warmup: Optional[int] = None, warmup_full: Optional[int] = None, first_extra: Optional[int] = None,
+                          precision: Optional[str] = None, verify: bool = True, boundary_tol=None, sm_budget: int = NUM_SMS,
+                          labels_map='general', device_adapter: bool = True) -> list:
+    """Stage II of the captures of SEVERAL subjects, with as few launches as their models allow.
+
+    ``subjects``: dictionaries with ``cfg``, ``mocap_fnames`` and the subject's Stage-I outputs ``markers_latent``,
+    ``latent_labels``, ``betas``, ``marker_meta`` and (optional) ``v_template_fname``.  Returns one list per subject with one
+    dictionary per capture: what ``mosh_stageii_batch`` returns for that subject with the same keyword arguments, except
+    ``stageii_debug_details['b200']`` and, in the planned (``chunk_len=None``) schedule, the chunk length, which is planned over
+    all frame counts of the launch.
+
+    Every subject's pack and device model come from the subject cache (``subject_for``).  Subjects whose packs have one kernel
+    shape (``kernel_shape_key``) and whose ``mosh2_options`` and default schedule (``default_schedule``: precision, warm-up,
+    boundary tolerance) are equal share one multi-model job (mosh2_job_create_multi) and one verified launch
+    (``launch_verified``); e.g. male and female SMPL-H subjects share a launch, a DMPL subject (float64 exact preset) does not
+    share one with float32 SMPL-H subjects.  ``b200['batch']`` holds the figures of the capture's launch, marked
+    ``'shared': True``, and ``'launches'``, the number of launches of the call."""
+    global SUBJECT_CACHE_SIZE
+    t0 = time.time()
+    if mode not in BOUNDARY_TOL:
+        raise ValueError(f"mode must be 'fast' or 'exact', not {mode!r}")
+    subjects = list(subjects)
+    bound = SUBJECT_CACHE_SIZE
+    SUBJECT_CACHE_SIZE = max(bound, len(subjects))      # (every model of the call stays open until its launch is done)
+    try:
+        subs = []
+        for s in subjects:
+            cfg = s['cfg']
+            fnames = list(s['mocap_fnames'])
+            if not fnames:
+                raise ValueError('a subject without captures')
+            only = [cfg.mocap.subject_name] if cfg.mocap.multi_subject else None
+            seqs = []
+            for fn in fnames:
+                mocap = MocapSession(fn, mocap_unit=cfg.mocap.unit, mocap_rotate=cfg.mocap.rotate, labels_map=labels_map, only_subjects=only)
+                sel, raw_cols, obs, vis, F = _select_input(mocap, cfg, s['latent_labels'], device_adapter)
+                seqs.append(dict(fname=fn, mocap=mocap, sel=sel, raw_cols=raw_cols, obs=obs, vis=vis, F=F))
+            pk, opts, flags, model, cache_hit = subject_for(cfg, s['markers_latent'], s['latent_labels'], s['betas'], s['marker_meta'],
+                                                            s.get('v_template_fname'), device)
+            key = subject_launch_key(pk, opts, mode)
+            subs.append(dict(cfg=cfg, seqs=seqs, pk=pk, opts=opts, flags=flags, model=model, cache_hit=cache_hit, sched=key[2],
+                             key=key, labels=list(s['latent_labels'])))
+        groups = launch_groups([s['key'] for s in subs])
+        out = [None] * len(subs)
+        for g, members in enumerate(groups):
+            _solve_subject_group([subs[i] for i in members], g, len(groups), t0, chunk_len, chunk_warmup, warmup_full,
+                                 first_extra, precision, verify, boundary_tol, sm_budget, mode)
+            for i in members:
+                out[i] = subs[i]['out']
+    finally:
+        SUBJECT_CACHE_SIZE = bound
+        while len(_SUBJECT_CACHE) > SUBJECT_CACHE_SIZE:
+            _, old = _SUBJECT_CACHE.popitem(last=False)
+            old['model'].close()
+    return out
+
+
+def _solve_subject_group(group, g, n_groups, t0, chunk_len, chunk_warmup, warmup_full, first_extra, precision, verify,
+                         boundary_tol, sm_budget, mode):
+    """One launch of ``mosh_stageii_subjects``: the captures of the subjects of ``group`` back to back on one multi-model job;
+    sets every member's ``'out'``."""
+    w_def, wf_def, prec_def, tol_def = group[0]['sched']
+    chunk_warmup = w_def if chunk_warmup is None else int(chunk_warmup)
+    warmup_full = (wf_def if chunk_warmup == w_def else -1) if warmup_full is None else int(warmup_full)
+    precision = precision or prec_def
+    if boundary_tol is None:
+        boundary_tol = tol_def
+    seqs = [(k, s) for k, sub in enumerate(group) for s in sub['seqs']]
+    counts = [s['F'] for _, s in seqs]
+    if first_extra is None:
+        first_extra = first_chunk_extra(chunk_warmup, warmup_full)
+    if chunk_len is None:
+        chunk_len = plan_chunk_len(counts, sm_budget, chunk_warmup, warmup_full if warmup_full >= 0 else chunk_warmup,
+                                   first_extra=first_extra)
+    if chunk_len >= max(counts):
+        chunk_len = 0
+    prec = {'f32': _lib.MOSH2_F32, 'f64': _lib.MOSH2_F64}[precision]
+    pk0 = group[0]['pk']
+    job = _lib.multi_job([sub['model'] for sub in group], [k for k, _ in seqs], counts, group[0]['opts'], chunk_len=chunk_len,
+                         chunk_warmup=chunk_warmup, warmup_full=warmup_full, first_extra=first_extra, precision=prec)
+    try:
+        offsets = job.seq_offsets
+        if any(s['raw_cols'] is None for _, s in seqs):
+            # host-adapter captures: one upload of the whole frame axis; the device-adapter ranges are written over it
+            obs = np.zeros((job.n_frames, pk0.n_markers, 3))
+            vis = np.zeros((job.n_frames, pk0.n_markers), dtype=bool)
+            for q, (_, s) in enumerate(seqs):
+                if s['raw_cols'] is None:
+                    obs[offsets[q]:offsets[q + 1]], vis[offsets[q]:offsets[q + 1]] = s['obs'], s['vis']
+            job.upload(obs, vis)
+        for q, (k, s) in enumerate(seqs):          # issued back to back: every call stages its own rows
+            if s['raw_cols'] is not None:
+                rot = group[k]['cfg'].mocap.rotate
+                m = s['mocap']
+                job.upload_markers_range(int(offsets[q]), s['F'], m.raw, s['raw_cols'], s['sel'].start, s['sel'].step,
+                                         m.unit_per_metre, None if rot is None else _rotation_xyz(rot))
+
+        def host_side():                            # the result-independent half of every output, behind the solve
+            for k, s in seqs:
+                if s['raw_cols'] is not None:
+                    s['obs'], s['vis'] = s['mocap'].frames_for_labels(group[k]['labels'], s['sel'])
+                s['lists'] = observation_lists(s['obs'], s['vis'], group[k]['labels'])
+                s['markers_orig'] = s['mocap'].markers[s['sel']]
+
+        bad, report = launch_verified(job, boundary_tol if verify else None, while_running=host_side)
+        res = download_verified(job, bad, report)
+        kernel_ms = float(sum(report['kernel_ms']))
+        n_chunks = job.num_chunks
+        totals = job.totals()
+    finally:
+        job.close()
+
+    batch = {'shared': True, 'launch': g, 'launches': n_groups, 'subjects': len(group), 'captures': len(seqs),
+             'frames': int(sum(counts)), 'kernel_ms': kernel_ms, 'wall_s': time.time() - t0, 'chunks': n_chunks, 'chunk_len': chunk_len,
+             'chunk_warmup': chunk_warmup, 'warmup_full': warmup_full, 'first_extra': first_extra, 'precision': precision, 'mode': mode,
+             'boundary_check': report, 'totals': totals, 'subject_cache_hits': [sub['cache_hit'] for sub in group]}
+    for sub in group:
+        sub['out'] = []
+    for q, (k, s) in enumerate(seqs):
+        sub = group[k]
+        r = _SeqResult(res, int(offsets[q]), int(offsets[q + 1]))
+        data = assemble_stageii_data(r, s['obs'], s['vis'], sub['labels'], sub['pk'], sub['flags'], bool(sub['opts'].optimize_dynamics),
+                                     s.get('lists'))
+        m = s['mocap']
+        solved = (r.status & _lib.ST_SOLVED) != 0
+        data['stageii_debug_details'].update({
+            'markers_orig': s['markers_orig'] if 'markers_orig' in s else m.markers[s['sel']],
+            'labels_orig': m.labels,
+            'mocap_fname': s['fname'],
+            'mocap_frame_rate': m.frame_rate,
+            'mocap_time_length': m.time_length(),
+            'b200': {'batch': batch, 'batch_index': q, 'subject_index': k, 'frame_offset': int(offsets[q]),
+                     'device_adapter': s['raw_cols'] is not None, 'status': r.status.copy(), 'counters': r.counters.copy(),
+                     'pose_reduced': r.pose[solved], 'frame_ids': np.nonzero(solved)[0]},
+        })
+        sub['out'].append(data)
+    n_fb = int(((res.status & _lib.ST_GN_FALLBACK) != 0).sum())
+    if n_fb:
+        logger.warning('%d frames hit a non-positive-definite Gauss-Newton system (Cauchy step used)', n_fb)

@@ -129,6 +129,30 @@ mosh2_stageii_kernel(const __grid_constant__ mosh2::Model<real> m, const __grid_
     s.run_chunk(job.chunk_ids ? job.chunk_ids[blockIdx.x] : int(blockIdx.x));
 }
 
+// The same for a multi-model job (mosh2_job_create_multi): the sequences of the launch belong to subjects with models of one
+// kernel shape, so `w` and `d` serve every chunk.  The block copies its chunk's Model record from the device array `models`
+// into the shared-memory header (mosh2_host::multi_smem_header, behind the global-workspace base) and binds its Solver to
+// that copy; the Solver stages that model's tables (Model::stage_blob) as in the single-model kernel.
+template <class real, bool BIG>
+__global__ void __launch_bounds__(threads_for<real>(), 1)
+mosh2_stageii_multi_kernel(const mosh2::Model<real> *__restrict__ models, const int *__restrict__ model_of_chunk,
+                           const __grid_constant__ mosh2::Job<real> job, const __grid_constant__ mosh2::Work<real, BIG> w,
+                           const __grid_constant__ mosh2::Dims d) {
+    static_assert(sizeof(mosh2::Model<real>) % 8 == 0, "the Model record is copied in 8-byte words");
+    const int chunk = job.chunk_ids ? job.chunk_ids[blockIdx.x] : int(blockIdx.x);
+    mosh2::Model<real> *rec = reinterpret_cast<mosh2::Model<real> *>(mosh2::m2_smem() + mosh2::kSmemHeader);
+    {
+        const unsigned long long *src = reinterpret_cast<const unsigned long long *>(models + model_of_chunk[chunk]);
+        unsigned long long *dst = reinterpret_cast<unsigned long long *>(rec);
+        for (int i = threadIdx.x; i < int(sizeof(mosh2::Model<real>) / 8); i += blockDim.x) dst[i] = src[i];
+    }
+    if (BIG && threadIdx.x == 0) *reinterpret_cast<char **>(mosh2::m2_smem()) = job.gws + size_t(blockIdx.x) * job.gws_stride;
+    __syncthreads();
+    mosh2::Cta c{int(threadIdx.x), int(blockDim.x)};
+    mosh2::Solver<real, BIG> s(*rec, job, w, d, c);
+    s.run_chunk(chunk);
+}
+
 // device copy of every model array in one precision
 template <class real>
 struct DevModel {
@@ -411,6 +435,13 @@ struct mosh2_job {
     struct RangeSlot { void *h = nullptr, *d = nullptr; size_t bytes = 0; cudaEvent_t done = nullptr; };
     std::vector<RangeSlot> range_slots;
     int *h_status = nullptr, *h_counters = nullptr;
+    // multi-model job (mosh2_job_create_multi; `model` is models[0]): the Model records of the job's precision as the kernel
+    // reads them (host copy, whose first record also carries the job's workspace plan, and device array), and the model
+    // index of every chunk -- an array of its own, the chunk records are rewritten in place by mosh2_job_relaunch_chunks
+    std::vector<mosh2_model *> models;
+    std::vector<unsigned char> h_models;
+    void *d_models = nullptr;
+    int *d_model_of_chunk = nullptr;
     size_t n_obs = 0, n_out = 0;
     size_t o_fullpose = 0, o_pose = 0, o_trans = 0, o_dmpls = 0, o_mk = 0, o_errs = 0;   // element offsets in d_out
 };
@@ -427,6 +458,21 @@ cudaError_t launch_kernel(mosh2_job *j, const mosh2::Model<real> &m, const mosh2
     const cudaError_t e = cudaFuncSetAttribute(mosh2_stageii_kernel<real, BIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(j->smem));
     if (e != cudaSuccess) return e;
     mosh2_stageii_kernel<real, BIG><<<j->launch_blocks, threads, j->smem, j->stream>>>(m, job, w, d);
+    return cudaGetLastError();
+}
+
+template <class real, bool BIG>
+cudaError_t launch_multi_kernel(mosh2_job *j, const mosh2::Job<real> &job, int threads) {
+    const mosh2::Model<real> &m = *reinterpret_cast<const mosh2::Model<real> *>(j->h_models.data());
+    const mosh2::Dims d = mosh2::make_dims(m);
+    mosh2::Work<real, BIG> w{};
+    mosh2::Arena S{mosh2_host::multi_smem_header<real>()}, G{0};
+    mosh2::carve<real, BIG>(w, d, m, S, G);
+    w.tc = (w.tc_ok && threads >= 128) ? 1 : 0;
+    const cudaError_t e = cudaFuncSetAttribute(mosh2_stageii_multi_kernel<real, BIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(j->smem));
+    if (e != cudaSuccess) return e;
+    mosh2_stageii_multi_kernel<real, BIG><<<j->launch_blocks, threads, j->smem, j->stream>>>(
+        static_cast<const mosh2::Model<real> *>(j->d_models), j->d_model_of_chunk, job, w, d);
     return cudaGetLastError();
 }
 
@@ -463,7 +509,10 @@ int launch(mosh2_job *j, const mosh2::Model<real> &m) {
         if (t >= 128 && t <= threads && t % 32 == 0) threads = t;
     }
     CU(cudaEventRecord(j->ev0, j->stream));
-    if (j->big_in_global) CU((launch_kernel<real, true>(j, m, job, threads)));
+    if (j->d_models) {
+        if (j->big_in_global) CU((launch_multi_kernel<real, true>(j, job, threads)));
+        else CU((launch_multi_kernel<real, false>(j, job, threads)));
+    } else if (j->big_in_global) CU((launch_kernel<real, true>(j, m, job, threads)));
     else CU((launch_kernel<real, false>(j, m, job, threads)));
     CU(cudaGetLastError());
     CU(cudaEventRecord(j->ev1, j->stream));
@@ -471,9 +520,10 @@ int launch(mosh2_job *j, const mosh2::Model<real> &m) {
 }
 
 template <class real>
-void plan_workspace(mosh2::Model<real> &m, size_t *smem, size_t *gws, int *big) {
+void plan_workspace(mosh2::Model<real> &m, size_t *smem, size_t *gws, int *big, unsigned header = mosh2::kSmemHeader) {
     // preference order: 20-marker tiles, then 10-marker tiles, while the workspace fits the shared-memory budget; the
-    // f64 / oversized case moves A, its factor and the Jacobian tiles to a per-CTA global workspace
+    // f64 / oversized case moves A, its factor and the Jacobian tiles to a per-CTA global workspace.  `header`: bytes in
+    // front of the workspace (a multi-model job keeps the chunk's Model record there)
     const int tries[3][2] = {{20, 0}, {10, 0}, {10, 1}};   // markers per tile (a warp owns ten), big
     const char *dev_tile = getenv("MOSH2_DEV_TILE");      // development aid: 10 = skip the 20-marker tile
     const bool dev_big = getenv("MOSH2_DEV_BIG") != nullptr;   // development aid: force the global-workspace layout
@@ -482,7 +532,7 @@ void plan_workspace(mosh2::Model<real> &m, size_t *smem, size_t *gws, int *big) 
         m.dev_no_tc = getenv("MOSH2_DEV_NO_TC") ? 1 : 0;      // development aid: J^T J on the CUDA cores
         const bool in_global = tries[pass][1] != 0;
         const mosh2::Dims d = mosh2::make_dims(m);
-        mosh2::Arena S{mosh2::kSmemHeader}, G{0};
+        mosh2::Arena S{header}, G{0};
         if (in_global) { mosh2::Work<real, true> w{}; mosh2::carve<real, true>(w, d, m, S, G); }
         else { mosh2::Work<real, false> w{}; mosh2::carve<real, false>(w, d, m, S, G); }
         *big = in_global ? 1 : 0;
@@ -706,6 +756,87 @@ int mosh2_job_create_batch(mosh2_model *m, const mosh2_options *opt, int32_t n_s
     return 0;
 }
 
+}  // extern "C"
+
+namespace {
+
+// mosh2_job_create_multi in the job's compute type, on a batch job `j` of models[0]: the shape check, the workspace plan
+// with the Model record in the shared-memory header, and the device arrays of Model records and chunk -> model indices
+template <class real>
+int make_multi(mosh2_job *j, mosh2_model *const *models, int32_t n_models, int32_t n_seq, const int32_t *frame_counts,
+               const int32_t *model_of_seq) {
+    auto dev_model = [](mosh2_model *mm) -> mosh2::Model<real> & {
+        if constexpr (sizeof(real) == 8) return mm->f64.m; else return mm->f32.m;
+    };
+    mosh2::Model<real> plan = dev_model(models[0]);
+    size_t smem = 0, gws = 0;
+    int big = 0;
+    plan_workspace(plan, &smem, &gws, &big, mosh2_host::multi_smem_header<real>());
+    if (smem > kMaxSmem) return fail(MOSH2_E_TOO_LARGE, "model needs %zu bytes of shared memory per block (max %zu)", smem, kMaxSmem);
+    const int dv = j->model->device;
+    const size_t stride = big ? gws : 0;
+    if (stride > j->gws_stride) {
+        g_blocks.put(dv, j->d_gws);
+        j->d_gws = nullptr;
+        CU(g_blocks.get(dv, stride * j->n_chunks, &j->d_gws));
+    }
+    j->smem = smem; j->big_in_global = big; j->gws_stride = stride;
+    std::vector<mosh2::Model<real>> recs(n_models);
+    for (int k = 0; k < n_models; ++k) {
+        recs[k] = dev_model(models[k]);
+        recs[k].tile_markers = plan.tile_markers;
+        recs[k].dev_no_tc = plan.dev_no_tc;
+    }
+    j->h_models.assign(reinterpret_cast<const unsigned char *>(recs.data()), reinterpret_cast<const unsigned char *>(recs.data() + n_models));
+    const std::vector<int> moc = mosh2_host::model_of_chunks(j->tab0, frame_counts, n_seq, model_of_seq);
+    CU(g_blocks.get(dv, j->h_models.size(), &j->d_models));
+    CU(g_blocks.get(dv, moc.size() * sizeof(int), reinterpret_cast<void **>(&j->d_model_of_chunk)));
+    CU(cudaMemcpy(j->d_models, j->h_models.data(), j->h_models.size(), cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(j->d_model_of_chunk, moc.data(), moc.size() * sizeof(int), cudaMemcpyHostToDevice));
+    j->models.assign(models, models + n_models);
+    return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int mosh2_job_create_multi(mosh2_model *const *models, int32_t n_models, const mosh2_options *opt, int32_t n_seq,
+                           const int32_t *frame_counts, const int32_t *model_of_seq, const mosh2_schedule *sched,
+                           int32_t precision, mosh2_job **out) {
+    if (!models || n_models < 1 || !opt || !out || n_seq < 1 || !frame_counts || !model_of_seq) return fail(MOSH2_E_INVALID, "bad argument");
+    if (precision != MOSH2_F32 && precision != MOSH2_F64) return fail(MOSH2_E_INVALID, "precision must be MOSH2_F32 or MOSH2_F64");
+    *out = nullptr;
+    for (int k = 0; k < n_models; ++k) {
+        if (!models[k]) return fail(MOSH2_E_INVALID, "model %d is NULL", k);
+        if (models[k]->device != models[0]->device)
+            return fail(MOSH2_E_INVALID, "model %d is on device %d, model 0 on device %d", k, models[k]->device, models[0]->device);
+    }
+    for (int q = 0; q < n_seq; ++q)
+        if (model_of_seq[q] < 0 || model_of_seq[q] >= n_models)
+            return fail(MOSH2_E_INVALID, "sequence %d refers to model %d of %d", q, model_of_seq[q], n_models);
+    CU(cudaSetDevice(models[0]->device));
+    for (int k = 0; k < n_models; ++k)
+        if (const int rc = models[k]->ensure(precision)) return rc;
+    for (int k = 1; k < n_models; ++k) {
+        const char *field = precision == MOSH2_F64 ? mosh2_host::kernel_shape_mismatch(models[0]->f64.m, models[k]->f64.m)
+                                                   : mosh2_host::kernel_shape_mismatch(models[0]->f32.m, models[k]->f32.m);
+        if (field) return fail(MOSH2_E_INVALID, "model %d does not have the kernel shape of model 0: %s differs", k, field);
+    }
+    mosh2_job *j = nullptr;
+    if (const int rc = mosh2_job_create_batch(models[0], opt, n_seq, frame_counts, sched, precision, &j)) return rc;
+    const int rc = precision == MOSH2_F64 ? make_multi<double>(j, models, n_models, n_seq, frame_counts, model_of_seq)
+                                          : make_multi<float>(j, models, n_models, n_seq, frame_counts, model_of_seq);
+    if (rc) {
+        const std::string msg = g_err;
+        mosh2_job_destroy(j);
+        g_err = msg;
+        return rc;
+    }
+    *out = j;
+    return 0;
+}
+
 int mosh2_job_upload(mosh2_job *j, const double *obs, const uint8_t *vis) {
     if (!j || !obs || !vis) return fail(MOSH2_E_INVALID, "null argument");
     CU(cudaSetDevice(j->model->device));
@@ -822,6 +953,7 @@ int mosh2_job_upload_markers_range(mosh2_job *j, int32_t frame0, int32_t nfr, co
 int mosh2_job_linearize(mosh2_job *j, const mosh2_options *opt, int32_t step, int32_t build, const double *x, const mosh2_lin_out *out) {
     if (!j || !x || !out || (step != 1 && step != 2)) return fail(MOSH2_E_INVALID, "bad argument");
     if (j->n_chunks < j->n_frames) return fail(MOSH2_E_INVALID, "mosh2_job_linearize needs a job of one-frame chunks (chunk_len = 1)");
+    if (j->d_models) return fail(MOSH2_E_INVALID, "mosh2_job_linearize does not take a multi-model job");
     CU(cudaSetDevice(j->model->device));
     if (opt) {      // the weights of this evaluation (Stage I anneals them between minimisations)
         mosh2::Options &o = j->opt;
@@ -1042,6 +1174,8 @@ void mosh2_job_destroy(mosh2_job *j) {
     g_blocks.put(dv, j->d_raw);
     g_blocks.put(dv, j->d_lin);
     g_blocks.put(dv, j->d_cols);
+    g_blocks.put(dv, j->d_models);
+    g_blocks.put(dv, j->d_model_of_chunk);
     for (void *p : {j->h_obs, j->h_out, static_cast<void *>(j->h_vis), static_cast<void *>(j->h_status), static_cast<void *>(j->h_counters), j->h_raw})
         g_blocks.put(-1, p);
     for (auto &s : j->range_slots) {        // (the stream is idle: every slot's copy and kernel have finished)

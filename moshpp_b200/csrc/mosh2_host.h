@@ -71,4 +71,46 @@ inline std::vector<int> chunk_table(const int *frame_counts, int n_seq, int chun
     return tab;
 }
 
+// ---- multi-model jobs (mosh2_job_create_multi) ------------------------------------------------------------------------------
+// The chunks of one launch may belong to sequences of different subjects.  Each thread block copies the Model record of its
+// chunk's subject into the shared-memory header, behind the base of the per-CTA global workspace, so the workspace of a
+// multi-model launch starts this many bytes into the dynamic shared memory.
+template <class real>
+constexpr unsigned multi_smem_header() { return mosh2::kSmemHeader + ((unsigned(sizeof(mosh2::Model<real>)) + 15u) & ~15u); }
+
+// Model index of every chunk of `tab` (chunk_table): the chunk's sequence is found from the first frame of its sequence.
+inline std::vector<int> model_of_chunks(const std::vector<int> &tab, const int *frame_counts, int n_seq, const int *model_of_seq) {
+    std::vector<int> out(tab.size() / mosh2::kChunkRec);
+    int q = 0, s0 = 0;
+    for (size_t c = 0; c < out.size(); ++c) {
+        const int first = tab[c * mosh2::kChunkRec + 2];
+        while (q + 1 < n_seq && s0 + frame_counts[q] <= first) s0 += frame_counts[q++];
+        out[c] = model_of_seq[q];
+    }
+    return out;
+}
+
+// One workspace plan serves several models when they have the same kernel shape: equal sizes, free-variable counts, finger /
+// face / joint-angle ranges, prior size and hand-block structure.  Returns the name of the first field (as in mosh2_model_desc)
+// in which `b` differs from `a`, or nullptr.  Their tables (shape, latent markers, attachment, prior, ...) may differ.
+template <class real>
+const char *kernel_shape_mismatch(const mosh2::Model<real> &a, const mosh2::Model<real> &b) {
+    const struct { const char *name; int a, b; } f[] = {
+        {"n_joints", a.nJ, b.nJ}, {"n_markers", a.M, b.M}, {"body_dof", a.body_dof, b.body_dof}, {"p_red", a.p_red, b.p_red},
+        {"n_hand_red", a.n_hand_red, b.n_hand_red}, {"n_hand_full", a.n_hand_full, b.n_hand_full}, {"n_dmpl", a.nd, b.nd},
+        {"kw", a.kw, b.kw}, {"n_free1", a.n1, b.n1}, {"n_free2", a.n2, b.n2}, {"finger_lo", a.finger_lo, b.finger_lo},
+        {"finger_hi", a.finger_hi, b.finger_hi}, {"n_expr", a.n_expr, b.n_expr}, {"face_lo", a.face_lo, b.face_lo},
+        {"face_hi", a.face_hi, b.face_hi}, {"n_jangles", a.n_jang, b.n_jang}, {"prior_k", a.prior_k, b.prior_k},
+        {"prior_d", a.prior_d, b.prior_d}, {"hand_comps (hand blocks)", a.hb_n, b.hb_n},
+        {"hand_comps (hand-block table size)", a.hct_size, b.hct_size}};
+    for (const auto &e : f)
+        if (e.a != e.b) return e.name;
+    for (int k = 0; k < a.hb_n; ++k) {
+        const mosh2::HandBlock &x = a.hb[k], &y = b.hb[k];
+        if (x.r0 != y.r0 || x.r1 != y.r1 || x.q0 != y.q0 || x.q1 != y.q1 || x.ct_off != y.ct_off || x.rw4 != y.rw4)
+            return "hand_comps (hand-block structure)";
+    }
+    return nullptr;
+}
+
 }  // namespace mosh2_host

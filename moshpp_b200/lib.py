@@ -13,7 +13,7 @@ import numpy as np
 
 from .pack import StageIIPack
 
-ABI_VERSION = 105          # MOSH2_VERSION of include/mosh2.h that the ctypes structs below encode
+ABI_VERSION = 106          # MOSH2_VERSION of include/mosh2.h that the ctypes structs below encode
 MOSH2_F32, MOSH2_F64 = 0, 1
 ST_SOLVED, ST_SKIPPED, ST_HAS_VELO, ST_HAS_EXTRAP, ST_GN_FALLBACK, ST_MAXITER, ST_SHORT_WARMUP = 1, 2, 4, 8, 16, 32, 64
 ERR_NAMES = ('data', 'poseB', 'velo', 'poseH', 'dmpl', 'extrap_dmpl', 'poseF', 'expr')   # column order of mosh2_result.errs
@@ -116,6 +116,8 @@ def load_library(path: Optional[str] = None):
     lib.mosh2_model_destroy.restype = None
     lib.mosh2_job_create.argtypes = [vp, C.POINTER(Options), C.c_int32, C.POINTER(Schedule), C.c_int32, C.POINTER(vp)]
     lib.mosh2_job_create_batch.argtypes = [vp, C.POINTER(Options), C.c_int32, _i32p, C.POINTER(Schedule), C.c_int32, C.POINTER(vp)]
+    lib.mosh2_job_create_multi.argtypes = [C.POINTER(vp), C.c_int32, C.POINTER(Options), C.c_int32, _i32p, _i32p, C.POINTER(Schedule),
+                                           C.c_int32, C.POINTER(vp)]
     lib.mosh2_job_upload.argtypes = [vp, _f64p, _u8p]
     lib.mosh2_job_linearize.argtypes = [vp, C.POINTER(Options), C.c_int32, C.c_int32, _f64p, C.POINTER(LinOut)]
     lib.mosh2_job_upload_markers.argtypes = [vp, _f64p, C.c_int32, C.c_int32, _i32p, C.c_int32, C.c_int32, C.c_double, _f64p]
@@ -152,7 +154,7 @@ EXPORTED_SYMBOLS = (
     'mosh2_solve', 'mosh2_job_upload_device', 'mosh2_job_row_width', 'mosh2_job_download_device', 'mosh2_job_span_ms',
     'mosh2_job_create_batch', 'mosh2_job_upload_device_range', 'mosh2_job_warm_states', 'mosh2_job_relaunch_chunks',
     'mosh2_job_boundary_deltas', 'mosh2_release_cached_memory', 'mosh2_mesh_distance', 'mosh2_job_upload_markers', 'mosh2_job_linearize',
-    'mosh2_job_chunk_ranges', 'mosh2_job_upload_markers_range')
+    'mosh2_job_chunk_ranges', 'mosh2_job_upload_markers_range', 'mosh2_job_create_multi')
 
 
 def _ptr(a: np.ndarray, typ):
@@ -289,10 +291,20 @@ class Model:
             pass
 
 
+def multi_job(models, model_of_seq, counts, options: Options, *, chunk_len: int = 0, chunk_warmup: int = 0, warmup_full: int = -1,
+              first_extra: int = 0, precision: int = MOSH2_F32) -> 'Job':
+    """Sequences of several subjects solved by one launch (mosh2_job_create_multi): sequence q has ``counts[q]`` frames and is
+    solved with ``models[model_of_seq[q]]``.  The models (``Model``, one device, one kernel shape) must stay open while the job
+    lives.  Returns a ``Job`` with the interface of a batch job; its frame axis holds the sequences back to back."""
+    return Job(models[0], counts, options, make_schedule(chunk_len, chunk_warmup, warmup_full, first_extra), precision,
+               models=list(models), model_of_seq=model_of_seq)
+
+
 class Job:
     """Staged upload / launch / download on device-resident buffers (used by bench.py)."""
 
-    def __init__(self, model: Model, n_frames, options: Options, schedule: Schedule, precision: int):
+    def __init__(self, model: Model, n_frames, options: Options, schedule: Schedule, precision: int, *, models=None,
+                 model_of_seq=None):
         counts = np.ascontiguousarray(np.atleast_1d(n_frames), dtype=np.int32)
         self.frame_counts = counts
         self.seq_offsets = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
@@ -301,9 +313,19 @@ class Job:
         self.handle = C.c_void_p()
         self.options = options
         self.schedule = schedule
-        rc = self.lib.mosh2_job_create_batch(model.handle, C.byref(options), len(counts), _ptr(counts, _i32p), C.byref(schedule),
-                                             precision, C.byref(self.handle))
-        model._check(rc, 'mosh2_job_create')
+        self.models = models            # multi-model job: every model, kept referenced while the job lives
+        if models is None:
+            rc = self.lib.mosh2_job_create_batch(model.handle, C.byref(options), len(counts), _ptr(counts, _i32p), C.byref(schedule),
+                                                 precision, C.byref(self.handle))
+            model._check(rc, 'mosh2_job_create')
+        else:
+            mos = np.ascontiguousarray(model_of_seq, dtype=np.int32)
+            if mos.shape != counts.shape:
+                raise ValueError(f'{len(counts)} sequences, {len(mos)} model indices')
+            handles = (C.c_void_p * len(models))(*[m.handle for m in models])
+            rc = self.lib.mosh2_job_create_multi(handles, len(models), C.byref(options), len(counts), _ptr(counts, _i32p), _ptr(mos, _i32p),
+                                                 C.byref(schedule), precision, C.byref(self.handle))
+            model._check(rc, 'mosh2_job_create_multi')
         self.result = ResultArrays(n_frames, pack_dims(model.pk))
         self._keep = None
 

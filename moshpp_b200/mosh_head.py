@@ -1,5 +1,7 @@
 """The MoSh++ head without the reference: ``MoSh`` and ``run_moshpp_once`` (src/moshpp/mosh_head.py:65-301,561-606), plus
-``run_moshpp_subject``, which solves all captures of a subject in one launch.
+``run_moshpp_subject``, which solves all captures of a subject in one launch, and for a dataset the reference's jobs filter
+(``universal_mosh_jobs_filter``, tools/run_tools.py:45-67) and ``run_moshpp_jobs``, which solves the captures of many subjects
+in one launch per group of kernel-compatible subjects.
 
 The reference's head imports human_body_prior, loguru, omegaconf, psbody and the marker-layout tools, so the plug-in point
 of its two stage functions cannot be imported where psbody is absent.  This one runs on the package alone:
@@ -260,4 +262,79 @@ def run_moshpp_subject(cfg, mocap_fnames: Optional[List[str]] = None, *, stagei_
             mp.cfg.moshpp[k] = batch_cfg.moshpp[k]
         mp.stageii_data = amass_io.merge_stageii(data, head.stagei_data, to_container(mp.cfg), elapsed, mp.stageii_fname)
         logger.debug('created stageii_fname: %s', mp.stageii_fname)
+    return heads
+
+
+def universal_mosh_jobs_filter(total_jobs, only_stagei: bool = False, determine_shape_for_each_seq: bool = False) -> list:
+    """tools/run_tools.py:45-67: the jobs (``MoSh`` keyword overrides, dotted keys) that still have work to do.  A job whose
+    Stage-II pickle exists is done.  A job's key is ``<dataset>_<session>`` of its capture path (``_<capture file>`` added under
+    ``moshpp.perseq_mosh_stagei``, ``_<session>_<subject>`` for a chosen subject of a multi-subject capture); the first job of a
+    key whose Stage I does not exist yet is kept and, unless ``determine_shape_for_each_seq``, the later jobs of that key are
+    dropped: one of them makes the shape the others need.  ``only_stagei``: jobs whose Stage I exists are dropped too."""
+    filtered_jobs, exclude_keys = [], []
+    for cur_job in total_jobs:
+        mocap_fname_split = cur_job['mocap.fname'].split('/')
+        mocap_key = '_'.join(mocap_fname_split[-3:-1])
+        mosh_cfg = prepare_cfg(**copy.deepcopy(cur_job))
+        if mosh_cfg.moshpp.perseq_mosh_stagei:
+            mocap_key += f'_{mocap_fname_split[-1]}'
+        if mosh_cfg.mocap.subject_id >= 0 and mosh_cfg.mocap.multi_subject:
+            mocap_key += f'_{mosh_cfg.mocap.session_name}'
+            mocap_key += f'_{mosh_cfg.mocap.subject_name}'
+        if mocap_key in exclude_keys:
+            continue
+        if os.path.exists(mosh_cfg.dirs.stageii_fname):
+            continue
+        if not os.path.exists(mosh_cfg.dirs.stagei_fname) and not determine_shape_for_each_seq:
+            exclude_keys.append(mocap_key)
+        if only_stagei and os.path.exists(mosh_cfg.dirs.stagei_fname):
+            continue
+        filtered_jobs.append(cur_job)
+    return filtered_jobs
+
+
+def run_moshpp_jobs(jobs, *, stagei_func=None, stageii_subjects_func=None) -> List[MoSh]:
+    """A dataset: ``run_moshpp_once`` of every job (``MoSh`` keyword overrides, dotted keys), with the Stage-II solves of all
+    subjects in one ``chmosh.mosh_stageii_subjects`` call -- one launch per group of kernel-compatible subjects instead of one
+    per subject or capture.
+
+    The jobs are grouped by their Stage-I pickle (``dirs.stagei_fname``): one group per subject, or per capture under
+    ``moshpp.perseq_mosh_stagei``.  Each group's Stage I is run (from its first job's configuration, as ``run_moshpp_once`` of
+    that job would) or loaded through ``MoSh.mosh_stagei``.  Every job without a Stage-II pickle is then solved; its pickle
+    is written at the path, and with the contents, that ``run_moshpp_once`` of that job produces, apart from the timing
+    entries (``stageii_elapsed_time`` is the time of the whole call).  Returns one ``MoSh`` per job, in the order of ``jobs``."""
+    heads = [MoSh(**dict(job)) for job in jobs]
+    groups = {}
+    for mp in heads:
+        groups.setdefault(mp.stagei_fname, []).append(mp)
+    subjects, members = [], []
+    for group in groups.values():
+        for mp in group:                        # (the first job makes the Stage I, the others load it)
+            mp.mosh_stagei(stagei_func)
+        if group[0].cfg.runtime.stagei_only:
+            continue
+        todo = []
+        for mp in group:
+            if os.path.exists(mp.stageii_fname):
+                mp.stageii_data = _load(mp.stageii_fname)
+                logger.info('loading mosh stageii results from %s', mp.stageii_fname)
+            else:
+                todo.append(mp)
+        if todo:
+            subjects.append(dict(cfg=todo[0].cfg, mocap_fnames=[mp.cfg.mocap.fname for mp in todo], **todo[0]._stageii_args()))
+            members.append(todo)
+    if not subjects:
+        return heads
+    if stageii_subjects_func is None:
+        from .chmosh import mosh_stageii_subjects as stageii_subjects_func
+    logger.info('attempting mosh stageii of %d captures of %d subjects', sum(len(t) for t in members), len(subjects))
+    tm = time.time()
+    results = stageii_subjects_func(subjects)
+    elapsed = time.time() - tm
+    for sub, todo, outs in zip(subjects, members, results):
+        for mp, data in zip(todo, outs):
+            for k in ('optimize_fingers', 'optimize_face'):     # the Stage-II gating the solver applied to its cfg
+                mp.cfg.moshpp[k] = sub['cfg'].moshpp[k]
+            mp.stageii_data = amass_io.merge_stageii(data, mp.stagei_data, to_container(mp.cfg), elapsed, mp.stageii_fname)
+            logger.debug('created stageii_fname: %s', mp.stageii_fname)
     return heads

@@ -554,14 +554,16 @@ from .cfg import AttrDict, STAGEII_WEIGHTS, default_cfg  # noqa: E402,F401
 
 def make_case(out_dir: str, config: str = 'C2', *, frames: Optional[int] = None, n_verts: Optional[int] = None,
               seq_idx: int = 0, noise_mm: float = 1.0, dropout: float = 0.03, hand_side: str = 'left',
-              write_mocap: bool = True, reuse_model: bool = True) -> Dict:
+              write_mocap: bool = True, reuse_model: bool = True, model_seed: int = 0) -> Dict:
     """Writes one synthetic Stage-II case (model, priors, mocap file) and returns everything
-    ``mosh_stageii`` needs plus the ground truth."""
+    ``mosh_stageii`` needs plus the ground truth.  ``seq_idx`` picks the shape (and with it the latent markers) and the
+    motion; ``model_seed`` > 0 writes and uses a second model file of the same family and size (another template, shape
+    space and joint regressor; e.g. the other gender's model)."""
     c = dict(CONFIGS[config])
     mt = c['model_type']
     F = int(frames or c['frames'])
     os.makedirs(out_dir, exist_ok=True)
-    tag = f'{mt}_{n_verts or NUM_VERTS[mt]}' + (f'_{hand_side}' if mt == 'mano' else '')
+    tag = f'{mt}_{n_verts or NUM_VERTS[mt]}' + (f'_{hand_side}' if mt == 'mano' else '') + (f'_m{model_seed}' if model_seed else '')
     model_fname = os.path.join(out_dir, f'model_{tag}.pkl')
     hand_prior_fname = os.path.join(out_dir, 'pose_hand_prior.npz')
     body_prior_fname = os.path.join(out_dir, 'pose_body_prior.pkl')
@@ -570,7 +572,7 @@ def make_case(out_dir: str, config: str = 'C2', *, frames: Optional[int] = None,
         with open(model_fname, 'rb') as f:
             model = pickle.load(f)
     else:
-        model = make_body_model(mt, n_verts=n_verts, seed=SEED_MODEL + (7 if hand_side == 'right' else 0))
+        model = make_body_model(mt, n_verts=n_verts, seed=SEED_MODEL + (7 if hand_side == 'right' else 0) + 1000 * model_seed)
         with open(model_fname, 'wb') as f:
             pickle.dump(model, f, protocol=pickle.HIGHEST_PROTOCOL)
     if not os.path.exists(hand_prior_fname):
@@ -664,7 +666,8 @@ from .stagei import write_marker_layout  # noqa: E402,F401  (re-exported: the fi
 def make_subject(out_dir: str, config: str = 'C2', frames=(1000, 2000), **kw):
     """Several captures of ONE synthetic subject (one shape, one set of latent markers): a case of ``sum(frames)`` frames
     (``make_case``, npz configurations) whose capture file is cut into consecutive captures of ``frames[k]`` frames.
-    Returns (the case, the capture file names)."""
+    ``seq_idx`` (shape, latent markers and motion) and ``model_seed`` (a second model file) of ``make_case`` make other
+    subjects.  Returns (the case, the capture file names)."""
     case = make_case(out_dir, config, frames=int(sum(frames)), **kw)
     if not case['mocap_fname'].endswith('.npz'):
         raise ValueError(f'{config}: make_subject cuts npz captures only')
