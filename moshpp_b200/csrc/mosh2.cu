@@ -107,7 +107,8 @@ class BlockCache {
 };
 BlockCache g_blocks;
 
-constexpr size_t kMaxSmem = 227 * 1024;
+using mosh2_host::kMaxSmem;
+using mosh2_host::plan_workspace;
 #ifndef MOSH2_F32_THREADS
 #define MOSH2_F32_THREADS 384      // 168 registers per thread: measured best of 256 / 320 / 384 / 512 (profiles/)
 #endif
@@ -517,29 +518,6 @@ int launch(mosh2_job *j, const mosh2::Model<real> &m) {
     CU(cudaGetLastError());
     CU(cudaEventRecord(j->ev1, j->stream));
     return 0;
-}
-
-template <class real>
-void plan_workspace(mosh2::Model<real> &m, size_t *smem, size_t *gws, int *big, unsigned header = mosh2::kSmemHeader) {
-    // preference order: 20-marker tiles, then 10-marker tiles, while the workspace fits the shared-memory budget; the
-    // f64 / oversized case moves A, its factor and the Jacobian tiles to a per-CTA global workspace.  `header`: bytes in
-    // front of the workspace (a multi-model job keeps the chunk's Model record there)
-    const int tries[3][2] = {{20, 0}, {10, 0}, {10, 1}};   // markers per tile (a warp owns ten), big
-    const char *dev_tile = getenv("MOSH2_DEV_TILE");      // development aid: 10 = skip the 20-marker tile
-    const bool dev_big = getenv("MOSH2_DEV_BIG") != nullptr;   // development aid: force the global-workspace layout
-    for (int pass = dev_big ? 2 : ((dev_tile && atoi(dev_tile) == 10) ? 1 : 0); pass < 3; ++pass) {
-        m.tile_markers = tries[pass][0];
-        m.dev_no_tc = getenv("MOSH2_DEV_NO_TC") ? 1 : 0;      // development aid: J^T J on the CUDA cores
-        const bool in_global = tries[pass][1] != 0;
-        const mosh2::Dims d = mosh2::make_dims(m);
-        mosh2::Arena S{header}, G{0};
-        if (in_global) { mosh2::Work<real, true> w{}; mosh2::carve<real, true>(w, d, m, S, G); }
-        else { mosh2::Work<real, false> w{}; mosh2::carve<real, false>(w, d, m, S, G); }
-        *big = in_global ? 1 : 0;
-        *smem = (S.off + 15) & ~size_t(15);
-        *gws = (G.off + 255) & ~size_t(255);
-        if (S.off <= kMaxSmem) return;
-    }
 }
 
 // mosh2_job_linearize in the job's compute type: the caller's float64 states are rounded to `real` on the way in, every

@@ -405,8 +405,9 @@ struct Work {
     SPtr<real> x, xt, pose_prev, velo_tgt, dm_tgt;
     // forward scratch of the latest evaluation
     SPtr<real> fullpose, Rl, dRl, Jp, Rg, tg, vp, pj, Rsk, mk, rm, obs, py, pq, pxg;
-    // Jacobian / normal equations
-    SPtr<real> Loc, MtR, u, dtg, Linv, Pn, g, Ag, dgn, d, tmp, ds;
+    // Jacobian / normal equations (the build scratch Loc .. dtg is "big": laid over Lm, in the global workspace with BIG)
+    BPtr<real, BIG> Loc, MtR, u, dtg;
+    SPtr<real> Linv, Pn, g, Ag, dgn, d, tmp, ds;
     BPtr<real, BIG> Jt, Jf, A, Lm;
     SPtr<real> red, sc, hct;
     SPtr<int> colmap, colsrc, jlist, isc;
@@ -416,7 +417,8 @@ struct Work {
     SPtr<int> c_parents, c_fk_order, c_wj, c_free1, c_free2, c_pids;
     SPtr<int> c_tin, c_tsz;   // pre-order index and subtree size of every joint: j in subtree(a) <=> tin[j]-tin[a] in [0, tsz[a])
     SPtr<real> c_wv, c_v0, c_coefs, c_j0, c_hmean, c_pmeans, c_pnlw;
-    SPtr<real> c_jd;          // joint-position directions of the per-frame linear coefficients (DMPL, expressions)
+    SPtr<real> c_jd;          // joint-position directions of the per-frame linear coefficients (DMPL, expressions); not staged
+                              // with BIG, where the kernel reads Model::jd (Solver::jdir)
     SPtr<long long> prof;
     SPtr<uint8_t> vis;
     SPtr<uint32_t> c_chain;   // [joint][4 words]: the joint's ancestor chain, root first, one byte per joint id, 255-padded
@@ -563,15 +565,11 @@ M2_HD void carve(Work<real, BIG> &w, const Dims &d, const Model<real> &m, Arena 
         B.off = mark_b;
         w.Jt.ofs = B.take<real>(d.jt_size);
         w.Jf.ofs = B.take<real>(3 * d.tmk * d.npad);
-        if (!BIG) {
-            w.Loc.ofs = S.take<real>(3 * kM3 * d.M); w.MtR.ofs = S.take<real>(kM3 * d.S);
-            w.u.ofs = S.take<real>(kM3 * d.nJ); w.dtg.ofs = S.take<real>(3 * d.nJ * d.nd + 1);
-        }
+        // (with BIG these go to the global workspace as well: in float64, 36 M words each for Loc and MtR and 3 nJ nd for dtg
+        // -- 106 KB for SMPL-X with 80 expressions -- do not fit next to the rest of the shared part)
+        w.Loc.ofs = B.take<real>(3 * kM3 * d.M); w.MtR.ofs = B.take<real>(kM3 * d.S);
+        w.u.ofs = B.take<real>(kM3 * d.nJ); w.dtg.ofs = B.take<real>(3 * d.nJ * d.nd + 1);
         if (B.off < end_b) B.off = end_b;
-    }
-    if (BIG) {
-        w.Loc.ofs = S.take<real>(3 * kM3 * d.M); w.MtR.ofs = S.take<real>(kM3 * d.S);
-        w.u.ofs = S.take<real>(kM3 * d.nJ); w.dtg.ofs = S.take<real>(3 * d.nJ * d.nd + 1);
     }
     w.Linv.ofs = S.take<real>(size_t((d.n2 + kCholNB - 1) / kCholNB) * kCholNB * kCholNB);
     w.Pn.ofs = S.take<real>(size_t(kCholNB) * d.ldp);
@@ -589,6 +587,8 @@ M2_HD void carve(Work<real, BIG> &w, const Dims &d, const Model<real> &m, Arena 
     // coefficients, joint positions and directions, prior means, hand-PCA blocks, free-variable lists -- form ONE
     // contiguous region: the host library keeps a byte-identical image of it (Model::stage_blob, stage_image below) and a chunk
     // fetches it with a single bulk asynchronous copy (cp.async.bulk completing on an mbarrier) instead of thirteen copy loops.
+    // The joint directions c_jd come last and are left out with BIG (3 nJ nd words, as dtg): the image is laid out without
+    // BIG, and a BIG block copies the prefix of it that ends with hct.
     S.off = (S.off + 15) & ~size_t(15);
     w.stage_ofs = uint32_t(S.off);
     w.c_parents.ofs = S.take<int>(d.nJ); w.c_fk_order.ofs = S.take<int>(d.nJ);
@@ -597,8 +597,8 @@ M2_HD void carve(Work<real, BIG> &w, const Dims &d, const Model<real> &m, Arena 
     w.c_wv.ofs = S.take<real>(d.S * d.kw); w.c_v0.ofs = S.take<real>(3 * d.S); w.c_coefs.ofs = S.take<real>(3 * d.M);
     w.c_j0.ofs = S.take<real>(3 * d.nJ); w.c_hmean.ofs = S.take<real>(m.n_hand_full + 1);
     w.c_pmeans.ofs = S.take<real>(d.K * d.D + 1); w.c_pnlw.ofs = S.take<real>(d.K + 1);
-    w.c_jd.ofs = S.take<real>(size_t(3) * d.nJ * d.nd + 1);
     w.hct.ofs = S.take<real>(hct_size + 4);
+    if (!BIG) w.c_jd.ofs = S.take<real>(size_t(3) * d.nJ * d.nd + 1);
     S.off = (S.off + 15) & ~size_t(15);
     w.stage_bytes = uint32_t(S.off) - w.stage_ofs;
     // tables the chunk derives itself
@@ -659,6 +659,10 @@ struct Solver {
         : m(m_), job(j_), w(w_), cta(c_), d(d_) {}
 
 #define CTA_FOR(i, n) _Pragma("unroll 1") for (int i = cta.tid; i < (n); i += cta.nthr)
+
+    // joint-position directions of the linear coefficients [nJ][3][nd]: staged in shared memory, or with BIG the model's own
+    // table (carve() leaves them out of the staged region there)
+    M2_D const real *jdir() const { return BIG ? m.jd : static_cast<const real *>(w.c_jd); }
 
     // ---- CTA-wide maximum of one per-thread value, broadcast (rare path: boundary repair)
     M2_D void cta_max(real *v) {
@@ -794,7 +798,7 @@ struct Solver {
         }
         CTA_FOR(i, 3 * d.nJ) {
             real v = w.c_j0[i];
-            for (int q = 0; q < d.nd; ++q) v += w.c_jd[i * d.nd + q] * dl[q];
+            for (int q = 0; q < d.nd; ++q) v += jdir()[i * d.nd + q] * dl[q];
             w.Jp[i] = v;
         }
         CTA_FOR(i, d.D) w.pxg[i] = th[w.c_pids[i]];          // the pose coefficients the prior sees, in its own order
@@ -1181,12 +1185,12 @@ struct Solver {
             for (int u = 0; u < kMaxDepth / 4; ++u) cw[u] = w.c_chain[j * (kMaxDepth / 4) + u];
             int prev = int(cw[0] & 255u);
             real acc[3];
-            for (int r = 0; r < 3; ++r) acc[r] = w.c_jd[(3 * prev + r) * d.nd + i];
+            for (int r = 0; r < 3; ++r) acc[r] = jdir()[(3 * prev + r) * d.nd + i];
             for (int k = 1; k < kMaxDepth; ++k) {
                 const int cj = int((cw[k >> 2] >> (8 * (k & 3))) & 255u);
                 if (cj == 255) break;
                 real dj[3], t[3];
-                for (int r = 0; r < 3; ++r) dj[r] = w.c_jd[(3 * cj + r) * d.nd + i] - w.c_jd[(3 * prev + r) * d.nd + i];
+                for (int r = 0; r < 3; ++r) dj[r] = jdir()[(3 * cj + r) * d.nd + i] - jdir()[(3 * prev + r) * d.nd + i];
                 mat3_vec(w.Rg + 9 * prev, dj, t);
                 for (int r = 0; r < 3; ++r) acc[r] = acc[r] + t[r];
                 prev = cj;
@@ -1272,7 +1276,7 @@ struct Solver {
                     if (j < 0) continue;
                     const real wt = w.c_wv[s * d.kw + kk];
                     real df[3], o[3];
-                    for (int r = 0; r < 3; ++r) df[r] = sdv[3 * t + r] - w.c_jd[(3 * j + r) * d.nd + i];
+                    for (int r = 0; r < 3; ++r) df[r] = sdv[3 * t + r] - jdir()[(3 * j + r) * d.nd + i];
                     mat3_vec(w.Rg + 9 * j, df, o);
                     for (int r = 0; r < 3; ++r) dv[r] += wt * (o[r] + w.dtg[3 * (j * d.nd + i) + r]);
                 }

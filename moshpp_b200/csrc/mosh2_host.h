@@ -1,5 +1,7 @@
 // mosh2_host.h -- host-side layout helpers shared by libmosh2.so and the test-only host build.
 #pragma once
+#include <cstddef>
+#include <cstdlib>
 #include <vector>
 
 #include "mosh2_device.cuh"
@@ -77,6 +79,33 @@ inline std::vector<int> chunk_table(const int *frame_counts, int n_seq, int chun
 // multi-model launch starts this many bytes into the dynamic shared memory.
 template <class real>
 constexpr unsigned multi_smem_header() { return mosh2::kSmemHeader + ((unsigned(sizeof(mosh2::Model<real>)) + 15u) & ~15u); }
+
+// ---- the workspace plan of a job ----------------------------------------------------------------------------------------------
+constexpr size_t kMaxSmem = 227 * 1024;      // dynamic shared memory per block on sm_90
+
+// Chooses the layout of `m`'s workspace and sets m.tile_markers (and m.dev_no_tc).  Preference order: 20-marker tiles, then
+// 10-marker tiles, while the workspace fits the shared-memory budget; then (*big = 1) the layout that moves A, its factor, the
+// Jacobian tiles and the linear-block scratch to a per-CTA global workspace of *gws bytes.  *smem > kMaxSmem: the model does
+// not fit at all.  `header`: bytes in front of the workspace (a multi-model job keeps the chunk's Model record there).
+template <class real>
+void plan_workspace(mosh2::Model<real> &m, size_t *smem, size_t *gws, int *big, unsigned header = mosh2::kSmemHeader) {
+    const int tries[3][2] = {{20, 0}, {10, 0}, {10, 1}};   // markers per tile (a warp owns ten), big
+    const char *dev_tile = getenv("MOSH2_DEV_TILE");      // development aid: 10 = skip the 20-marker tile
+    const bool dev_big = getenv("MOSH2_DEV_BIG") != nullptr;   // development aid: force the global-workspace layout
+    for (int pass = dev_big ? 2 : ((dev_tile && atoi(dev_tile) == 10) ? 1 : 0); pass < 3; ++pass) {
+        m.tile_markers = tries[pass][0];
+        m.dev_no_tc = getenv("MOSH2_DEV_NO_TC") ? 1 : 0;      // development aid: J^T J on the CUDA cores
+        const bool in_global = tries[pass][1] != 0;
+        const mosh2::Dims d = mosh2::make_dims(m);
+        mosh2::Arena S{header}, G{0};
+        if (in_global) { mosh2::Work<real, true> w{}; mosh2::carve<real, true>(w, d, m, S, G); }
+        else { mosh2::Work<real, false> w{}; mosh2::carve<real, false>(w, d, m, S, G); }
+        *big = in_global ? 1 : 0;
+        *smem = (S.off + 15) & ~size_t(15);
+        *gws = (G.off + 255) & ~size_t(255);
+        if (S.off <= kMaxSmem) return;
+    }
+}
 
 // Model index of every chunk of `tab` (chunk_table): the chunk's sequence is found from the first frame of its sequence.
 inline std::vector<int> model_of_chunks(const std::vector<int> &tab, const int *frame_counts, int n_seq, const int *model_of_seq) {

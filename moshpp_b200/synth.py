@@ -549,21 +549,29 @@ CONFIGS = {
 }
 
 
+# make_case arguments of a model with the reference's SMPL-X face layout (moshpp_conf.yaml: betas_expr_start_id 300,
+# num_expressions 80; SMPL-X files carry 400 shape components)
+REFERENCE_FACE = dict(n_betas=400, expr_start=300, num_expressions=80)
+
 from .cfg import AttrDict, STAGEII_WEIGHTS, default_cfg  # noqa: E402,F401
 
 
 def make_case(out_dir: str, config: str = 'C2', *, frames: Optional[int] = None, n_verts: Optional[int] = None,
               seq_idx: int = 0, noise_mm: float = 1.0, dropout: float = 0.03, hand_side: str = 'left',
-              write_mocap: bool = True, reuse_model: bool = True, model_seed: int = 0) -> Dict:
+              write_mocap: bool = True, reuse_model: bool = True, model_seed: int = 0, n_betas: int = 24,
+              expr_start: int = 16, num_expressions: int = 8) -> Dict:
     """Writes one synthetic Stage-II case (model, priors, mocap file) and returns everything
     ``mosh_stageii`` needs plus the ground truth.  ``seq_idx`` picks the shape (and with it the latent markers) and the
     motion; ``model_seed`` > 0 writes and uses a second model file of the same family and size (another template, shape
-    space and joint regressor; e.g. the other gender's model)."""
+    space and joint regressor; e.g. the other gender's model).  ``n_betas``: shape components of the model file;
+    ``expr_start`` / ``num_expressions``: the expression components of the configurations with ``optimize_face``
+    (``REFERENCE_FACE`` is the layout of the reference's SMPL-X face setup)."""
     c = dict(CONFIGS[config])
     mt = c['model_type']
     F = int(frames or c['frames'])
     os.makedirs(out_dir, exist_ok=True)
-    tag = f'{mt}_{n_verts or NUM_VERTS[mt]}' + (f'_{hand_side}' if mt == 'mano' else '') + (f'_m{model_seed}' if model_seed else '')
+    tag = (f'{mt}_{n_verts or NUM_VERTS[mt]}' + (f'_{hand_side}' if mt == 'mano' else '') + (f'_m{model_seed}' if model_seed else '')
+           + (f'_b{n_betas}' if n_betas != 24 else ''))
     model_fname = os.path.join(out_dir, f'model_{tag}.pkl')
     hand_prior_fname = os.path.join(out_dir, 'pose_hand_prior.npz')
     body_prior_fname = os.path.join(out_dir, 'pose_body_prior.pkl')
@@ -572,7 +580,8 @@ def make_case(out_dir: str, config: str = 'C2', *, frames: Optional[int] = None,
         with open(model_fname, 'rb') as f:
             model = pickle.load(f)
     else:
-        model = make_body_model(mt, n_verts=n_verts, seed=SEED_MODEL + (7 if hand_side == 'right' else 0) + 1000 * model_seed)
+        model = make_body_model(mt, n_verts=n_verts, n_betas=n_betas,
+                                seed=SEED_MODEL + (7 if hand_side == 'right' else 0) + 1000 * model_seed)
         with open(model_fname, 'wb') as f:
             pickle.dump(model, f, protocol=pickle.HIGHEST_PROTOCOL)
     if not os.path.exists(hand_prior_fname):
@@ -602,10 +611,10 @@ def make_case(out_dir: str, config: str = 'C2', *, frames: Optional[int] = None,
         'moshpp.verbosity': 0,
     })
     face = bool(c.get('optimize_face', False))
-    if face:                 # the fixture model has 24 shape components: 16 betas, then 8 used as expressions
+    if face:                 # by default the model has 24 shape components: 16 betas, then 8 used as expressions
         cfg.moshpp.optimize_face = True
-        cfg.surface_model.betas_expr_start_id = 16
-        cfg.surface_model.num_expressions = 8
+        cfg.surface_model.betas_expr_start_id = expr_start
+        cfg.surface_model.num_expressions = num_expressions
 
     sm = _pack.load_surface_model(model_fname, pose_hand_prior_fname=hand_prior_fname,
                                   use_hands_mean=cfg.surface_model.use_hands_mean,
@@ -622,7 +631,7 @@ def make_case(out_dir: str, config: str = 'C2', *, frames: Optional[int] = None,
     pk = _pack.build_pack(sm, betas, markers_latent, num_betas=16, prior=prior, dmpl_dirs=dm_dirs,
                           num_dmpls=8 if c['optimize_dynamics'] else 0,
                           optimize_fingers=c['optimize_fingers'], optimize_face=face,
-                          expr_start=16 if face else 0, num_expressions=8 if face else 0)
+                          expr_start=expr_start if face else 0, num_expressions=num_expressions if face else 0)
     cfg_idx = list(CONFIGS).index(config)
     pose, trans, dm = make_motion(pk, F, seed=SEED_MOTION + cfg_idx + 1000 * seq_idx)
     if not c['optimize_fingers'] and pk.n_hand_red:
@@ -647,7 +656,10 @@ def make_case(out_dir: str, config: str = 'C2', *, frames: Optional[int] = None,
     data[:, :pk.n_markers] = np.where(vis[:, perm, None], obs[:, perm], np.nan) * 1000.0
     data[:, -1] = 1000.0 * (trans + 0.3)
     side = f'_{hand_side}' if mt == 'mano' else ''
-    mocap_fname = os.path.join(out_dir, f'mocap_{config}{side}_{seq_idx:02d}_{F}.{c["mocap_ext"]}')
+    # (a model with another shape space, or other expressions, synthesises other observations: a file of its own)
+    size = f'_b{n_betas}' if n_betas != 24 else ''
+    size += f'_e{expr_start}x{num_expressions}' if face and (expr_start, num_expressions) != (16, 8) else ''
+    mocap_fname = os.path.join(out_dir, f'mocap_{config}{side}{size}_{seq_idx:02d}_{F}.{c["mocap_ext"]}')
     if write_mocap:
         if c['mocap_ext'] == 'npz':
             np.savez(mocap_fname, markers=data, labels=np.array(file_labels), frame_rate=120.0)

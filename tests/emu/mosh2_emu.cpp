@@ -283,7 +283,26 @@ int run_gn(const mosh2_model_desc *desc, int n, const double *A, const double *g
     return 0;
 }
 
+template <class real>
+int run_plan(const mosh2_model_desc *desc, int multi, int64_t *out) {
+    mosh2::Model<real> m = gn_case::dims_model<real>(*desc);
+    size_t smem = 0, gws = 0;
+    int big = 0;
+    mosh2_host::plan_workspace(m, &smem, &gws, &big, multi ? mosh2_host::multi_smem_header<real>() : mosh2::kSmemHeader);
+    out[0] = int64_t(smem); out[1] = int64_t(gws); out[2] = big; out[3] = m.tile_markers; out[4] = int64_t(mosh2_host::kMaxSmem);
+    return 0;
+}
+
 }  // namespace
+
+// The library's workspace plan (mosh2_host::plan_workspace) for a model with the dimensions of `desc`, as mosh2_job_create
+// (multi = 0) or mosh2_job_create_multi (multi = 1) makes it.  out[5]: shared-memory bytes per block, global-workspace bytes
+// per block, 1 if the global-workspace layout was chosen, markers per Jacobian tile, the shared-memory budget.  The job fits
+// iff out[0] <= out[4].
+extern "C" int mosh2_emu_plan(const mosh2_model_desc *desc, int32_t precision, int32_t multi, int64_t *out) {
+    if (precision == MOSH2_F64) return run_plan<double>(desc, multi, out);
+    return run_plan<float>(desc, multi, out);
+}
 
 // `threads` is accepted for the signature of gn_run and ignored: the host build is one thread
 extern "C" int mosh2_emu_gauss_newton(int32_t precision, int32_t big, int32_t threads, const mosh2_model_desc *desc, int32_t n,

@@ -14,7 +14,7 @@
 
 namespace gn_case {
 
-constexpr size_t kMaxSmem = 227 * 1024;     // the library's shared-memory budget per block (mosh2.cu)
+using mosh2_host::kMaxSmem;                  // the library's shared-memory budget per block
 constexpr unsigned char kNaN = 0xff;         // every byte 0xff: a NaN in float32 and in float64
 
 template <class real>
