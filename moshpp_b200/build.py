@@ -13,6 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libmosh2.so')
+PROF_LIB = os.path.join(HERE, 'libmosh2_prof.so')     # development build with the phase timers (-DMOSH2_PROFILE)
 EMU_SRC = os.path.join(ROOT, 'tests', 'emu', 'mosh2_emu.cpp')
 EMU_ADAPTER_SRC = os.path.join(ROOT, 'tests', 'emu', 'mosh2_emu_adapter.cpp')
 EMU_MULTI_SRC = os.path.join(ROOT, 'tests', 'emu', 'mosh2_emu_multi.cpp')    # includes EMU_SRC: one translation unit
@@ -42,17 +43,19 @@ def _nvcc() -> str:
     raise RuntimeError('nvcc not found: libmosh2.so cannot be built (there is no CPU fallback)')
 
 
-def build_library(force: bool = False, verbose: bool = False) -> str:
+def build_library(force: bool = False, verbose: bool = False, profile: bool = False) -> str:
+    """``profile``: the development build libmosh2_prof.so, whose kernel accumulates phase clocks (tools/gpu_phases.py)."""
     srcs = [os.path.join(CSRC, "mosh2.cu"), os.path.join(CSRC, "mosh2_device.cuh"), os.path.join(CSRC, "mosh2_host.h"),
             os.path.join(CSRC, "mesh_distance.cuh"), os.path.join(ROOT, 'include', 'mosh2.h')]
-    if force or _stale(LIB, srcs):
-        cmd = [_nvcc()] + NVCC_FLAGS + (['-Xptxas', '-v'] if verbose else []) + ['-o', LIB, srcs[0]]
+    out = PROF_LIB if profile else LIB
+    if force or _stale(out, srcs):
+        cmd = [_nvcc()] + NVCC_FLAGS + (['-DMOSH2_PROFILE'] if profile else []) + (['-Xptxas', '-v'] if verbose else []) + ['-o', out, srcs[0]]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError('nvcc failed:\n' + r.stdout + r.stderr)
         if verbose:
             print(r.stdout + r.stderr)
-    return LIB
+    return out
 
 
 def build_emu(force: bool = False) -> str:
@@ -95,4 +98,4 @@ def build_gn_test(force: bool = False) -> str:
 
 
 if __name__ == '__main__':
-    print(build_library(force='--force' in sys.argv, verbose='-v' in sys.argv))
+    print(build_library(force='--force' in sys.argv, verbose='-v' in sys.argv, profile='--profile' in sys.argv))

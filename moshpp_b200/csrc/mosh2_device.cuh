@@ -1478,7 +1478,17 @@ struct Solver {
                     }
             }
         }
-        CTA_FOR(cc, n) {                                 // (six rows in flight, for the same reason; same order of the sum)
+        // J^T r, a thread per column: on the tensor-core paths the first (ntile mod nwarp) warps took one 16x16 block more,
+        // so the columns start at the warp after them (the same sums in the same order, on other threads)
+        int jr_tid = cta.tid;
+#if M2_GPU
+        if (sizeof(real) == 8 || w.tc) {
+            const int nb16 = (n + 15) >> 4, nwarp = cta.nthr >> 5;
+            jr_tid = (cta.tid + cta.nthr - 32 * ((nb16 * (nb16 + 1) / 2) % nwarp)) % cta.nthr;
+        }
+#endif
+#pragma unroll 1
+        for (int cc = jr_tid; cc < n; cc += cta.nthr) {  // (six rows in flight, for the same reason; same order of the sum)
             real s = 0;
             for (int row = 0; row < trows; row += 6) {
                 real jv[6];
