@@ -432,29 +432,188 @@ def download_verified(job, bad, report):
     return res
 
 
-def _select_input(mocap: MocapSession, cfg, latent_labels, device_adapter: bool):
-    """(selected frames, file column of every latent marker or None, obs, vis, number of frames) of one capture.
+def _check_mode(mode: str):
+    if mode not in BOUNDARY_TOL:
+        raise ValueError(f"mode must be 'fast' or 'exact', not {mode!r}")
+
+
+def _read_capture(fname: str, cfg, latent_labels, labels_map, device_adapter: bool) -> dict:
+    """One capture of a Stage-II call: its MocapSession, the selected frames ``sel``, the file column of every latent marker
+    ``raw_cols`` (None: host adapter), the host adapter's ``obs`` / ``vis`` and the number of frames ``F``.
 
     Input adapter.  Normally on the device: the raw marker table of the file goes up as it is and one kernel produces the
-    observations and the visibility mask (mosh2_job_upload_markers); the host copy of the same clean-up -- needed for the
-    output dictionary only -- is made behind the solve.  Labels that own several columns, and frame selections that are
-    not a forward range inside the file, take the host path (``frames_for_labels``, obs / vis returned here) in front of
+    observations and the visibility mask (mosh2_job_upload_markers_range); the host copy of the same clean-up -- needed for
+    the output dictionary only -- is made behind the solve.  Labels that own several columns, and frame selections that are
+    not a forward range inside the file, take the host path (``frames_for_labels``, obs / vis read here) in front of
     the solve."""
+    mocap = MocapSession(fname, mocap_unit=cfg.mocap.unit, mocap_rotate=cfg.mocap.rotate, labels_map=labels_map,
+                         only_subjects=[cfg.mocap.subject_name] if cfg.mocap.multi_subject else None)
+    labels = list(latent_labels)
     end = len(mocap) if cfg.mocap.end_fidx == -1 else cfg.mocap.end_fidx
-    selected_frames = range(cfg.mocap.start_fidx, end, cfg.mocap.ds_rate)                         # chmosh.py:539-540
-    raw_cols = mocap.raw_columns_for_labels(list(latent_labels)) if device_adapter else None
-    if raw_cols is not None and not (len(selected_frames) and selected_frames.step > 0 and selected_frames.start >= 0
-                                     and selected_frames[-1] < len(mocap)):
+    sel = range(cfg.mocap.start_fidx, end, cfg.mocap.ds_rate)                                      # chmosh.py:539-540
+    raw_cols = mocap.raw_columns_for_labels(labels) if device_adapter else None
+    if raw_cols is not None and not (len(sel) and sel.step > 0 and sel.start >= 0 and sel[-1] < len(mocap)):
         raw_cols = None
     if raw_cols is None:
-        obs, vis = mocap.frames_for_labels(list(latent_labels), selected_frames)
+        obs, vis = mocap.frames_for_labels(labels, sel)
         F = obs.shape[0]
     else:
         obs = vis = None
-        F = len(selected_frames)
+        F = len(sel)
     if F == 0:
         raise ValueError('no frames selected')
-    return selected_frames, raw_cols, obs, vis, F
+    return dict(fname=fname, cfg=cfg, labels=labels, mocap=mocap, sel=sel, raw_cols=raw_cols, obs=obs, vis=vis, F=F)
+
+
+def _subject(seqs, cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname, device: int,
+             subject_cache: bool = True) -> dict:
+    """A subject of a launch: its captures ``seqs`` (``_read_capture``) with its pack, options, flags and device model from
+    the subject cache, or with ``subject_cache=False`` prepared for this call alone (``model`` None: ``_solve_launch`` makes
+    it and closes it at the end)."""
+    if subject_cache:
+        pk, opts, flags, model, cache_hit = subject_for(cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname, device)
+    else:
+        pk, opts, flags = prepare_stageii(cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname)
+        model, cache_hit = None, False
+    return dict(seqs=seqs, pk=pk, opts=opts, flags=flags, model=model, cache_hit=cache_hit, device=device)
+
+
+def _resolve_schedule(pk, mode: str, counts, chunk_len, chunk_warmup, warmup_full, first_extra, precision, verify: bool,
+                      boundary_tol, sm_budget: int) -> dict:
+    """The schedule of one launch over sequences of ``counts`` frames: the keyword overrides of the public entry points over
+    the defaults of the pack and ``mode`` (``default_schedule``).  Returns chunk_len (0: one chunk per sequence),
+    chunk_warmup, warmup_full, first_extra, precision ('f32' | 'f64'), mode, prec (the MOSH2_* code of the precision) and tol
+    (the boundary tolerance; None: no boundary check)."""
+    w_def, wf_def, prec_def, tol_def = default_schedule(pk.model_type, mode, pk.n_dmpl)
+    chunk_warmup = w_def if chunk_warmup is None else int(chunk_warmup)
+    warmup_full = (wf_def if chunk_warmup == w_def else -1) if warmup_full is None else int(warmup_full)
+    if first_extra is None:
+        first_extra = first_chunk_extra(chunk_warmup, warmup_full)
+    if chunk_len is None:
+        chunk_len = plan_chunk_len(counts, sm_budget, chunk_warmup, warmup_full if warmup_full >= 0 else chunk_warmup,
+                                   first_extra=first_extra)
+    if chunk_len >= max(counts):
+        chunk_len = 0
+    precision = precision or prec_def
+    if boundary_tol is None:
+        boundary_tol = tol_def
+    return dict(chunk_len=chunk_len, chunk_warmup=chunk_warmup, warmup_full=warmup_full, first_extra=first_extra, precision=precision,
+                mode=mode, prec={'f32': _lib.MOSH2_F32, 'f64': _lib.MOSH2_F64}[precision], tol=boundary_tol if verify else None)
+
+
+class _Laps:
+    """Host time between consecutive calls, by name (``b200['host_ms']`` of ``mosh_stageii``)."""
+
+    def __init__(self):
+        self.ms = {}
+        self.t = time.perf_counter()
+
+    def __call__(self, name: str):
+        now = time.perf_counter()
+        self.ms[name] = self.ms.get(name, 0.0) + (now - self.t) * 1e3
+        self.t = now
+
+
+class _SeqResult:
+    """Rows [a, b) of a batch job's ResultArrays: the result arrays of one capture."""
+
+    def __init__(self, res: '_lib.ResultArrays', a: int, b: int):
+        for k in ('fullpose', 'pose', 'trans', 'dmpls', 'markers_sim', 'errs', 'status', 'counters'):
+            setattr(self, k, getattr(res, k)[a:b].copy())
+        self.nd = res.nd
+
+
+def _solve_launch(subs, sched: dict, t0: float, laps: Optional[_Laps] = None):
+    """One verified launch of the captures of the subjects ``subs`` (``_subject``), back to back on the job's frame axis in
+    the order given: a batch job of the subject's model (mosh2_job_create_batch) for one subject, a multi-model job
+    (mosh2_job_create_multi) for several.  ``sched``: ``_resolve_schedule``.  Every capture uploads its own raw marker table
+    into its range of the job (mosh2_job_upload_markers_range); the host-adapter captures go up in one ``job.upload``.
+
+    Returns the per-capture dictionaries, in frame-axis order, each with the capture's own ``b200`` entries (status, counters,
+    frame ids, adapter), and the figures of the launch (device time, chunks, schedule, boundary check, totals).  Sets the
+    ``offset`` of every capture record on the frame axis.  ``laps``: the host-time laps of ``mosh_stageii``."""
+    laps = laps or _Laps()
+    seqs = [(sub, s) for sub in subs for s in sub['seqs']]
+    counts = [s['F'] for _, s in seqs]
+    kw = dict(chunk_len=sched['chunk_len'], chunk_warmup=sched['chunk_warmup'], warmup_full=sched['warmup_full'],
+              first_extra=sched['first_extra'], precision=sched['prec'])
+    own = [sub for sub in subs if sub['model'] is None]
+    for sub in own:
+        sub['model'] = _lib.Model(sub['pk'], device=sub['device'])
+    laps('model_create_ms')
+    try:
+        if len(subs) == 1:
+            job = subs[0]['model'].job(counts, subs[0]['opts'], **kw)
+        else:
+            job = _lib.multi_job([sub['model'] for sub in subs], [k for k, sub in enumerate(subs) for _ in sub['seqs']], counts,
+                                 subs[0]['opts'], **kw)
+        laps('job_create_ms')
+        try:
+            offsets = job.seq_offsets
+            host = [q for q, (_, s) in enumerate(seqs) if s['raw_cols'] is None]
+            if len(seqs) == 1 and host:             # one host-adapter capture fills the frame axis
+                job.upload(seqs[0][1]['obs'], seqs[0][1]['vis'])
+            elif host:
+                # host-adapter captures: one upload of the whole frame axis; the device-adapter ranges are written over it
+                obs = np.zeros((job.n_frames, subs[0]['pk'].n_markers, 3))
+                vis = np.zeros((job.n_frames, subs[0]['pk'].n_markers), dtype=bool)
+                for q in host:
+                    obs[offsets[q]:offsets[q + 1]], vis[offsets[q]:offsets[q + 1]] = seqs[q][1]['obs'], seqs[q][1]['vis']
+                job.upload(obs, vis)
+            for q, (_, s) in enumerate(seqs):       # issued back to back: every call stages its own rows
+                if s['raw_cols'] is not None:
+                    m, rot = s['mocap'], s['cfg'].mocap.rotate
+                    job.upload_markers_range(int(offsets[q]), s['F'], m.raw, s['raw_cols'], s['sel'].start, s['sel'].step,
+                                             m.unit_per_metre, None if rot is None else _rotation_xyz(rot))
+            side = {'ms': 0.0}
+
+            def host_side():                        # the result-independent half of every output, behind the solve
+                t_side = time.perf_counter()
+                for _, s in seqs:
+                    if s['raw_cols'] is not None:
+                        s['obs'], s['vis'] = s['mocap'].frames_for_labels(s['labels'], s['sel'])
+                    s['lists'] = observation_lists(s['obs'], s['vis'], s['labels'])
+                    s['markers_orig'] = s['mocap'].markers[s['sel']]
+                side['ms'] = (time.perf_counter() - t_side) * 1e3
+
+            bad, report = launch_verified(job, sched['tol'], while_running=host_side)
+            res = download_verified(job, bad, report)
+            laps('solve_ms')
+            laps.ms['overlapped_host_ms'] = side['ms']
+            n_chunks, totals = job.num_chunks, job.totals()
+        finally:
+            job.close()
+    finally:
+        for sub in own:
+            sub['model'].close()
+    laps('close_ms')
+
+    outs = []
+    for q, (sub, s) in enumerate(seqs):
+        s['offset'] = int(offsets[q])
+        r = res if len(seqs) == 1 else _SeqResult(res, int(offsets[q]), int(offsets[q + 1]))
+        data = assemble_stageii_data(r, s['obs'], s['vis'], s['labels'], sub['pk'], sub['flags'], bool(sub['opts'].optimize_dynamics),
+                                     s['lists'])
+        m = s['mocap']
+        solved = (r.status & _lib.ST_SOLVED) != 0
+        data['stageii_debug_details'].update({
+            'markers_orig': s['markers_orig'],
+            'labels_orig': m.labels,
+            'mocap_fname': s['fname'],
+            'mocap_frame_rate': m.frame_rate,
+            'mocap_time_length': m.time_length(),
+            'b200': {'device_adapter': s['raw_cols'] is not None, 'status': r.status.copy(), 'counters': r.counters.copy(),
+                     'pose_reduced': r.pose[solved], 'frame_ids': np.nonzero(solved)[0]},
+        })
+        outs.append(data)
+    laps('assemble_ms')
+    n_fb = int(((res.status & _lib.ST_GN_FALLBACK) != 0).sum())
+    if n_fb:
+        logger.warning('%d frames hit a non-positive-definite Gauss-Newton system (Cauchy step used)', n_fb)
+    figures = {'kernel_ms': float(sum(report['kernel_ms'])), 'wall_s': time.time() - t0, 'chunks': n_chunks}
+    figures.update({k: sched[k] for k in ('chunk_len', 'chunk_warmup', 'warmup_full', 'first_extra', 'precision', 'mode')})
+    figures.update(boundary_check=report, totals=totals)
+    return outs, figures
 
 
 def mosh_stageii(mocap_fname: str, cfg, markers_latent: np.ndarray, latent_labels: list, betas: np.ndarray,
@@ -478,118 +637,22 @@ def mosh_stageii(mocap_fname: str, cfg, markers_latent: np.ndarray, latent_label
     order, units) runs on the GPU from the raw marker table of the file; False = on the host in front of the solve.
     """
     t0 = time.time()
-    lap = {}
-    tl = [time.perf_counter()]
-
-    def mark(name):
-        now = time.perf_counter()
-        lap[name] = lap.get(name, 0.0) + (now - tl[0]) * 1e3
-        tl[0] = now
-
-    if mode not in BOUNDARY_TOL:
-        raise ValueError(f"mode must be 'fast' or 'exact', not {mode!r}")
-    mocap = MocapSession(mocap_fname, mocap_unit=cfg.mocap.unit, mocap_rotate=cfg.mocap.rotate,
-                         labels_map=labels_map,
-                         only_subjects=[cfg.mocap.subject_name] if cfg.mocap.multi_subject else None)
-    mark('read_mocap_ms')
-    if subject_cache:
-        pk, opts, flags, model, cache_hit = subject_for(cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname, device)
+    laps = _Laps()
+    _check_mode(mode)
+    cap = _read_capture(mocap_fname, cfg, latent_labels, labels_map, device_adapter)
+    laps('read_mocap_ms')
+    sub = _subject([cap], cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname, device, subject_cache)
+    laps('prepare_ms')
+    sched = _resolve_schedule(sub['pk'], mode, [cap['F']], chunk_len, chunk_warmup, warmup_full, first_extra, precision, verify,
+                              boundary_tol, sm_budget)
+    laps('dense_view_ms')
+    (data,), figures = _solve_launch([sub], sched, t0, laps)
+    if cap['raw_cols'] is not None:             # the table rows the selection spans (float64) and the column map
+        h2d = ((cap['F'] - 1) * cap['sel'].step + 1) * cap['mocap'].raw.shape[1] * 24 + 4 * len(cap['labels'])
     else:
-        pk, opts, flags = prepare_stageii(cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname)
-        model, cache_hit = None, False
-    mark('prepare_ms')
-    dyn = bool(opts.optimize_dynamics)
-    w_def, wf_def, prec_def, tol_def = default_schedule(pk.model_type, mode, pk.n_dmpl)
-    chunk_warmup = w_def if chunk_warmup is None else int(chunk_warmup)
-    warmup_full = (wf_def if chunk_warmup == w_def else -1) if warmup_full is None else int(warmup_full)
-    precision = precision or prec_def
-    if boundary_tol is None:
-        boundary_tol = tol_def
-
-    selected_frames, raw_cols, obs, vis, F = _select_input(mocap, cfg, latent_labels, device_adapter)
-    if first_extra is None:
-        first_extra = first_chunk_extra(chunk_warmup, warmup_full)
-    if chunk_len is None:
-        chunk_len = plan_chunk_len([F], sm_budget, chunk_warmup, warmup_full if warmup_full >= 0 else chunk_warmup,
-                                   first_extra=first_extra)
-    if chunk_len >= F:
-        chunk_len = 0
-    prec = {'f32': _lib.MOSH2_F32, 'f64': _lib.MOSH2_F64}[precision]
-    mark('dense_view_ms')
-
-    own_model = model is None
-    if own_model:
-        model = _lib.Model(pk, device=device)
-    mark('model_create_ms')
-    try:
-        job = model.job(F, opts, chunk_len=chunk_len, chunk_warmup=chunk_warmup, warmup_full=warmup_full, precision=prec,
-                        first_extra=first_extra)
-        mark('job_create_ms')
-        try:
-            # the result-independent half of the output (per-frame observation / label lists, the copy of the original
-            # markers) is put together on the host while the device solves
-            side = {}
-
-            def host_side():
-                t_side = time.perf_counter()
-                if raw_cols is not None:
-                    side['obs'], side['vis'] = mocap.frames_for_labels(list(latent_labels), selected_frames)
-                side['lists'] = observation_lists(side.get('obs', obs), side.get('vis', vis), latent_labels)
-                side['markers_orig'] = mocap.markers[selected_frames]
-                side['ms'] = (time.perf_counter() - t_side) * 1e3
-
-            if raw_cols is not None:
-                rot = None if cfg.mocap.rotate is None else _rotation_xyz(cfg.mocap.rotate)
-                job.upload_markers(mocap.raw, raw_cols, selected_frames.start, selected_frames.step, mocap.unit_per_metre, rot)
-            res, report = solve_verified(job, obs, vis, tol=boundary_tol if verify else None, while_running=host_side)
-            if raw_cols is not None:
-                obs, vis = side['obs'], side['vis']
-            mark('solve_ms')
-            lap['overlapped_host_ms'] = side.get('ms', 0.0)
-            kernel_ms = float(sum(report['kernel_ms']))
-            n_chunks = job.num_chunks
-            totals = job.totals()
-        finally:
-            job.close()
-    finally:
-        if own_model:
-            model.close()
-
-    mark('close_ms')
-    data = assemble_stageii_data(res, obs, vis, latent_labels, pk, flags, dyn, side.get('lists'))
-    mark('assemble_ms')
-    dbg = data['stageii_debug_details']
-    dbg.update({
-        'markers_orig': side['markers_orig'] if 'markers_orig' in side else mocap.markers[selected_frames],
-        'labels_orig': mocap.labels,
-        'mocap_fname': mocap_fname,
-        'mocap_frame_rate': mocap.frame_rate,
-        'mocap_time_length': mocap.time_length(),
-        'b200': {
-            'kernel_ms': kernel_ms, 'wall_s': time.time() - t0, 'chunks': n_chunks, 'chunk_len': chunk_len,
-            'chunk_warmup': chunk_warmup, 'warmup_full': warmup_full, 'first_extra': first_extra, 'precision': precision, 'mode': mode,
-            'boundary_check': report, 'totals': totals, 'host_ms': lap, 'subject_cache_hit': cache_hit,
-            'device_adapter': raw_cols is not None,
-            'h2d_bytes': int(((F - 1) * selected_frames.step + 1) * mocap.raw.shape[1] * 24 + 4 * len(latent_labels)) if raw_cols is not None
-            else int(obs.size * (4 if precision == 'f32' else 8) + vis.size),
-            'status': res.status.copy(),
-            'counters': res.counters.copy(), 'pose_reduced': res.pose[(res.status & _lib.ST_SOLVED) != 0],
-            'frame_ids': np.nonzero((res.status & _lib.ST_SOLVED) != 0)[0],
-        },
-    })
-    n_fb = int(((res.status & _lib.ST_GN_FALLBACK) != 0).sum())
-    if n_fb:
-        logger.warning('%d frames hit a non-positive-definite Gauss-Newton system (Cauchy step used)', n_fb)
+        h2d = cap['obs'].size * (4 if sched['precision'] == 'f32' else 8) + cap['vis'].size
+    data['stageii_debug_details']['b200'].update(figures, host_ms=laps.ms, subject_cache_hit=sub['cache_hit'], h2d_bytes=int(h2d))
     return data
-
-
-class _SeqResult:
-    """Rows [a, b) of a batch job's ResultArrays: the result arrays of one capture."""
-
-    def __init__(self, res: '_lib.ResultArrays', a: int, b: int):
-        for k in ('fullpose', 'pose', 'trans', 'dmpls', 'markers_sim', 'errs', 'status', 'counters'):
-            setattr(self, k, getattr(res, k)[a:b].copy())
-        self.nd = res.nd
 
 
 def mosh_stageii_batch(mocap_fnames, cfg, markers_latent: np.ndarray, latent_labels: list, betas: np.ndarray, marker_meta: dict,
@@ -609,106 +672,19 @@ def mosh_stageii_batch(mocap_fnames, cfg, markers_latent: np.ndarray, latent_lab
     status / counters / frame ids and, under ``'batch'``, the figures of the whole launch (device time, chunks, boundary
     check, totals), marked ``'shared': True`` -- the same for every capture of the call."""
     t0 = time.time()
-    if mode not in BOUNDARY_TOL:
-        raise ValueError(f"mode must be 'fast' or 'exact', not {mode!r}")
-    mocap_fnames = list(mocap_fnames)
-    if not mocap_fnames:
+    _check_mode(mode)
+    seqs = [_read_capture(fn, cfg, latent_labels, labels_map, device_adapter) for fn in mocap_fnames]
+    if not seqs:
         raise ValueError('no captures given')
-    only = [cfg.mocap.subject_name] if cfg.mocap.multi_subject else None
-    seqs = []
-    for fn in mocap_fnames:
-        mocap = MocapSession(fn, mocap_unit=cfg.mocap.unit, mocap_rotate=cfg.mocap.rotate, labels_map=labels_map, only_subjects=only)
-        sel, raw_cols, obs, vis, F = _select_input(mocap, cfg, latent_labels, device_adapter)
-        seqs.append(dict(fname=fn, mocap=mocap, sel=sel, raw_cols=raw_cols, obs=obs, vis=vis, F=F))
-    if subject_cache:
-        pk, opts, flags, model, cache_hit = subject_for(cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname, device)
-    else:
-        pk, opts, flags = prepare_stageii(cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname)
-        model, cache_hit = None, False
-    dyn = bool(opts.optimize_dynamics)
-    w_def, wf_def, prec_def, tol_def = default_schedule(pk.model_type, mode, pk.n_dmpl)
-    chunk_warmup = w_def if chunk_warmup is None else int(chunk_warmup)
-    warmup_full = (wf_def if chunk_warmup == w_def else -1) if warmup_full is None else int(warmup_full)
-    precision = precision or prec_def
-    if boundary_tol is None:
-        boundary_tol = tol_def
+    sub = _subject(seqs, cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname, device, subject_cache)
     counts = [s['F'] for s in seqs]
-    if first_extra is None:
-        first_extra = first_chunk_extra(chunk_warmup, warmup_full)
-    if chunk_len is None:
-        chunk_len = plan_chunk_len(counts, sm_budget, chunk_warmup, warmup_full if warmup_full >= 0 else chunk_warmup,
-                                   first_extra=first_extra)
-    if chunk_len >= max(counts):
-        chunk_len = 0
-    prec = {'f32': _lib.MOSH2_F32, 'f64': _lib.MOSH2_F64}[precision]
-    labels = list(latent_labels)
-
-    own_model = model is None
-    if own_model:
-        model = _lib.Model(pk, device=device)
-    try:
-        job = model.job(counts, opts, chunk_len=chunk_len, chunk_warmup=chunk_warmup, warmup_full=warmup_full, precision=prec,
-                        first_extra=first_extra)
-        try:
-            offsets = job.seq_offsets
-            if any(s['raw_cols'] is None for s in seqs):
-                # host-adapter captures: one upload of the whole frame axis; the device-adapter ranges are written over it
-                obs = np.zeros((job.n_frames, pk.n_markers, 3))
-                vis = np.zeros((job.n_frames, pk.n_markers), dtype=bool)
-                for k, s in enumerate(seqs):
-                    if s['raw_cols'] is None:
-                        obs[offsets[k]:offsets[k + 1]], vis[offsets[k]:offsets[k + 1]] = s['obs'], s['vis']
-                job.upload(obs, vis)
-            rot = None if cfg.mocap.rotate is None else _rotation_xyz(cfg.mocap.rotate)
-            for k, s in enumerate(seqs):            # issued back to back: every call stages its own rows
-                if s['raw_cols'] is not None:
-                    m = s['mocap']
-                    job.upload_markers_range(int(offsets[k]), s['F'], m.raw, s['raw_cols'], s['sel'].start, s['sel'].step,
-                                             m.unit_per_metre, rot)
-
-            def host_side():                        # the result-independent half of every output, behind the solve
-                for s in seqs:
-                    if s['raw_cols'] is not None:
-                        s['obs'], s['vis'] = s['mocap'].frames_for_labels(labels, s['sel'])
-                    s['lists'] = observation_lists(s['obs'], s['vis'], labels)
-                    s['markers_orig'] = s['mocap'].markers[s['sel']]
-
-            bad, report = launch_verified(job, boundary_tol if verify else None, while_running=host_side)
-            res = download_verified(job, bad, report)
-            kernel_ms = float(sum(report['kernel_ms']))
-            n_chunks = job.num_chunks
-            totals = job.totals()
-        finally:
-            job.close()
-    finally:
-        if own_model:
-            model.close()
-
-    batch = {'shared': True, 'captures': len(seqs), 'frames': int(sum(counts)), 'kernel_ms': kernel_ms, 'wall_s': time.time() - t0,
-             'chunks': n_chunks, 'chunk_len': chunk_len, 'chunk_warmup': chunk_warmup, 'warmup_full': warmup_full,
-             'first_extra': first_extra, 'precision': precision, 'mode': mode, 'boundary_check': report, 'totals': totals,
-             'subject_cache_hit': cache_hit}
-    out = []
-    for k, s in enumerate(seqs):
-        r = _SeqResult(res, int(offsets[k]), int(offsets[k + 1]))
-        data = assemble_stageii_data(r, s['obs'], s['vis'], labels, pk, flags, dyn, s.get('lists'))
-        m = s['mocap']
-        solved = (r.status & _lib.ST_SOLVED) != 0
-        data['stageii_debug_details'].update({
-            'markers_orig': s['markers_orig'] if 'markers_orig' in s else m.markers[s['sel']],
-            'labels_orig': m.labels,
-            'mocap_fname': s['fname'],
-            'mocap_frame_rate': m.frame_rate,
-            'mocap_time_length': m.time_length(),
-            'b200': {'batch': batch, 'batch_index': k, 'frame_offset': int(offsets[k]), 'device_adapter': s['raw_cols'] is not None,
-                     'status': r.status.copy(), 'counters': r.counters.copy(), 'pose_reduced': r.pose[solved],
-                     'frame_ids': np.nonzero(solved)[0]},
-        })
-        out.append(data)
-    n_fb = int(((res.status & _lib.ST_GN_FALLBACK) != 0).sum())
-    if n_fb:
-        logger.warning('%d frames hit a non-positive-definite Gauss-Newton system (Cauchy step used)', n_fb)
-    return out
+    sched = _resolve_schedule(sub['pk'], mode, counts, chunk_len, chunk_warmup, warmup_full, first_extra, precision, verify,
+                              boundary_tol, sm_budget)
+    outs, figures = _solve_launch([sub], sched, t0)
+    batch = {'shared': True, 'captures': len(seqs), 'frames': int(sum(counts)), **figures, 'subject_cache_hit': sub['cache_hit']}
+    for q, (s, data) in enumerate(zip(seqs, outs)):
+        data['stageii_debug_details']['b200'].update(batch=batch, batch_index=q, frame_offset=s['offset'])
+    return outs
 
 
 def kernel_shape_key(pk) -> tuple:
@@ -760,123 +736,35 @@ def mosh_stageii_subjects(subjects, *, device: int = 0, mode: str = 'fast', chun
     ``'shared': True``, and ``'launches'``, the number of launches of the call."""
     global SUBJECT_CACHE_SIZE
     t0 = time.time()
-    if mode not in BOUNDARY_TOL:
-        raise ValueError(f"mode must be 'fast' or 'exact', not {mode!r}")
+    _check_mode(mode)
     subjects = list(subjects)
     bound = SUBJECT_CACHE_SIZE
     SUBJECT_CACHE_SIZE = max(bound, len(subjects))      # (every model of the call stays open until its launch is done)
     try:
         subs = []
         for s in subjects:
-            cfg = s['cfg']
-            fnames = list(s['mocap_fnames'])
-            if not fnames:
+            seqs = [_read_capture(fn, s['cfg'], s['latent_labels'], labels_map, device_adapter) for fn in s['mocap_fnames']]
+            if not seqs:
                 raise ValueError('a subject without captures')
-            only = [cfg.mocap.subject_name] if cfg.mocap.multi_subject else None
-            seqs = []
-            for fn in fnames:
-                mocap = MocapSession(fn, mocap_unit=cfg.mocap.unit, mocap_rotate=cfg.mocap.rotate, labels_map=labels_map, only_subjects=only)
-                sel, raw_cols, obs, vis, F = _select_input(mocap, cfg, s['latent_labels'], device_adapter)
-                seqs.append(dict(fname=fn, mocap=mocap, sel=sel, raw_cols=raw_cols, obs=obs, vis=vis, F=F))
-            pk, opts, flags, model, cache_hit = subject_for(cfg, s['markers_latent'], s['latent_labels'], s['betas'], s['marker_meta'],
-                                                            s.get('v_template_fname'), device)
-            key = subject_launch_key(pk, opts, mode)
-            subs.append(dict(cfg=cfg, seqs=seqs, pk=pk, opts=opts, flags=flags, model=model, cache_hit=cache_hit, sched=key[2],
-                             key=key, labels=list(s['latent_labels'])))
-        groups = launch_groups([s['key'] for s in subs])
-        out = [None] * len(subs)
+            subs.append(_subject(seqs, s['cfg'], s['markers_latent'], s['latent_labels'], s['betas'], s['marker_meta'],
+                                 s.get('v_template_fname'), device))
+        groups = launch_groups([subject_launch_key(sub['pk'], sub['opts'], mode) for sub in subs])
+        out = [[] for _ in subs]
         for g, members in enumerate(groups):
-            _solve_subject_group([subs[i] for i in members], g, len(groups), t0, chunk_len, chunk_warmup, warmup_full,
-                                 first_extra, precision, verify, boundary_tol, sm_budget, mode)
-            for i in members:
-                out[i] = subs[i]['out']
+            group = [subs[i] for i in members]
+            counts = [s['F'] for sub in group for s in sub['seqs']]
+            sched = _resolve_schedule(group[0]['pk'], mode, counts, chunk_len, chunk_warmup, warmup_full, first_extra, precision,
+                                      verify, boundary_tol, sm_budget)
+            outs, figures = _solve_launch(group, sched, t0)
+            batch = {'shared': True, 'launch': g, 'launches': len(groups), 'subjects': len(group), 'captures': len(counts),
+                     'frames': int(sum(counts)), **figures, 'subject_cache_hits': [sub['cache_hit'] for sub in group]}
+            seqs = [(k, i, s) for k, i in enumerate(members) for s in subs[i]['seqs']]
+            for q, ((k, i, s), data) in enumerate(zip(seqs, outs)):
+                data['stageii_debug_details']['b200'].update(batch=batch, batch_index=q, subject_index=k, frame_offset=s['offset'])
+                out[i].append(data)
     finally:
         SUBJECT_CACHE_SIZE = bound
         while len(_SUBJECT_CACHE) > SUBJECT_CACHE_SIZE:
             _, old = _SUBJECT_CACHE.popitem(last=False)
             old['model'].close()
     return out
-
-
-def _solve_subject_group(group, g, n_groups, t0, chunk_len, chunk_warmup, warmup_full, first_extra, precision, verify,
-                         boundary_tol, sm_budget, mode):
-    """One launch of ``mosh_stageii_subjects``: the captures of the subjects of ``group`` back to back on one multi-model job;
-    sets every member's ``'out'``."""
-    w_def, wf_def, prec_def, tol_def = group[0]['sched']
-    chunk_warmup = w_def if chunk_warmup is None else int(chunk_warmup)
-    warmup_full = (wf_def if chunk_warmup == w_def else -1) if warmup_full is None else int(warmup_full)
-    precision = precision or prec_def
-    if boundary_tol is None:
-        boundary_tol = tol_def
-    seqs = [(k, s) for k, sub in enumerate(group) for s in sub['seqs']]
-    counts = [s['F'] for _, s in seqs]
-    if first_extra is None:
-        first_extra = first_chunk_extra(chunk_warmup, warmup_full)
-    if chunk_len is None:
-        chunk_len = plan_chunk_len(counts, sm_budget, chunk_warmup, warmup_full if warmup_full >= 0 else chunk_warmup,
-                                   first_extra=first_extra)
-    if chunk_len >= max(counts):
-        chunk_len = 0
-    prec = {'f32': _lib.MOSH2_F32, 'f64': _lib.MOSH2_F64}[precision]
-    pk0 = group[0]['pk']
-    job = _lib.multi_job([sub['model'] for sub in group], [k for k, _ in seqs], counts, group[0]['opts'], chunk_len=chunk_len,
-                         chunk_warmup=chunk_warmup, warmup_full=warmup_full, first_extra=first_extra, precision=prec)
-    try:
-        offsets = job.seq_offsets
-        if any(s['raw_cols'] is None for _, s in seqs):
-            # host-adapter captures: one upload of the whole frame axis; the device-adapter ranges are written over it
-            obs = np.zeros((job.n_frames, pk0.n_markers, 3))
-            vis = np.zeros((job.n_frames, pk0.n_markers), dtype=bool)
-            for q, (_, s) in enumerate(seqs):
-                if s['raw_cols'] is None:
-                    obs[offsets[q]:offsets[q + 1]], vis[offsets[q]:offsets[q + 1]] = s['obs'], s['vis']
-            job.upload(obs, vis)
-        for q, (k, s) in enumerate(seqs):          # issued back to back: every call stages its own rows
-            if s['raw_cols'] is not None:
-                rot = group[k]['cfg'].mocap.rotate
-                m = s['mocap']
-                job.upload_markers_range(int(offsets[q]), s['F'], m.raw, s['raw_cols'], s['sel'].start, s['sel'].step,
-                                         m.unit_per_metre, None if rot is None else _rotation_xyz(rot))
-
-        def host_side():                            # the result-independent half of every output, behind the solve
-            for k, s in seqs:
-                if s['raw_cols'] is not None:
-                    s['obs'], s['vis'] = s['mocap'].frames_for_labels(group[k]['labels'], s['sel'])
-                s['lists'] = observation_lists(s['obs'], s['vis'], group[k]['labels'])
-                s['markers_orig'] = s['mocap'].markers[s['sel']]
-
-        bad, report = launch_verified(job, boundary_tol if verify else None, while_running=host_side)
-        res = download_verified(job, bad, report)
-        kernel_ms = float(sum(report['kernel_ms']))
-        n_chunks = job.num_chunks
-        totals = job.totals()
-    finally:
-        job.close()
-
-    batch = {'shared': True, 'launch': g, 'launches': n_groups, 'subjects': len(group), 'captures': len(seqs),
-             'frames': int(sum(counts)), 'kernel_ms': kernel_ms, 'wall_s': time.time() - t0, 'chunks': n_chunks, 'chunk_len': chunk_len,
-             'chunk_warmup': chunk_warmup, 'warmup_full': warmup_full, 'first_extra': first_extra, 'precision': precision, 'mode': mode,
-             'boundary_check': report, 'totals': totals, 'subject_cache_hits': [sub['cache_hit'] for sub in group]}
-    for sub in group:
-        sub['out'] = []
-    for q, (k, s) in enumerate(seqs):
-        sub = group[k]
-        r = _SeqResult(res, int(offsets[q]), int(offsets[q + 1]))
-        data = assemble_stageii_data(r, s['obs'], s['vis'], sub['labels'], sub['pk'], sub['flags'], bool(sub['opts'].optimize_dynamics),
-                                     s.get('lists'))
-        m = s['mocap']
-        solved = (r.status & _lib.ST_SOLVED) != 0
-        data['stageii_debug_details'].update({
-            'markers_orig': s['markers_orig'] if 'markers_orig' in s else m.markers[s['sel']],
-            'labels_orig': m.labels,
-            'mocap_fname': s['fname'],
-            'mocap_frame_rate': m.frame_rate,
-            'mocap_time_length': m.time_length(),
-            'b200': {'batch': batch, 'batch_index': q, 'subject_index': k, 'frame_offset': int(offsets[q]),
-                     'device_adapter': s['raw_cols'] is not None, 'status': r.status.copy(), 'counters': r.counters.copy(),
-                     'pose_reduced': r.pose[solved], 'frame_ids': np.nonzero(solved)[0]},
-        })
-        sub['out'].append(data)
-    n_fb = int(((res.status & _lib.ST_GN_FALLBACK) != 0).sum())
-    if n_fb:
-        logger.warning('%d frames hit a non-positive-definite Gauss-Newton system (Cauchy step used)', n_fb)

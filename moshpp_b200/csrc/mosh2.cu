@@ -427,10 +427,7 @@ struct mosh2_job {
     void *d_lin = nullptr;                       // linearise mode: states in, normal equations / Jacobian rows / residuals out
     size_t lin_bytes = 0;
     int lin_mode = 0, lin_step = 1;
-    void *h_raw = nullptr, *d_raw = nullptr;     // raw marker table of mosh2_job_upload_markers (pinned staging, device copy)
-    int *d_cols = nullptr;
-    size_t raw_bytes = 0;
-    // mosh2_job_upload_markers_range: one staging slot per upload in flight.  A slot holds the table rows, the rotation and
+    // mosh2_job_upload_markers[_range]: one staging slot per upload in flight.  A slot holds the table rows, the rotation and
     // the column map (pinned, and their device copy); `done` is recorded behind the gather kernel that reads them, and a
     // slot is only refilled once its event has completed, so uploads of several captures can be queued back to back.
     struct RangeSlot { void *h = nullptr, *d = nullptr; size_t bytes = 0; cudaEvent_t done = nullptr; };
@@ -832,41 +829,9 @@ int mosh2_job_upload(mosh2_job *j, const double *obs, const uint8_t *vis) {
 
 int mosh2_job_upload_markers(mosh2_job *j, const double *markers, int32_t n_file_frames, int32_t n_cols, const int32_t *col_of_marker,
                              int32_t frame_start, int32_t frame_step, double unit_per_metre, const double *rot3x3) {
-    if (!j || !markers || !col_of_marker) return fail(MOSH2_E_INVALID, "null argument");
-    const int F = j->n_frames, M = j->model->n_markers;
-    if (n_cols < 1 || frame_step < 1 || frame_start < 0 || !(unit_per_metre > 0) ||
-        size_t(frame_start) + size_t(F - 1) * frame_step >= size_t(n_file_frames))
-        return fail(MOSH2_E_INVALID, "frames %d + k*%d (k < %d) do not fit a file of %d frames", frame_start, frame_step, F, n_file_frames);
-    for (int i = 0; i < M; ++i)
-        if (col_of_marker[i] >= n_cols) return fail(MOSH2_E_INVALID, "marker %d: column %d of %d", i, col_of_marker[i], n_cols);
-    CU(cudaSetDevice(j->model->device));
-    const int dv = j->model->device;
-    // the rows [frame_start, last used frame] of the table, whole (all columns), through pinned staging
-    const size_t rows = size_t(F - 1) * frame_step + 1, bytes = rows * n_cols * 3 * sizeof(double), extra = 16 * sizeof(double);
-    if (bytes + extra > j->raw_bytes) {
-        g_blocks.put(-1, j->h_raw); g_blocks.put(dv, j->d_raw);
-        j->h_raw = j->d_raw = nullptr; j->raw_bytes = 0;
-        CU(g_blocks.get(-1, bytes + extra, &j->h_raw));
-        CU(g_blocks.get(dv, bytes + extra, &j->d_raw));
-        j->raw_bytes = bytes + extra;
-    }
-    if (!j->d_cols) CU(g_blocks.get(dv, size_t(M) * sizeof(int), reinterpret_cast<void **>(&j->d_cols)));
-    CU(cudaStreamSynchronize(j->stream));          // (the staging buffers may still feed an earlier upload)
-    char *h = static_cast<char *>(j->h_raw);
-    memcpy(h, markers + size_t(frame_start) * n_cols * 3, bytes);
-    if (rot3x3) memcpy(h + bytes, rot3x3, 9 * sizeof(double));
-    CU(cudaMemcpyAsync(j->d_raw, h, bytes + (rot3x3 ? 9 * sizeof(double) : 0), cudaMemcpyHostToDevice, j->stream));
-    CU(cudaMemcpyAsync(j->d_cols, col_of_marker, size_t(M) * sizeof(int), cudaMemcpyHostToDevice, j->stream));
-    const size_t n = size_t(F) * M;
-    const int blocks = int((n + 255) / 256);
-    const double *d_raw = static_cast<const double *>(j->d_raw);
-    const double *d_rot = rot3x3 ? reinterpret_cast<const double *>(static_cast<const char *>(j->d_raw) + bytes) : nullptr;
-    if (j->precision == MOSH2_F64)
-        gather_markers_kernel<double><<<blocks, 256, 0, j->stream>>>(d_raw, n_cols, j->d_cols, M, F, frame_step, unit_per_metre, d_rot, static_cast<double *>(j->d_obs), j->d_vis);
-    else
-        gather_markers_kernel<float><<<blocks, 256, 0, j->stream>>>(d_raw, n_cols, j->d_cols, M, F, frame_step, unit_per_metre, d_rot, static_cast<float *>(j->d_obs), j->d_vis);
-    CU(cudaGetLastError());
-    return 0;
+    if (!j) return fail(MOSH2_E_INVALID, "null argument");
+    return mosh2_job_upload_markers_range(j, 0, j->n_frames, markers, n_file_frames, n_cols, col_of_marker, frame_start, frame_step,
+                                          unit_per_metre, rot3x3);
 }
 
 int mosh2_job_upload_markers_range(mosh2_job *j, int32_t frame0, int32_t nfr, const double *markers, int32_t n_file_frames, int32_t n_cols,
@@ -913,15 +878,15 @@ int mosh2_job_upload_markers_range(mosh2_job *j, int32_t frame0, int32_t nfr, co
     memcpy(h + o_cols, col_of_marker, size_t(M) * sizeof(int32_t));
     CU(cudaMemcpyAsync(slot->d, h, total, cudaMemcpyHostToDevice, j->stream));
     const char *d = static_cast<const char *>(slot->d);
-    const double *d_raw = reinterpret_cast<const double *>(d), *d_rot = rot3x3 ? reinterpret_cast<const double *>(d + bytes) : nullptr;
+    const double *d_table = reinterpret_cast<const double *>(d), *d_rot = rot3x3 ? reinterpret_cast<const double *>(d + bytes) : nullptr;
     const int *d_cols = reinterpret_cast<const int *>(d + o_cols);
     const size_t n = size_t(nfr) * M, o0 = size_t(frame0) * M;
     const int blocks = int((n + 255) / 256);
     if (j->precision == MOSH2_F64)
-        gather_markers_kernel<double><<<blocks, 256, 0, j->stream>>>(d_raw, n_cols, d_cols, M, nfr, frame_step, unit_per_metre, d_rot,
+        gather_markers_kernel<double><<<blocks, 256, 0, j->stream>>>(d_table, n_cols, d_cols, M, nfr, frame_step, unit_per_metre, d_rot,
                                                                      static_cast<double *>(j->d_obs) + 3 * o0, j->d_vis + o0);
     else
-        gather_markers_kernel<float><<<blocks, 256, 0, j->stream>>>(d_raw, n_cols, d_cols, M, nfr, frame_step, unit_per_metre, d_rot,
+        gather_markers_kernel<float><<<blocks, 256, 0, j->stream>>>(d_table, n_cols, d_cols, M, nfr, frame_step, unit_per_metre, d_rot,
                                                                     static_cast<float *>(j->d_obs) + 3 * o0, j->d_vis + o0);
     CU(cudaGetLastError());
     CU(cudaEventRecord(slot->done, j->stream));
@@ -1149,12 +1114,10 @@ void mosh2_job_destroy(mosh2_job *j) {
                     static_cast<void *>(j->d_delta), j->d_obs, j->d_out, static_cast<void *>(j->d_vis), static_cast<void *>(j->d_status),
                     static_cast<void *>(j->d_counters), static_cast<void *>(j->d_totals), static_cast<void *>(j->d_prof), j->d_gws})
         g_blocks.put(dv, p);
-    g_blocks.put(dv, j->d_raw);
     g_blocks.put(dv, j->d_lin);
-    g_blocks.put(dv, j->d_cols);
     g_blocks.put(dv, j->d_models);
     g_blocks.put(dv, j->d_model_of_chunk);
-    for (void *p : {j->h_obs, j->h_out, static_cast<void *>(j->h_vis), static_cast<void *>(j->h_status), static_cast<void *>(j->h_counters), j->h_raw})
+    for (void *p : {j->h_obs, j->h_out, static_cast<void *>(j->h_vis), static_cast<void *>(j->h_status), static_cast<void *>(j->h_counters)})
         g_blocks.put(-1, p);
     for (auto &s : j->range_slots) {        // (the stream is idle: every slot's copy and kernel have finished)
         g_blocks.put(-1, s.h);

@@ -327,26 +327,18 @@ class Job:
                                                  C.byref(schedule), precision, C.byref(self.handle))
             model._check(rc, 'mosh2_job_create_multi')
         self.result = ResultArrays(n_frames, pack_dims(model.pk))
-        self._keep = None
 
     def upload(self, obs: np.ndarray, vis: np.ndarray):
         obs = np.ascontiguousarray(obs, dtype=np.float64)
         vis8 = np.ascontiguousarray(vis, dtype=np.uint8)
-        self._keep = (obs, vis8)
         self.model._check(self.lib.mosh2_job_upload(self.handle, _ptr(obs, _f64p), _ptr(vis8, _u8p)), 'mosh2_job_upload')
 
     def upload_markers(self, raw: np.ndarray, col_of_marker, frame_start: int, frame_step: int, unit_per_metre: float, rot3x3=None):
-        """The mocap input adapter on the device (mosh2_job_upload_markers): ``raw`` = the capture file's marker table
+        """The mocap input adapter on the device over the whole frame axis (``upload_markers_range`` from frame 0, as
+        mosh2_job_upload_markers does): ``raw`` = the capture file's marker table
         [file frames, file columns, 3] float64 in file units; ``col_of_marker[i]`` = file column of latent marker i (-1: absent);
         job frame f = file frame frame_start + f * frame_step."""
-        raw = np.ascontiguousarray(raw, dtype=np.float64)
-        cols = np.ascontiguousarray(col_of_marker, dtype=np.int32)
-        assert raw.ndim == 3 and raw.shape[2] == 3 and cols.shape == (self.model.pk.n_markers,)
-        rot = None if rot3x3 is None else np.ascontiguousarray(rot3x3, dtype=np.float64).reshape(3, 3)
-        self._keep = (raw, cols, rot)
-        self.model._check(self.lib.mosh2_job_upload_markers(self.handle, _ptr(raw, _f64p), raw.shape[0], raw.shape[1], _ptr(cols, _i32p),
-                                                            int(frame_start), int(frame_step), float(unit_per_metre),
-                                                            _ptr(rot, _f64p) if rot is not None else None), 'mosh2_job_upload_markers')
+        self.upload_markers_range(0, self.n_frames, raw, col_of_marker, frame_start, frame_step, unit_per_metre, rot3x3)
 
     def upload_markers_range(self, frame0: int, n: int, raw: np.ndarray, col_of_marker, frame_start: int, frame_step: int,
                              unit_per_metre: float, rot3x3=None):
