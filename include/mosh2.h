@@ -184,7 +184,7 @@ int mosh2_job_upload_markers_range(mosh2_job *j, int32_t frame0, int32_t n, cons
  * frame's own terms are data, the pose prior (+ joint-angle term) and, with step == 2, the finger term, (optimize_face)
  * the jaw and expression terms and (optimize_dynamics of the job's options, at the job's wt_dmpl) the DMPL term, under opt's
  * wt_data / wt_poseB / wt_poseH / wt_poseF / wt_expr taken as they are (Stage I's annealed weights; no visibility
- * scaling).  step 1 / 2 picks the
+ * scaling) and opt's optimize_fingers; every other option is the job's (opt may be NULL: the job's weights).  step 1 / 2 picks the
  * free-variable list free1 / free2 of the model description (n columns).  Outputs (host, float64, any pointer may be NULL):
  *   errs [F][8] SSE per term, markers_sim [F][M][3], r [F][3M] weighted data residual (sim - obs) wt_data (0 where invisible),
  *   vp [F][3M][3] posed attachment vertices; with build != 0 also A [F][n][n], g [F][n] (normal equations of the frame's own

@@ -163,116 +163,20 @@ struct DevModel {
     ~DevModel() {
         for (void *p : owned) g_blocks.put(device, p);
     }
-    template <class T, class U>
-    int up(const U *src, size_t n, const T **dst) {
-        *dst = nullptr;
-        if (n == 0) {       // keep a valid pointer so kernels can form addresses
-            void *p = nullptr;
-            CU(g_blocks.get(device, 16, &p));
-            owned.push_back(p);
-            *dst = static_cast<const T *>(p);
-            return 0;
-        }
-        std::vector<T> tmp(n);
-        for (size_t i = 0; i < n; ++i) tmp[i] = static_cast<T>(src[i]);
-        void *p = nullptr;
-        CU(g_blocks.get(device, n * sizeof(T), &p));
-        owned.push_back(p);
-        CU(cudaMemcpy(p, tmp.data(), n * sizeof(T), cudaMemcpyHostToDevice));
-        *dst = static_cast<const T *>(p);
-        return 0;
-    }
+    // the tables of mosh2_host::build_model, each copied to a block of the cache
     int build(const mosh2_model_desc &d) {
-        const size_t nJ = d.n_joints, S = size_t(3) * d.n_markers, nd = d.n_dmpl;
-        m.nJ = d.n_joints; m.M = d.n_markers; m.body_dof = d.body_dof; m.p_red = d.p_red;
-        m.n_hand_red = d.n_hand_red; m.n_hand_full = d.n_hand_full; m.nd = d.n_dmpl; m.kw = d.kw;
-        m.prior_k = d.prior_k; m.prior_d = d.prior_d;
-        m.n1 = d.n_free1; m.n2 = d.n_free2; m.finger_lo = d.finger_lo; m.finger_hi = d.finger_hi;
-        m.n_expr = d.n_expr; m.face_lo = d.face_lo; m.face_hi = d.face_hi;
-        m.n_jang = d.n_jangles;
-        for (int i = 0; i < d.n_jangles && i < mosh2::kMaxJangles; ++i) { m.jang_id[i] = d.jangles_ids[i]; m.jang_sign[i] = real(d.jangles_signs[i]); }
-        int rc;
-        if ((rc = up<int>(d.parents, nJ, &m.parents))) return rc;
-        std::vector<int> order(nJ), ids(d.prior_d);
-        std::vector<double> hct;
-        {   // joints sorted by depth (stable): parents before children
-            std::vector<int> depth(nJ, 0);
-            for (size_t j = 0; j < nJ; ++j) { int dj = 0; for (int a = d.parents[j]; a >= 0; a = d.parents[a]) ++dj; depth[j] = dj; }
-            for (size_t j = 0; j < nJ; ++j) order[j] = int(j);
-            std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return depth[a] < depth[b]; });
-            if ((rc = up<int>(order.data(), nJ, &m.fk_order))) return rc;
-        }
-        if ((rc = up<int>(d.w_joint, S * d.kw, &m.w_joint))) return rc;
-        {   // dense blocks of the hand-PCA matrix (rows with the same non-zero column range), stored transposed
-            mosh2::HandBlock blocks[mosh2::kMaxHandBlocks];
-            const int nb = mosh2_host::hand_blocks(d.hand_comps, d.n_hand_red, d.n_hand_full, blocks, hct);
-            m.hb_n = nb;
-            for (int b = 0; b < nb; ++b) m.hb[b] = blocks[b];
-            m.hct_size = int(hct.size());
-            if ((rc = up<real>(hct.data(), hct.size(), &m.hct))) return rc;
-        }
-        if ((rc = up<real>(d.hands_mean, d.n_hand_full, &m.hands_mean))) return rc;
-        if ((rc = up<real>(d.v0, S * 3, &m.v0))) return rc;
-        if ((rc = up<real>(d.sd, S * 3 * nd, &m.sd))) return rc;
-        {   // pose-blend table twice: [(nJ-1)][9 e][3 c][Sp] (eval: four slots per 16-byte load, no padding) and
-            // [(nJ-1)][9 e][3M slots][x y z -] (build: one slot per 16-byte load)
-            const size_t S3 = size_t(3) * d.n_markers;
-            const size_t Sp = (S3 + 3) & ~size_t(3);
-            std::vector<double> pdc((nJ - 1) * 27 * Sp, 0.0), pd4((nJ - 1) * 9 * S3 * 4, 0.0);
-            for (size_t j = 0; j + 1 < nJ; ++j)
-                for (size_t sl = 0; sl < S3; ++sl)
-                    for (int c = 0; c < 3; ++c)
-                        for (int e = 0; e < 9; ++e) {
-                            const double v = d.pd[(j * 3 * S3 + 3 * sl + c) * 9 + e];
-                            pdc[((j * 9 + e) * 3 + c) * Sp + sl] = v;
-                            pd4[((j * 9 + e) * S3 + sl) * 4 + c] = v;
-                        }
-            if ((rc = up<real>(pdc.data(), pdc.size(), &m.pdc))) return rc;
-            if ((rc = up<real>(pd4.data(), pd4.size(), &m.pd4))) return rc;
-        }
-        if ((rc = up<real>(d.w_val, S * d.kw, &m.w_val))) return rc;
-        if ((rc = up<real>(d.j0, nJ * 3, &m.j0))) return rc;
-        if ((rc = up<real>(d.jd, nJ * 3 * nd, &m.jd))) return rc;
-        if ((rc = up<real>(d.coefs, size_t(d.n_markers) * 3, &m.coefs))) return rc;
-        if ((rc = up<real>(d.prior_means, size_t(d.prior_k) * d.prior_d, &m.prior_means))) return rc;
-        {
-            const size_t K = d.prior_k, D = d.prior_d, D4 = (D + 3) & ~size_t(3);
-            m.prior_d4 = int(D4);
-            std::vector<double> q4(K * D * D4, 0.0);
-            for (size_t k = 0; k < K; ++k)
-                for (size_t i = 0; i < D; ++i)
-                    for (size_t l = 0; l < D; ++l) q4[(k * D + i) * D4 + l] = d.prior_Q[(k * D + i) * D + l];
-            if ((rc = up<real>(q4.data(), q4.size(), &m.prior_Q4))) return rc;
-            std::vector<double> qt(K * D * D4, 0.0);
-            for (size_t k = 0; k < K; ++k)
-                for (size_t i = 0; i < D; ++i)
-                    for (size_t l = 0; l < D; ++l) qt[(k * D + l) * D4 + i] = d.prior_Q[(k * D + i) * D + l];
-            if ((rc = up<real>(qt.data(), qt.size(), &m.prior_Qt))) return rc;
-        }
-        if ((rc = up<real>(d.prior_neglogw, d.prior_k, &m.prior_nlw))) return rc;
-        {
-            for (int i = 0; i < d.prior_d; ++i) ids[i] = d.prior_ids ? d.prior_ids[i] : d.prior_off + i;
-            if ((rc = up<int>(ids.data(), ids.size(), &m.prior_ids))) return rc;
-        }
-        if ((rc = up<int>(d.free1, d.n_free1, &m.free1))) return rc;
-        if ((rc = up<int>(d.free2, d.n_free2, &m.free2))) return rc;
-        {   // image of the staged shared-memory tables (mosh2::carve / stage_image): what a chunk fetches with one bulk copy
-            const mosh2::Dims dd = mosh2::make_dims(m);
-            mosh2::Work<real, false> w{};
-            mosh2::Arena S{mosh2::kSmemHeader}, G{0};
-            mosh2::carve<real, false>(w, dd, m, S, G);
-            std::vector<unsigned char> img(w.stage_bytes, 0);
-            const int *isrc[6] = {d.parents, order.data(), d.w_joint, d.free1, d.free2, ids.data()};
-            const double *rsrc[9] = {d.w_val, d.v0, d.coefs, d.j0, d.hands_mean, d.prior_means, d.prior_neglogw, d.jd, hct.data()};
-            mosh2::stage_image(w, dd, m.hct_size, m.n_hand_full, [&](uint32_t ofs, int id, size_t n) {
-                if (id < 6) { int *o = reinterpret_cast<int *>(img.data() + ofs); for (size_t i = 0; i < n; ++i) o[i] = isrc[id][i]; }
-                else { real *o = reinterpret_cast<real *>(img.data() + ofs); for (size_t i = 0; i < n; ++i) o[i] = real(rsrc[id - 6][i]); }
-            });
-            const unsigned char *blob = nullptr;
-            if ((rc = up<unsigned char>(img.data(), img.size(), &blob))) return rc;
-            m.stage_blob = blob;
-        }
-        return 0;
+        int rc = 0;
+        auto place = [&](const auto *host, size_t n) -> decltype(host) {
+            void *p = nullptr;
+            cudaError_t e = g_blocks.get(device, n ? n * sizeof(*host) : 16, &p);   // (n = 0: still a valid address for the kernels)
+            if (e == cudaSuccess) {
+                owned.push_back(p);
+                if (n) e = cudaMemcpy(p, host, n * sizeof(*host), cudaMemcpyHostToDevice);
+            }
+            if (e != cudaSuccess) { rc = fail(MOSH2_E_CUDA, "model upload: %s", cudaGetErrorString(e)); return nullptr; }
+            return static_cast<decltype(host)>(p);
+        };
+        return mosh2_host::build_model<real>(d, m, place) ? 0 : rc;
     }
 };
 
@@ -401,7 +305,7 @@ struct mosh2_model {
 struct mosh2_job {
     mosh2_model *model = nullptr;
     int precision = MOSH2_F32;
-    int n_frames = 0, chunk_len = 0, warmup = 0, warm_full = 0, n_chunks = 1;
+    int n_frames = 0, n_chunks = 1;
     int *d_chunk_tab = nullptr, *d_chunk_ids = nullptr, *d_warm_f = nullptr;
     void *d_warm_x = nullptr;
     float *d_delta = nullptr;
@@ -427,6 +331,7 @@ struct mosh2_job {
     void *d_lin = nullptr;                       // linearise mode: states in, normal equations / Jacobian rows / residuals out
     size_t lin_bytes = 0;
     int lin_mode = 0, lin_step = 1;
+    mosh2_host::LinLayout lin{};                 // layout of d_lin for the current call
     // mosh2_job_upload_markers[_range]: one staging slot per upload in flight.  A slot holds the table rows, the rotation and
     // the column map (pinned, and their device copy); `done` is recorded behind the gather kernel that reads them, and a
     // slot is only refilled once its event has completed, so uploads of several captures can be queued back to back.
@@ -448,29 +353,21 @@ namespace {
 
 template <class real, bool BIG>
 cudaError_t launch_kernel(mosh2_job *j, const mosh2::Model<real> &m, const mosh2::Job<real> &job, int threads) {
-    const mosh2::Dims d = mosh2::make_dims(m);
-    mosh2::Work<real, BIG> w{};
-    mosh2::Arena S{mosh2::kSmemHeader}, G{0};
-    mosh2::carve<real, BIG>(w, d, m, S, G);
-    w.tc = (w.tc_ok && threads >= 128) ? 1 : 0;
+    const mosh2_host::Layout<real, BIG> L = mosh2_host::layout<real, BIG>(m, mosh2::kSmemHeader, threads);
     const cudaError_t e = cudaFuncSetAttribute(mosh2_stageii_kernel<real, BIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(j->smem));
     if (e != cudaSuccess) return e;
-    mosh2_stageii_kernel<real, BIG><<<j->launch_blocks, threads, j->smem, j->stream>>>(m, job, w, d);
+    mosh2_stageii_kernel<real, BIG><<<j->launch_blocks, threads, j->smem, j->stream>>>(m, job, L.w, L.d);
     return cudaGetLastError();
 }
 
 template <class real, bool BIG>
 cudaError_t launch_multi_kernel(mosh2_job *j, const mosh2::Job<real> &job, int threads) {
     const mosh2::Model<real> &m = *reinterpret_cast<const mosh2::Model<real> *>(j->h_models.data());
-    const mosh2::Dims d = mosh2::make_dims(m);
-    mosh2::Work<real, BIG> w{};
-    mosh2::Arena S{mosh2_host::multi_smem_header<real>()}, G{0};
-    mosh2::carve<real, BIG>(w, d, m, S, G);
-    w.tc = (w.tc_ok && threads >= 128) ? 1 : 0;
+    const mosh2_host::Layout<real, BIG> L = mosh2_host::layout<real, BIG>(m, mosh2_host::multi_smem_header<real>(), threads);
     const cudaError_t e = cudaFuncSetAttribute(mosh2_stageii_multi_kernel<real, BIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(j->smem));
     if (e != cudaSuccess) return e;
     mosh2_stageii_multi_kernel<real, BIG><<<j->launch_blocks, threads, j->smem, j->stream>>>(
-        static_cast<const mosh2::Model<real> *>(j->d_models), j->d_model_of_chunk, job, w, d);
+        static_cast<const mosh2::Model<real> *>(j->d_models), j->d_model_of_chunk, job, L.w, L.d);
     return cudaGetLastError();
 }
 
@@ -489,17 +386,7 @@ int launch(mosh2_job *j, const mosh2::Model<real> &m) {
     job.status = j->d_status; job.counters = j->d_counters; job.totals = j->d_totals; job.prof = j->d_prof;
     job.gws = static_cast<char *>(j->d_gws); job.gws_stride = j->gws_stride;
     job.lin_mode = j->lin_mode; job.lin_step = j->lin_step;
-    if (j->lin_mode) {      // layout of d_lin (reals): x [F][NX] | A [F][n][n] | g [F][n] | J [F][3M][n] | r [F][3M] | vp [F][9M]
-        const size_t F = j->n_frames, M = j->model->n_markers, NX = 3 + j->model->p_red + j->model->n_dmpl;
-        const size_t n = j->lin_step == 2 ? m.n2 : m.n1;
-        real *p = static_cast<real *>(j->d_lin);
-        job.lin_x = p; p += F * NX;
-        job.lin_A = p; p += F * n * n;
-        job.lin_g = p; p += F * n;
-        job.lin_J = p; p += F * 3 * M * n;
-        job.lin_r = p; p += F * 3 * M;
-        job.lin_vp = p;
-    }
+    if (j->lin_mode) mosh2_host::bind_lin(job, static_cast<real *>(j->d_lin), j->lin);
     job.opt = j->opt;
     int threads = threads_for<real>();
     if (const char *e = getenv("MOSH2_DEV_THREADS")) {      // development aid: any multiple of 32 from 128 up to the launch bound
@@ -522,8 +409,8 @@ int launch(mosh2_job *j, const mosh2::Model<real> &m) {
 template <class real>
 int linearize(mosh2_job *j, const mosh2::Model<real> &m, int32_t step, int32_t build, const double *x, const mosh2_lin_out *out) {
     const size_t F = j->n_frames, M = j->model->n_markers, NX = 3 + j->model->p_red + j->model->n_dmpl;
-    const size_t n = step == 2 ? m.n2 : m.n1, n2 = m.n2 > m.n1 ? m.n2 : m.n1;
-    const size_t words = F * (NX + n2 * n2 + n2 + 3 * M * n2 + 3 * M + 9 * M);
+    const size_t n = step == 2 ? m.n2 : m.n1;
+    const size_t words = mosh2_host::lin_layout(F, M, NX, std::max(m.n1, m.n2)).words;      // room for either step
     if (words * sizeof(real) > j->lin_bytes) {
         g_blocks.put(j->model->device, j->d_lin);
         j->d_lin = nullptr; j->lin_bytes = 0;
@@ -535,18 +422,15 @@ int linearize(mosh2_job *j, const mosh2::Model<real> &m, int32_t step, int32_t b
     CU(cudaMemsetAsync(j->d_out, 0, j->n_out * j->esz, j->stream));
     j->lin_mode = build ? 2 : 1;
     j->lin_step = step;
+    j->lin = mosh2_host::lin_layout(F, M, NX, n);
     j->subset = false;
     j->launch_blocks = int(F);
     const int rc = launch<real>(j, m);
     j->lin_mode = 0;
     j->launch_blocks = j->n_chunks;
     if (rc) return rc;
-    const real *p = static_cast<const real *>(j->d_lin) + F * NX;
-    const real *dA = p; p += F * n * n;
-    const real *dg = p; p += F * n;
-    const real *dJ = p; p += F * 3 * M * n;
-    const real *dr = p; p += F * 3 * M;
-    const real *dvp = p;
+    const real *p = static_cast<const real *>(j->d_lin), *dA = p + j->lin.A, *dg = p + j->lin.g, *dJ = p + j->lin.J;
+    const real *dr = p + j->lin.r, *dvp = p + j->lin.vp;
     const real *dout = static_cast<const real *>(j->d_out);
     struct Back { double *dst; const real *src; size_t cnt; std::vector<real> h; };
     Back b[7] = {{out->r, dr, F * 3 * M, {}}, {out->vp, dvp, F * 9 * M, {}}, {out->errs, dout + j->o_errs, F * mosh2::N_ERR, {}},
@@ -589,30 +473,8 @@ void mosh2_default_options(mosh2_options *o) {
 int mosh2_model_create(const mosh2_model_desc *d, int device, mosh2_model **out) {
     if (!d || !out) return fail(MOSH2_E_INVALID, "null argument");
     *out = nullptr;
-    if (d->n_joints < 1 || d->n_markers < 1 || d->kw < 1 || d->kw > 8 || d->n_free1 < 1 || d->n_free2 < d->n_free1)
-        return fail(MOSH2_E_INVALID, "inconsistent model sizes");
-    if (d->n_expr < 0 || d->n_expr > d->n_dmpl || d->face_lo < 0 || d->face_hi < d->face_lo || d->face_hi > d->p_red)
-        return fail(MOSH2_E_INVALID, "inconsistent face description: n_expr=%d of %d linear coefficients, jaw ids [%d, %d)", d->n_expr,
-                    d->n_dmpl, d->face_lo, d->face_hi);
-    if (d->n_joints > 254) return fail(MOSH2_E_TOO_LARGE, "%d joints (max 254)", d->n_joints);
-    if (d->n_jangles < 0 || d->n_jangles > mosh2::kMaxJangles || (d->n_jangles > 0 && (!d->jangles_ids || !d->jangles_signs)))
-        return fail(MOSH2_E_INVALID, "joint-angle term: %d entries (max %d)", d->n_jangles, mosh2::kMaxJangles);
-    for (int i = 0; i < d->n_jangles; ++i)
-        if (d->jangles_ids[i] < 0 || d->jangles_ids[i] >= d->p_red) return fail(MOSH2_E_INVALID, "joint-angle entry %d refers to pose id %d of %d", i, d->jangles_ids[i], d->p_red);
-    for (int i = 0; i < d->prior_d; ++i) {
-        const int id = d->prior_ids ? d->prior_ids[i] : d->prior_off + i;
-        if (id < 0 || id >= d->p_red) return fail(MOSH2_E_INVALID, "prior dimension %d refers to pose id %d of %d", i, id, d->p_red);
-    }
-    for (int j = 0; j < d->n_joints; ++j) {
-        int depth = 1;
-        for (int a = d->parents[j]; a >= 0; a = d->parents[a]) {
-            if (a >= d->n_joints || ++depth > d->n_joints) return fail(MOSH2_E_INVALID, "parents[] is not a forest (joint %d)", j);
-        }
-        if (depth > mosh2::kMaxDepth) return fail(MOSH2_E_TOO_LARGE, "kinematic chain of joint %d is %d levels deep (max %d)", j, depth, mosh2::kMaxDepth);
-    }
-    if (d->body_dof + d->n_hand_full != 3 * d->n_joints || d->body_dof + d->n_hand_red != d->p_red)
-        return fail(MOSH2_E_INVALID, "pose layout mismatch: body_dof=%d hand_full=%d hand_red=%d p_red=%d joints=%d",
-                    d->body_dof, d->n_hand_full, d->n_hand_red, d->p_red, d->n_joints);
+    std::string msg;
+    if (const int rc = mosh2_host::check_model_desc(*d, &msg)) return fail(rc, "%s", msg.c_str());
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
         cudaGetLastError();
@@ -660,23 +522,13 @@ int mosh2_job_create_batch(mosh2_model *m, const mosh2_options *opt, int32_t n_s
     mosh2_job *j = new (std::nothrow) mosh2_job;
     if (!j) return fail(MOSH2_E_INVALID, "out of host memory");
     j->model = m; j->precision = precision; j->n_frames = n_frames;
-    const int chunk_len = sched ? sched->chunk_len : 0, chunk_warmup = sched ? sched->chunk_warmup : 0;
-    j->chunk_len = chunk_len > 0 ? chunk_len : 0;
-    j->warmup = chunk_warmup > 0 ? chunk_warmup : 0;
-    j->warm_full = (!sched || sched->warmup_full < 0 || sched->warmup_full > j->warmup) ? j->warmup : sched->warmup_full;
-    const int first_extra = (sched && sched->first_extra > 0 && j->chunk_len > 0 && j->warmup > 0) ? sched->first_extra : 0;
-    j->tab = mosh2_host::chunk_table(frame_counts, n_seq, j->chunk_len, j->warmup, j->warm_full, first_extra);
+    j->tab = mosh2_host::schedule_table(sched, frame_counts, n_seq);
     j->tab0 = j->tab;
     const std::vector<int> &tab = j->tab;
     j->n_chunks = int(tab.size() / mosh2::kChunkRec);
     j->launch_blocks = j->n_chunks;
     j->esz = precision == MOSH2_F64 ? 8 : 4;
-    mosh2::Options &o = j->opt;
-    o.wt_data = opt->wt_data; o.wt_poseB = opt->wt_poseB; o.wt_poseH = opt->wt_poseH; o.wt_velo = opt->wt_velo;
-    o.wt_dmpl = opt->wt_dmpl; o.wt_annealing = opt->wt_annealing; o.wt_extrap = opt->wt_extrap_dmpl;
-    o.num_train_markers = opt->num_train_markers; o.delta_0 = opt->delta_0; o.e3_first = opt->e3_first; o.e3 = opt->e3;
-    o.maxiter = opt->maxiter; o.optimize_fingers = opt->optimize_fingers; o.optimize_dynamics = opt->optimize_dynamics;
-    o.wt_poseF = opt->wt_poseF; o.wt_expr = opt->wt_expr; o.optimize_face = opt->optimize_face;
+    j->opt = mosh2_host::to_options(*opt);
 
     size_t gws = 0;
     if (precision == MOSH2_F64) plan_workspace(m->f64.m, &j->smem, &gws, &j->big_in_global);
@@ -837,15 +689,12 @@ int mosh2_job_upload_markers(mosh2_job *j, const double *markers, int32_t n_file
 int mosh2_job_upload_markers_range(mosh2_job *j, int32_t frame0, int32_t nfr, const double *markers, int32_t n_file_frames, int32_t n_cols,
                                    const int32_t *col_of_marker, int32_t frame_start, int32_t frame_step, double unit_per_metre,
                                    const double *rot3x3) {
-    if (!j || !markers || !col_of_marker) return fail(MOSH2_E_INVALID, "null argument");
-    if (frame0 < 0 || nfr < 1 || frame0 > j->n_frames - nfr)
-        return fail(MOSH2_E_INVALID, "frame range [%d, %d) outside the job's %d frames", frame0, frame0 + nfr, j->n_frames);
+    if (!j) return fail(MOSH2_E_INVALID, "null argument");
     const int M = j->model->n_markers;
-    if (n_cols < 1 || frame_step < 1 || frame_start < 0 || !(unit_per_metre > 0) ||
-        size_t(frame_start) + size_t(nfr - 1) * frame_step >= size_t(n_file_frames))
-        return fail(MOSH2_E_INVALID, "frames %d + k*%d (k < %d) do not fit a file of %d frames", frame_start, frame_step, nfr, n_file_frames);
-    for (int i = 0; i < M; ++i)
-        if (col_of_marker[i] >= n_cols) return fail(MOSH2_E_INVALID, "marker %d: column %d of %d", i, col_of_marker[i], n_cols);
+    std::string msg;
+    if (const int rc = mosh2_host::check_marker_range(j->n_frames, M, frame0, nfr, markers, n_file_frames, n_cols, col_of_marker, frame_start,
+                                                      frame_step, unit_per_metre, &msg))
+        return fail(rc, "%s", msg.c_str());
     CU(cudaSetDevice(j->model->device));
     const int dv = j->model->device;
     // slot layout: rows [frame_start, last used frame] of the table (all columns) | rotation (9) | column map (M int32)
@@ -898,10 +747,7 @@ int mosh2_job_linearize(mosh2_job *j, const mosh2_options *opt, int32_t step, in
     if (j->n_chunks < j->n_frames) return fail(MOSH2_E_INVALID, "mosh2_job_linearize needs a job of one-frame chunks (chunk_len = 1)");
     if (j->d_models) return fail(MOSH2_E_INVALID, "mosh2_job_linearize does not take a multi-model job");
     CU(cudaSetDevice(j->model->device));
-    if (opt) {      // the weights of this evaluation (Stage I anneals them between minimisations)
-        mosh2::Options &o = j->opt;
-        o.wt_data = opt->wt_data; o.wt_poseB = opt->wt_poseB; o.wt_poseH = opt->wt_poseH; o.optimize_fingers = opt->optimize_fingers;
-    }
+    if (opt) mosh2_host::apply_call_weights(j->opt, *opt);
     if (j->precision == MOSH2_F64) return linearize<double>(j, j->model->f64.m, step, build, x, out);
     return linearize<float>(j, j->model->f32.m, step, build, x, out);
 }

@@ -49,7 +49,7 @@ gn_kernel(const __grid_constant__ mosh2::Model<real> m, const __grid_constant__ 
 template <class real, bool BIG>
 int run(int threads, const mosh2_model_desc *desc, int n, const double *A, const double *g, double *dgn_out, double *Ag_out,
         int *ok_out) {
-    mosh2::Model<real> m = gn_case::dims_model<real>(*desc);
+    mosh2::Model<real> m = mosh2_host::model_dims<real>(*desc);
     mosh2::Dims d;
     mosh2::Work<real, BIG> w;
     size_t smem = 0, gws_bytes = 0;

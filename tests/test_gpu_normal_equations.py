@@ -268,6 +268,34 @@ def test_kernel_normal_equations_equal_float64(cases, gpu_states, name, step, pr
 
 
 @pytest.mark.gpu
+def test_kernel_linearize_takes_the_face_weights_of_the_call(cases, gpu_states, emu_lin):
+    """mosh2_job_linearize evaluates the jaw and expression terms under the call's wt_poseF and wt_expr (Stage I anneals its
+    weights between minimisations), not under those the job was created with: a float64 job created with CF's options and
+    linearised with both weights tripled equals the host build given the tripled weights."""
+    case = cases('CF')
+    pk, opts = _prepare(case)
+    obs, vis, x = gpu_states(case, 'CF')
+    call = lib.Options.from_buffer_copy(opts)
+    call.wt_poseF *= 3
+    call.wt_expr *= 3
+    model = lib.Model(pk, device=0)
+    try:
+        job = model.job(obs.shape[0], opts, chunk_len=1, chunk_warmup=0, precision=lib.MOSH2_F64)
+        try:
+            job.upload(obs, vis)
+            got = job.linearize(x, call, 2, True)['errs']
+        finally:
+            job.close()
+    finally:
+        model.close()
+    want = emu_lin(pk, call, obs, vis, x, 2, 'f64')['errs']
+    for term in ('poseF', 'expr'):
+        ref = want[:, COL[term]]
+        assert np.all(ref > 0), term
+        assert np.abs(got[:, COL[term]] - ref).max() <= F64['sse'] * ref.max(), term
+
+
+@pytest.mark.gpu
 @pytest.mark.parametrize('switch', [('MOSH2_DEV_NO_TC', '1'), ('MOSH2_DEV_TILE', '10'), ('MOSH2_DEV_BIG', '1'),
                                     ('MOSH2_DEV_THREADS', '256'), ('MOSH2_DEV_THREADS', '128')])
 @pytest.mark.parametrize('step', [1, 2])
