@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MOSH2_VERSION 106
+#define MOSH2_VERSION 107
 
 enum {
     MOSH2_OK = 0,
@@ -219,9 +219,13 @@ int mosh2_job_boundary_deltas(mosh2_job *j, int32_t body_ids, float *out);
  * no warm-up; the chunk continues the recursion from the rows the previous launch emitted for the last two solved frames
  * in front of it, exactly as the previous chunk would have gone on (boundary repair); the repair of a chunk stops early once
  * two consecutive re-solved frames lie within merge_tol (rad; translation in 0.1 m) of the rows they replace -- the two
- * trajectories have merged and the remaining rows of the chunk stand (merge_tol = 0: re-solve the whole chunk).  async */
+ * trajectories have merged and the remaining rows of the chunk stand (merge_tol = 0: re-solve the whole chunk).
+ * root_turns (NULL: 0 for every chunk): per listed chunk, full turns added to the angle of the root its cold start finds (the
+ * first-frame alignment returns an angle in [0, pi]).  The sequential pass tracks the root as a free parameter from the first
+ * frame on, so after the body has turned past pi its axis-angle root lies beyond pi; a chunk whose cold start lies behind such
+ * a crossing must start on that branch, u (theta + 2 pi turns), to solve the sequential pass's problem.  async */
 int mosh2_job_relaunch_chunks(mosh2_job *j, int32_t n, const int32_t *chunk_ids, int32_t chunk_warmup, int32_t warmup_full,
-                              double merge_tol);
+                              double merge_tol, const int32_t *root_turns);
 int mosh2_job_download(mosh2_job *j, const mosh2_result *res); /* async D2H + stream sync */
 int mosh2_job_sync(mosh2_job *j);
 /* Results as ONE packed float32 device row per frame, for device-side consumers (NCCL gather): row f =

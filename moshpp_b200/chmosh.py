@@ -361,6 +361,42 @@ def default_schedule(model_type: str, mode: str = 'fast', n_linear: int = 0):
     return DEFAULT_WARMUP, DEFAULT_WARMUP_FULL, 'f32', BOUNDARY_TOL['fast']
 
 
+# A chunk whose warm-up state differs from the emitted row by more than this (rad, root + body pose) may have started on
+# another axis-angle branch of the root: two branches of one rotation lie 2 pi / sqrt(3) > 3.6 rad apart in some component,
+# the boundary deltas of a converged warm-up are below 1e-3.
+ROOT_BRANCH_DELTA = 1.0
+
+
+def root_branch_turns(root: np.ndarray, solved: np.ndarray, ranges: np.ndarray, seq_starts) -> np.ndarray:
+    """Full turns that put every chunk on the root branch of the sequential pass.
+
+    The sequential pass aligns the first frame of a sequence (angle in [0, pi]) and then tracks the root as a free
+    parameter: once the body has turned past pi, its axis-angle root lies beyond pi.  A chunk aligns the first frame of its
+    own warm-up and so starts on the principal branch: behind such a crossing it tracks u (theta - 2 pi n) where the
+    sequential pass tracks u theta.  This pass walks the chunks of every sequence in order and unwraps the emitted root across
+    each chunk boundary -- the first solved root of a chunk onto the equivalent rotation vector u (theta + 2 pi n) nearest to
+    the (unwrapped) last solved root in front of it.  ``root`` [F, 3] emitted roots, ``solved`` [F] bool, ``ranges``
+    [n_chunks, 2] emitted ranges (``Job.chunk_ranges``), ``seq_starts``: first frames of the sequences.  Returns n per chunk
+    (0: the chunk is on the branch of the chunks in front of it)."""
+    starts = set(int(s) for s in seq_starts)
+    turns = np.zeros(len(ranges), dtype=np.int64)
+    last = None                                   # unwrapped last solved root in front of the chunk
+    for c, (a, b) in enumerate(ranges):
+        if int(a) in starts:
+            last = None
+        fs = np.flatnonzero(solved[a:b]) + a
+        if not len(fs):
+            continue
+        r0, r1 = root[fs[0]], root[fs[-1]]
+        if last is not None:
+            th = np.linalg.norm(r0)
+            if th > 0:
+                turns[c] = int(np.round((r0 @ last / th - th) / (2 * np.pi)))
+        th1 = np.linalg.norm(r1)
+        last = r1 * (1 + 2 * np.pi * turns[c] / th1) if th1 > 0 else r1
+    return turns
+
+
 def launch_verified(job, tol, max_rounds: int = 12, while_running=None):
     """Launch + boundary check + repair rounds on the observations the job already holds (device work only; see
     ``solve_verified``).  Returns (chunk ids still over tolerance, report); report['kernel_ms'] lists the device time of
@@ -369,7 +405,8 @@ def launch_verified(job, tol, max_rounds: int = 12, while_running=None):
     job.launch()
     if while_running is not None:
         while_running()
-    report = {'rounds': 0, 'repaired_chunks': [], 'boundary_delta_first': None, 'boundary_delta_max': None, 'unverified_chunks': 0}
+    report = {'rounds': 0, 'repaired_chunks': [], 'boundary_delta_first': None, 'boundary_delta_max': None, 'unverified_chunks': 0,
+              'root_branch_chunks': 0}
     kernel_ms = []
     bad = np.zeros(0, dtype=np.int64)
     if job.schedule.chunk_len <= 0 or tol is None:
@@ -387,6 +424,18 @@ def launch_verified(job, tol, max_rounds: int = 12, while_running=None):
         report['boundary_delta_max'] = d.max(0).tolist()
         if not len(bad) or rnd == max_rounds:
             break
+        if rnd == 0 and d[:, 0].max() > ROOT_BRANCH_DELTA:
+            # chunks on another root branch (root_branch_turns) start again from a cold start on the branch of the
+            # sequential pass, all in this one round; the repair rounds below take over from there
+            res = job.download()
+            turns = root_branch_turns(res.pose[:, :3], (res.status & _lib.ST_SOLVED) != 0, job.chunk_ranges(), job.seq_offsets[:-1])
+            ids = np.flatnonzero(turns)
+            if len(ids):
+                job.relaunch_chunks(ids, job.schedule.chunk_warmup, job.schedule.warmup_full, root_turns=turns[ids])
+                report['rounds'] += 1
+                report['repaired_chunks'].append(len(ids))
+                report['root_branch_chunks'] = int(len(ids))
+                continue
         # of a run of consecutive failing chunks only every other one per round, starting with the first
         take, last = [], -2
         for c in bad:

@@ -771,7 +771,8 @@ int mosh2_job_launch(mosh2_job *j) {
     return launch<float>(j, j->model->f32.m);
 }
 
-int mosh2_job_relaunch_chunks(mosh2_job *j, int32_t n, const int32_t *chunk_ids, int32_t chunk_warmup, int32_t warmup_full, double merge_tol) {
+int mosh2_job_relaunch_chunks(mosh2_job *j, int32_t n, const int32_t *chunk_ids, int32_t chunk_warmup, int32_t warmup_full, double merge_tol,
+                              const int32_t *root_turns) {
     if (!j || n < 1 || !chunk_ids || !(merge_tol >= 0)) return fail(MOSH2_E_INVALID, "bad argument");
     j->merge_tol = merge_tol;
     CU(cudaSetDevice(j->model->device));
@@ -781,6 +782,7 @@ int mosh2_job_relaunch_chunks(mosh2_job *j, int32_t n, const int32_t *chunk_ids,
         if (c < 0 || c >= j->n_chunks) return fail(MOSH2_E_INVALID, "chunk %d out of range (%d chunks)", c, j->n_chunks);
         j->tab[size_t(c) * mosh2::kChunkRec + 3] = chunk_warmup;
         j->tab[size_t(c) * mosh2::kChunkRec + 4] = wf;
+        j->tab[size_t(c) * mosh2::kChunkRec + 5] = root_turns ? root_turns[k] : 0;
     }
     j->tab_dirty = true;
     CU(cudaStreamSynchronize(j->stream));

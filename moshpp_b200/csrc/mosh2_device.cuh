@@ -114,7 +114,7 @@ constexpr int kBS = 4;            // register tile of the J^T J accumulation and
 constexpr int kBlendGroups = 4;   // upper bound of the joint groups of the pose-blend partial sums (run time: 1..3, one round of threads)
 constexpr int kCholNB = 8;        // block column width of the Cholesky factorisation
 constexpr int kMaxHandBlocks = 4;
-constexpr int kChunkRec = 5;      // ints per chunk-table record
+constexpr int kChunkRec = 6;      // ints per chunk-table record
 constexpr int kMaxJangles = 16;   // joint-angle prior entries (the horse model has 12)
 
 struct Cta {
@@ -166,7 +166,8 @@ template <class real>
 struct Job {
     int n_frames, n_chunks;
     const int *chunk_tab;   // [n_chunks][kChunkRec]: first emitted frame, end of the emitted range, first frame of the chunk's
-                            // sequence, warm-up (solved frames), how many of them (the last ones) run the full per-frame schedule
+                            // sequence, warm-up (solved frames), how many of them (the last ones) run the full per-frame schedule,
+                            // full turns added to the root of the chunk's cold start (Solver::procrustes)
     const int *chunk_ids;   // launch of a subset of the chunks: blockIdx.x -> chunk, or null (all chunks)
     double merge_tol;       // resume mode: a re-solved frame within this of the row it replaces counts as merged (rad on root + body pose;
                             // x 10 on the other pose coefficients, x 0.1 m on the translation)
@@ -652,6 +653,7 @@ struct Solver {
     bool fwd_at_x = false;    // the forward scratch of the latest evaluation belongs to the current state w.x ...
     bool fwd_has_prior = false;   // ... including the prior products
     bool resuming = false;    // boundary repair: the chunk continues from emitted rows (run_chunk)
+    int root_turns = 0;       // full turns added to the angle of the cold start's root (run_chunk, procrustes)
     real resume_diff = 0;     // ... and how far the frame just solved is from the row it replaces
     int lin_f = -1;           // linearise mode: the frame this block works on (else -1)
 
@@ -2415,7 +2417,9 @@ struct Solver {
             double qw = V[best], qx = V[4 + best], qy = V[8 + best], qz = V[12 + best];
             if (qw < 0) { qw = -qw; qx = -qx; qy = -qy; qz = -qz; }
             const double vn = sqrt(qx * qx + qy * qy + qz * qz);
-            const double ang = 2 * atan2(vn, qw);
+            // (the angle lies in [0, pi], as the reference's cv2.Rodrigues returns it; a chunk whose cold start lies behind a pi
+            // crossing of the sequence's root is told how many full turns the sequential trajectory has added by then)
+            const double ang = 2 * atan2(vn, qw) + 6.283185307179586 * root_turns;
             double rv[3] = {0, 0, 0};
             if (vn > 1e-300) { rv[0] = qx / vn * ang; rv[1] = qy / vn * ang; rv[2] = qz / vn * ang; }
             const double R[9] = {1 - 2 * (qy * qy + qz * qz), 2 * (qx * qy - qz * qw), 2 * (qx * qz + qy * qw),
@@ -2511,6 +2515,7 @@ struct Solver {
         const int *rec = job.chunk_tab + kChunkRec * chunk;
         const int f_emit = lin ? chunk : rec[0], f_end = lin ? chunk + 1 : rec[1], s0 = lin ? chunk : rec[2];
         const int warmup = lin ? 0 : rec[3], warm_full = lin ? 0 : rec[4];
+        root_turns = lin ? 0 : rec[5];
         int f_begin = f_emit, f_full = f_emit;
         bool short_warmup = false;
         if (cta.tid == 0 && job.warm_f) job.warm_f[chunk] = -1;

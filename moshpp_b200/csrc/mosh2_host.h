@@ -221,7 +221,7 @@ inline void apply_call_weights(mosh2::Options &q, const mosh2_options &o) {
 
 // Chunk table of a job that holds n_seq sequences back to back on its frame axis: kChunkRec ints per chunk -- first
 // emitted frame, end of the emitted range, first frame of the chunk's sequence, warm-up length (solved frames), number of
-// fully solved warm-up frames.  chunk_len <= 0: one chunk per sequence (the reference's sequential pass).  Chunks never
+// fully solved warm-up frames, full turns added to the root of the chunk's cold start (0; mosh2_job_relaunch_chunks sets it).  chunk_len <= 0: one chunk per sequence (the reference's sequential pass).  Chunks never
 // straddle a sequence boundary.  first_extra > 0: the FIRST chunk of every sequence emits chunk_len + first_extra frames --
 // it has no warm-up to solve, so with first_extra = the cost of a warm-up every chunk of the sequence finishes at the same
 // time, and no later chunk starts so close to the sequence start that its walk-back is cut short.
@@ -235,7 +235,7 @@ inline std::vector<int> chunk_table(const int *frame_counts, int n_seq, int chun
         for (int f = 0; f < F;) {
             long long e = (long long)f + L + (f == 0 ? E : 0);
             if (e > F) e = F;
-            const int rec[mosh2::kChunkRec] = {s0 + f, s0 + int(e), s0, warmup, warm_full};
+            const int rec[mosh2::kChunkRec] = {s0 + f, s0 + int(e), s0, warmup, warm_full, 0};
             tab.insert(tab.end(), rec, rec + mosh2::kChunkRec);
             f = int(e);
         }

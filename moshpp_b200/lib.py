@@ -13,7 +13,7 @@ import numpy as np
 
 from .pack import StageIIPack
 
-ABI_VERSION = 106          # MOSH2_VERSION of include/mosh2.h that the ctypes structs below encode
+ABI_VERSION = 107          # MOSH2_VERSION of include/mosh2.h that the ctypes structs below encode
 MOSH2_F32, MOSH2_F64 = 0, 1
 ST_SOLVED, ST_SKIPPED, ST_HAS_VELO, ST_HAS_EXTRAP, ST_GN_FALLBACK, ST_MAXITER, ST_SHORT_WARMUP = 1, 2, 4, 8, 16, 32, 64
 ERR_NAMES = ('data', 'poseB', 'velo', 'poseH', 'dmpl', 'extrap_dmpl', 'poseF', 'expr')   # column order of mosh2_result.errs
@@ -130,7 +130,7 @@ def load_library(path: Optional[str] = None):
     lib.mosh2_job_launch.argtypes = [vp]
     lib.mosh2_job_warm_states.argtypes = [vp, _f64p, _i32p]
     lib.mosh2_job_boundary_deltas.argtypes = [vp, C.c_int32, C.POINTER(C.c_float)]
-    lib.mosh2_job_relaunch_chunks.argtypes = [vp, C.c_int32, _i32p, C.c_int32, C.c_int32, C.c_double]
+    lib.mosh2_job_relaunch_chunks.argtypes = [vp, C.c_int32, _i32p, C.c_int32, C.c_int32, C.c_double, _i32p]
     lib.mosh2_job_download.argtypes = [vp, C.POINTER(Result)]
     lib.mosh2_job_sync.argtypes = [vp]
     lib.mosh2_job_kernel_ms.argtypes = [vp, C.POINTER(C.c_float)]
@@ -418,11 +418,17 @@ class Job:
                           'mosh2_job_boundary_deltas')
         return out.astype(np.float64)
 
-    def relaunch_chunks(self, chunk_ids, chunk_warmup: int, warmup_full: int = -1, merge_tol: float = 0.0):
-        """Re-solves the listed chunks; ``chunk_warmup < 0`` = resume from the emitted rows (mosh2_job_relaunch_chunks)."""
+    def relaunch_chunks(self, chunk_ids, chunk_warmup: int, warmup_full: int = -1, merge_tol: float = 0.0, root_turns=None):
+        """Re-solves the listed chunks; ``chunk_warmup < 0`` = resume from the emitted rows; ``root_turns``: per listed chunk,
+        full turns added to the root angle of its cold start (mosh2_job_relaunch_chunks)."""
         ids = np.ascontiguousarray(chunk_ids, dtype=np.int32)
+        turns = None if root_turns is None else np.ascontiguousarray(root_turns, dtype=np.int32)
+        if turns is not None and turns.shape != ids.shape:
+            raise ValueError('root_turns: one value per chunk')
         self.model._check(self.lib.mosh2_job_relaunch_chunks(self.handle, len(ids), _ptr(ids, _i32p), int(chunk_warmup),
-                                                             int(warmup_full), float(merge_tol)), 'mosh2_job_relaunch_chunks')
+                                                             int(warmup_full), float(merge_tol),
+                                                             None if turns is None else _ptr(turns, _i32p)),
+                          'mosh2_job_relaunch_chunks')
 
     def download(self) -> ResultArrays:
         self.model._check(self.lib.mosh2_job_download(self.handle, C.byref(self.result.c)), 'mosh2_job_download')

@@ -18,6 +18,7 @@ observations, checked against the oracle in tests/test_synth.py.
 """
 from __future__ import annotations
 
+import hashlib
 import os
 import pickle
 from collections import OrderedDict
@@ -443,9 +444,45 @@ def rodrigues_batch(rv: np.ndarray) -> np.ndarray:
     return np.where(small[..., None], np.eye(3) + Ks, R)
 
 
+def rodrigues_inv_batch(R: np.ndarray) -> np.ndarray:
+    """Rotation matrices (..., 3, 3) -> axis-angle (..., 3) with the angle in [0, pi] (away from pi: the skew part; near
+    pi: the axis from the symmetric part)."""
+    r = np.stack([R[..., 2, 1] - R[..., 1, 2], R[..., 0, 2] - R[..., 2, 0], R[..., 1, 0] - R[..., 0, 1]], -1)
+    s = 0.5 * np.linalg.norm(r, axis=-1)
+    th = np.arctan2(s, (np.trace(R, axis1=-2, axis2=-1) - 1.0) * 0.5)
+    out = np.where(th[..., None] < 1e-12, 0.5 * r, r * (th / np.maximum(2.0 * s, 1e-300))[..., None])
+    near_pi = th > np.pi - 1e-3
+    if near_pi.any():
+        c = np.cos(th[near_pi])[:, None, None]
+        B = (0.5 * (R[near_pi] + np.swapaxes(R[near_pi], -1, -2)) - c * np.eye(3)) / (1.0 - c)     # = u u^T
+        k = np.argmax(np.diagonal(B, axis1=-2, axis2=-1), axis=-1)
+        u = B[np.arange(len(B)), :, k]
+        u /= np.linalg.norm(u, axis=-1, keepdims=True)
+        u *= np.where((u * r[near_pi]).sum(-1) < 0, -1.0, 1.0)[:, None]
+        out[near_pi] = u * th[near_pi][:, None]
+    return out
+
+
+def unwrap_axis_angle(rv: np.ndarray) -> np.ndarray:
+    """Axis-angle rows (F, 3) of a rotation trajectory, each replaced by the equivalent rotation vector u (theta + 2 pi n)
+    nearest to the row before: the continuous trajectory an iterative solver warm-started from the previous frame
+    follows (|theta| > pi once it has turned past pi)."""
+    out = np.array(rv, dtype=np.float64)
+    for f in range(1, len(out)):
+        th = np.linalg.norm(out[f])
+        if th < 1e-12:
+            continue
+        u = out[f] / th
+        out[f] = u * (th + 2 * np.pi * np.round((u @ out[f - 1] - th) / (2 * np.pi)))
+    return out
+
+
 def make_motion(p: _pack.StageIIPack, n_frames: int, seed: int, fps: float = 120.0,
-                body_amp: float = 0.35, finger_amp: float = 0.25):
-    """Smooth reduced-pose / translation / DMPL trajectories (SURVEY.md 8(d) "Motion")."""
+                body_amp: float = 0.35, finger_amp: float = 0.25, root_yaw=None):
+    """Smooth reduced-pose / translation / DMPL trajectories (SURVEY.md 8(d) "Motion").  ``root_yaw``: a turn of the
+    whole body about the up (y) axis -- (yaw_start, yaw_end) rad, linear in time, or one yaw per frame -- composed in
+    front of the small root motion; the root is then the continuous axis-angle trajectory (``unwrap_axis_angle``).
+    None keeps the random draws and the motion as they are."""
     rng = np.random.default_rng(seed)
     t = np.arange(n_frames) / fps
     P = p.p_red
@@ -478,6 +515,14 @@ def make_motion(p: _pack.StageIIPack, n_frames: int, seed: int, fps: float = 120
         dm[0] = 0.5 * e[0]
         for k in range(1, n_frames):
             dm[k] = rho * dm[k - 1] + np.sqrt(1 - rho ** 2) * 0.5 * e[k]
+    if root_yaw is not None:
+        yaw = np.asarray(root_yaw, dtype=np.float64)
+        if yaw.shape == (2,) and n_frames != 2:
+            yaw = np.linspace(yaw[0], yaw[1], n_frames)
+        if yaw.shape != (n_frames,):
+            raise ValueError(f'root_yaw: (start, end) or {n_frames} values')
+        R = rodrigues_batch(yaw[:, None] * np.array([0.0, 1.0, 0.0])) @ rodrigues_batch(pose[:, :3])
+        pose[:, :3] = unwrap_axis_angle(rodrigues_inv_batch(R))
     return pose, trans, dm
 
 
@@ -559,13 +604,14 @@ from .cfg import AttrDict, STAGEII_WEIGHTS, default_cfg  # noqa: E402,F401
 def make_case(out_dir: str, config: str = 'C2', *, frames: Optional[int] = None, n_verts: Optional[int] = None,
               seq_idx: int = 0, noise_mm: float = 1.0, dropout: float = 0.03, hand_side: str = 'left',
               write_mocap: bool = True, reuse_model: bool = True, model_seed: int = 0, n_betas: int = 24,
-              expr_start: int = 16, num_expressions: int = 8) -> Dict:
+              expr_start: int = 16, num_expressions: int = 8, root_yaw=None) -> Dict:
     """Writes one synthetic Stage-II case (model, priors, mocap file) and returns everything
     ``mosh_stageii`` needs plus the ground truth.  ``seq_idx`` picks the shape (and with it the latent markers) and the
     motion; ``model_seed`` > 0 writes and uses a second model file of the same family and size (another template, shape
     space and joint regressor; e.g. the other gender's model).  ``n_betas``: shape components of the model file;
     ``expr_start`` / ``num_expressions``: the expression components of the configurations with ``optimize_face``
-    (``REFERENCE_FACE`` is the layout of the reference's SMPL-X face setup)."""
+    (``REFERENCE_FACE`` is the layout of the reference's SMPL-X face setup); ``root_yaw``: a turn of the whole body about
+    the up axis (``make_motion``)."""
     c = dict(CONFIGS[config])
     mt = c['model_type']
     F = int(frames or c['frames'])
@@ -633,7 +679,7 @@ def make_case(out_dir: str, config: str = 'C2', *, frames: Optional[int] = None,
                           optimize_fingers=c['optimize_fingers'], optimize_face=face,
                           expr_start=expr_start if face else 0, num_expressions=num_expressions if face else 0)
     cfg_idx = list(CONFIGS).index(config)
-    pose, trans, dm = make_motion(pk, F, seed=SEED_MOTION + cfg_idx + 1000 * seq_idx)
+    pose, trans, dm = make_motion(pk, F, seed=SEED_MOTION + cfg_idx + 1000 * seq_idx, root_yaw=root_yaw)
     if not c['optimize_fingers'] and pk.n_hand_red:
         pose[:, pk.body_dof:] = 0.0
     mk = forward_markers(pk, pose, trans, dm if pk.n_dmpl else None)
@@ -659,6 +705,8 @@ def make_case(out_dir: str, config: str = 'C2', *, frames: Optional[int] = None,
     # (a model with another shape space, or other expressions, synthesises other observations: a file of its own)
     size = f'_b{n_betas}' if n_betas != 24 else ''
     size += f'_e{expr_start}x{num_expressions}' if face and (expr_start, num_expressions) != (16, 8) else ''
+    if root_yaw is not None:
+        size += '_yaw' + hashlib.blake2b(np.asarray(root_yaw, dtype=np.float64).tobytes(), digest_size=4).hexdigest()
     mocap_fname = os.path.join(out_dir, f'mocap_{config}{side}{size}_{seq_idx:02d}_{F}.{c["mocap_ext"]}')
     if write_mocap:
         if c['mocap_ext'] == 'npz':

@@ -96,11 +96,13 @@ struct HostJob {
 // Sequences back to back on one frame axis, chunked as mosh2_job_create_batch chunks them.  model_of_seq == nullptr: one model
 // (a batch job); else sequence q is solved with descs[model_of_seq[q]] and every chunk binds a copy of its model's record in the
 // multi-model shared-memory header (a multi-model job).  resume_all: then a boundary repair of every chunk, in order -- chunk c
-// continues from the rows chunk c-1 emitted.
+// continues from the rows chunk c-1 emitted.  root_turns (or nullptr): per chunk, full turns added to the root of its cold
+// start (what mosh2_job_relaunch_chunks writes into the chunk record; the chunks of a launch are independent, so setting them
+// before the one pass over the chunks gives the rows of a launch followed by a relaunch of the chunks with turns).
 template <class real>
 int solve(const mosh2_model_desc *const *descs, int n_models, const int *model_of_seq, const mosh2_options &opt, int n_seq,
           const int *counts, const double *obs, const uint8_t *vis, const mosh2_schedule *sched, const mosh2_result &res,
-          bool resume_all = false) {
+          bool resume_all = false, const int *root_turns = nullptr) {
     std::vector<std::unique_ptr<HostModel<real>>> hms;
     for (int k = 0; k < n_models; ++k) {
         std::string msg;
@@ -113,6 +115,8 @@ int solve(const mosh2_model_desc *const *descs, int n_models, const int *model_o
     const unsigned header = model_of_seq ? mosh2_host::multi_smem_header<real>() : mosh2::kSmemHeader;
     HostJob<real> hj(*descs[0], opt, n_frames, obs, vis, hms[0]->m, header);
     hj.set_chunks(mosh2_host::schedule_table(sched, counts, n_seq));
+    if (root_turns)
+        for (int c = 0; c < hj.job.n_chunks; ++c) hj.tab[size_t(c) * mosh2::kChunkRec + 5] = root_turns[c];
     const std::vector<int> moc = model_of_seq ? mosh2_host::model_of_chunks(hj.tab, counts, n_seq, model_of_seq)
                                               : std::vector<int>(size_t(hj.job.n_chunks), 0);
     for (int c = 0; c < hj.job.n_chunks; ++c) hj.run_chunk(c, hms[moc[c]]->m, model_of_seq != nullptr);
@@ -246,4 +250,12 @@ extern "C" int mosh2_emu_solve_resumed(const mosh2_model_desc *desc, const mosh2
                                        int32_t precision, const mosh2_result *res) {
     if (precision == MOSH2_F64) return solve<double>(&desc, 1, nullptr, *opt, 1, &n_frames, obs, vis, sched, *res, true);
     return solve<float>(&desc, 1, nullptr, *opt, 1, &n_frames, obs, vis, sched, *res, true);
+}
+
+// the chunked schedule with the chunk records' root turns (one per chunk of the schedule)
+extern "C" int mosh2_emu_solve_root_turns(const mosh2_model_desc *desc, const mosh2_options *opt, int32_t n_frames,
+                                          const double *obs, const uint8_t *vis, const mosh2_schedule *sched, const int32_t *root_turns,
+                                          int32_t precision, const mosh2_result *res) {
+    if (precision == MOSH2_F64) return solve<double>(&desc, 1, nullptr, *opt, 1, &n_frames, obs, vis, sched, *res, false, root_turns);
+    return solve<float>(&desc, 1, nullptr, *opt, 1, &n_frames, obs, vis, sched, *res, false, root_turns);
 }

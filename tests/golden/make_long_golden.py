@@ -37,6 +37,10 @@ LONG = {
     'C5d': ('C5', dict(frames=320, seq_idx=3)),
     # occlusion gap straddling a chunk boundary (ADVICE r1): built by the test from C2 with frames 90..139 blanked
     'GAP': ('C2', dict(frames=240)),
+    # the whole body turning about the up axis (synth.make_motion root_yaw): the root's axis-angle passes pi once (TURN), or
+    # starts facing backwards and sways around pi, passing it again and again (BACK)
+    'TURN': ('C2', dict(frames=600, root_yaw=(2.0, 5.0))),
+    'BACK': ('C2', dict(frames=600, root_yaw=tuple(np.pi + 0.3 * np.sin(2 * np.pi * 0.4 * np.arange(600) / 120.0 - np.arcsin(1 / 6))))),
 }
 POSE_FRAMES = 2000      # pose / dmpl rows stored per fixture (a contiguous run from the first solved frame)
 
