@@ -418,6 +418,8 @@ class StageI:
         sse = {'data': float(dev['errs'][:, 0].sum())}
         if pk.prior_k:
             sse['poseB'] = float(dev['errs'][:, 1].sum())
+            if len(pk.jangles_ids):         # the horse's joint-angle term (chmosh.py:358-360); the kernel reports it in poseH
+                sse['poseB_jangles'] = float(dev['errs'][:, 3].sum())
         if detailed and self.fingers:
             sse['poseH'] = float(dev['errs'][:, 3].sum())
         if detailed and self.face:
