@@ -353,7 +353,7 @@ namespace {
 
 template <class real, bool BIG>
 cudaError_t launch_kernel(mosh2_job *j, const mosh2::Model<real> &m, const mosh2::Job<real> &job, int threads) {
-    const mosh2_host::Layout<real, BIG> L = mosh2_host::layout<real, BIG>(m, mosh2::kSmemHeader, threads);
+    const mosh2_host::Layout<real, BIG> L = mosh2_host::layout<real, BIG>(m, mosh2::kSmemHeader);
     const cudaError_t e = cudaFuncSetAttribute(mosh2_stageii_kernel<real, BIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(j->smem));
     if (e != cudaSuccess) return e;
     mosh2_stageii_kernel<real, BIG><<<j->launch_blocks, threads, j->smem, j->stream>>>(m, job, L.w, L.d);
@@ -363,7 +363,7 @@ cudaError_t launch_kernel(mosh2_job *j, const mosh2::Model<real> &m, const mosh2
 template <class real, bool BIG>
 cudaError_t launch_multi_kernel(mosh2_job *j, const mosh2::Job<real> &job, int threads) {
     const mosh2::Model<real> &m = *reinterpret_cast<const mosh2::Model<real> *>(j->h_models.data());
-    const mosh2_host::Layout<real, BIG> L = mosh2_host::layout<real, BIG>(m, mosh2_host::multi_smem_header<real>(), threads);
+    const mosh2_host::Layout<real, BIG> L = mosh2_host::layout<real, BIG>(m, mosh2_host::multi_smem_header<real>());
     const cudaError_t e = cudaFuncSetAttribute(mosh2_stageii_multi_kernel<real, BIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(j->smem));
     if (e != cudaSuccess) return e;
     mosh2_stageii_multi_kernel<real, BIG><<<j->launch_blocks, threads, j->smem, j->stream>>>(
@@ -612,7 +612,6 @@ int make_multi(mosh2_job *j, mosh2_model *const *models, int32_t n_models, int32
     for (int k = 0; k < n_models; ++k) {
         recs[k] = dev_model(models[k]);
         recs[k].tile_markers = plan.tile_markers;
-        recs[k].dev_no_tc = plan.dev_no_tc;
     }
     j->h_models.assign(reinterpret_cast<const unsigned char *>(recs.data()), reinterpret_cast<const unsigned char *>(recs.data() + n_models));
     const std::vector<int> moc = mosh2_host::model_of_chunks(j->tab0, frame_counts, n_seq, model_of_seq);

@@ -14,9 +14,10 @@
 //   Jacobian  d v / d w_{a,k} = u_{a,k} x sum_{j in subtree(a)} w_j (p_j - tg_a)            (rigid part)
 //                              + Rskin Pd_j dvec(R_j)/dw_k                                    (pose blend)
 //             with u_{a,k} = Rg_par(a) vee(dR_{a,k} R_a^T); hand columns chained through C^T.
-//   normal eq A = J^T J and g = -J^T r are accumulated marker tile by marker tile (J^T J on the tensor cores: f32 as
-//             split TF32 with mma.sync m16n8k8, f64 with DMMA m8n8k4); the prior, velocity, finger, face and DMPL / expression
-//             terms have closed-form contributions (Q_k = .5 inv(cov_k), diagonals).
+//   normal eq A = J^T J and g = -J^T r are accumulated marker tile by marker tile, in float32 over every marker in one
+//             pass where the workspace fits (J^T J: f32 in register tiles on the CUDA cores, f64 with DMMA m8n8k4 on the tensor
+//             cores); the prior, velocity, finger, face and DMPL / expression terms have closed-form contributions
+//             (Q_k = .5 inv(cov_k), diagonals).
 //   The workspace layout (struct Work) is computed on the host and arrives as a kernel parameter of shared-memory offsets.
 #pragma once
 #include <math.h>
@@ -110,7 +111,7 @@ namespace mosh2 {
 enum { ST_SOLVED = 1, ST_SKIPPED = 2, ST_HAS_VELO = 4, ST_HAS_EXTRAP = 8, ST_GN_FALLBACK = 16, ST_MAXITER = 32, ST_SHORT_WARMUP = 64 };
 enum { ERR_DATA = 0, ERR_POSEB = 1, ERR_VELO = 2, ERR_POSEH = 3, ERR_DMPL = 4, ERR_EXTRAP = 5, ERR_POSEF = 6, ERR_EXPR = 7, N_ERR = 8 };
 
-constexpr int kBS = 4;            // register tile of the J^T J accumulation and of the Cholesky update
+constexpr int kBS = 4;            // register tile of the Cholesky update
 constexpr int kBlendGroups = 4;   // upper bound of the joint groups of the pose-blend partial sums (run time: 1..3, one round of threads)
 constexpr int kCholNB = 8;        // block column width of the Cholesky factorisation
 constexpr int kMaxHandBlocks = 4;
@@ -148,8 +149,9 @@ struct Model {
     int n_jang;                     // animal_horse: joint-angle term exp(2 s x)^2 on these reduced-pose ids (prior/horse_body_prior.py:56-71)
     int jang_id[kMaxJangles];
     real jang_sign[kMaxJangles];
-    int tile_markers;           // markers per Jacobian tile (20 or 10: a warp owns ten), chosen by the host from the shared-memory budget
-    int dev_no_tc;              // development switch (host): 1 = J^T J stays on the CUDA cores
+    int tile_markers;           // markers per Jacobian tile, chosen by the host from the shared-memory budget (plan_workspace)
+    int dev_no_tc;              // not read: the float32 J^T J has one path (CUDA-core register tiles); the test-only host
+                                // build (tests/emu/mosh2_emu.cpp) still assigns it
     const unsigned char *stage_blob;   // the small per-model tables laid out exactly like the staged region of the shared-memory
                                        // workspace (carve(): Work::stage_ofs / stage_bytes); one bulk asynchronous copy per chunk
 };
@@ -426,18 +428,19 @@ struct Work {
     SPtr<uint8_t> c_amask;    // [slot][joint]: bit i set <=> the slot's i-th skinning joint lies in the subtree of the joint
     SPtr<unsigned long long> mbar;   // completion barrier of the table staging
     uint32_t stage_ofs, stage_bytes;   // the staged per-model tables: one contiguous, 16-byte aligned region (c_parents ... hct)
-    int tc_ok;                // the model qualifies for the f32 tensor-core J^T J (f32, workspace in shared memory)
-    int tc;                   // set by the launcher: tensor cores in use
+    BPtr<real, BIG> Pb;       // the pose-blend partial sums of eval(): in Jt, or in Jf when Jt lies over A (one_pass)
+    int one_pass;             // every marker in one Jacobian tile (float32, workspace in shared memory): T3 writes A once per
+                              // build, and the build scratch that T3 no longer reads (Jt, Loc, MtR, u, dtg) lies over A
 };
 
 // ---------------------------------------------------------------------------------------------
-// tensor cores for the J^T J accumulation of the f32 kernel; bulk asynchronous copies
+// split-TF32 J^T J block; bulk asynchronous copies
 // ---------------------------------------------------------------------------------------------
-// A warp computes one 16x16 block of the upper triangle of Jf^T Jf over the rows of a tile with mma.sync m16n8k8 on
-// TF32 operands.  Every Jacobian value is split into a TF32 "hi" part and a TF32 "lo" remainder;
-// hi hi^T goes to one register accumulator, lo hi^T + hi lo^T + lo lo^T to another, and their sum is added to A
-// on the CUDA cores once per tile: close to fp32 accuracy (3xTF32), and the tensor core's truncating additions only
-// ever span the rows of one tile.
+// jtj_block_tf32: a warp computes one 16x16 block of the upper triangle of J^T J with mma.sync m16n8k8 on TF32 operands.
+// Every Jacobian value is split into a TF32 "hi" part and a TF32 "lo" remainder; hi hi^T goes to one register
+// accumulator, lo hi^T + hi lo^T + lo lo^T to another (3xTF32, close to fp32 accuracy).  The kernel does not use it:
+// on the north-star workload it was 1.7 % slower than J^T J on the CUDA cores (DESIGN.md section 8).  It stays for its
+// stand-alone test (tests/tc/jtj_tf32_test.cu).
 constexpr int kMaxDepth = 16;         // deepest kinematic chain the tree walk unrolls (checked at model creation)
 constexpr int kDR = 28;              // floats per joint in dRl: three 3x3 derivative matrices (27) padded to 16-byte vectors
 constexpr int kM3 = 12;              // floats per padded 3x3 matrix (MtR per slot, Loc per marker vertex) and per joint in u (3 x 4)
@@ -553,23 +556,40 @@ M2_HD void carve(Work<real, BIG> &w, const Dims &d, const Model<real> &m, Arena 
     w.mk.ofs = S.take<real>(3 * d.M); w.rm.ofs = S.take<real>(3 * d.M); w.obs.ofs = S.take<real>(3 * d.M);
     w.py.ofs = S.take<real>(d.K * d.D + 1); w.pq.ofs = S.take<real>(d.K + 1); w.pxg.ofs = S.take<real>(d.D + 1);
     // The Cholesky factor is alive only inside gauss_newton(); the Jacobian tiles and the other scratch of build()
-    // (and the pose-blend partial sums of eval(), which live in Jt) are dead there, so they share its storage.
+    // (and the pose-blend partial sums of eval(), Pb) are dead there, so they share its storage.
     // A and the Cholesky factor Lm are adjacent.  The factor is alive only inside gauss_newton(); the scratch of
-    // build() (and the pose-blend partial sums of eval(), which live in Jt) is dead there and is laid over it.
+    // build() (and Pb) is dead there and is laid over it.
+    // With every marker in one tile (one_pass), A is written only by T3, after the last reader of the full-pose hand tile
+    // Jt and the per-build scratch Loc .. dtg: those lie over A, the Jacobian rows Jf (read by T3) behind A, and the
+    // pose-blend partial sums move to Jf (A is alive during eval()).  53 SMPL-H markers with 111 unknowns fit in shared memory
+    // only so.
     {
         w.A.ofs = B.take<real>(size_t(d.n2) * d.lda);
-        w.tc_ok = (sizeof(real) == 4 && !BIG && !m.dev_no_tc) ? 1 : 0;
-        w.tc = 0;
+        w.one_pass = (sizeof(real) == 4 && !BIG && d.tmk >= d.M) ? 1 : 0;
         const size_t mark_b = B.off;
         w.Lm.ofs = B.take<real>(size_t(d.n2 + 1) * d.ld);
         const size_t end_b = B.off;
-        B.off = mark_b;
-        w.Jt.ofs = B.take<real>(d.jt_size);
-        w.Jf.ofs = B.take<real>(3 * d.tmk * d.npad);
         // (with BIG these go to the global workspace as well: in float64, 36 M words each for Loc and MtR and 3 nJ nd for dtg
         // -- 106 KB for SMPL-X with 80 expressions -- do not fit next to the rest of the shared part)
-        w.Loc.ofs = B.take<real>(3 * kM3 * d.M); w.MtR.ofs = B.take<real>(kM3 * d.S);
-        w.u.ofs = B.take<real>(kM3 * d.nJ); w.dtg.ofs = B.take<real>(3 * d.nJ * d.nd + 1);
+        auto scratch = [&] {
+            w.Loc.ofs = B.take<real>(3 * kM3 * d.M); w.MtR.ofs = B.take<real>(kM3 * d.S);
+            w.u.ofs = B.take<real>(kM3 * d.nJ); w.dtg.ofs = B.take<real>(3 * d.nJ * d.nd + 1);
+        };
+        if (w.one_pass) {
+            B.off = w.A.ofs;
+            w.Jt.ofs = B.take<real>(3 * d.tmk * d.NCt);
+            scratch();
+            if (B.off < mark_b) B.off = mark_b;
+            const int jf = 3 * d.tmk * d.npad, pb = kBlendGroups * 9 * d.M + 16;
+            w.Jf.ofs = B.take<real>(jf > pb ? jf : pb);
+            w.Pb.ofs = w.Jf.ofs;
+        } else {
+            B.off = mark_b;
+            w.Jt.ofs = B.take<real>(d.jt_size);
+            w.Jf.ofs = B.take<real>(3 * d.tmk * d.npad);
+            scratch();
+            w.Pb.ofs = w.Jt.ofs;
+        }
         if (B.off < end_b) B.off = end_b;
     }
     w.Linv.ofs = S.take<real>(size_t((d.n2 + kCholNB - 1) / kCholNB) * kCholNB * kCholNB);
@@ -666,6 +686,9 @@ struct Solver {
     // table (carve() leaves them out of the staged region there)
     M2_D const real *jdir() const { return BIG ? m.jd : static_cast<const real *>(w.c_jd); }
 
+    // carve() lays out only float32 shared-memory workspaces in one pass: the compiler drops the branch everywhere else
+    M2_D bool one_pass() const { return sizeof(real) == 4 && !BIG && w.one_pass; }
+
     // ---- CTA-wide maximum of one per-thread value, broadcast (rare path: boundary repair)
     M2_D void cta_max(real *v) {
 #if M2_GPU
@@ -724,7 +747,7 @@ struct Solver {
         }
     }
 
-    // ---- pose-blend partial sums: item (joint group, slot) -> x,y,z of the slot; part[g][3 s + c] (aliases Jt).
+    // ---- pose-blend partial sums: item (joint group, slot) -> x,y,z of the slot; part[g][3 s + c] (Pb).
     //      Lanes run over consecutive slots, so every warp load is one contiguous run of 16-byte vectors.
     M2_D int blend_groups(int nl) const {      // as many joint groups as fit one round of the nl blending threads
         const int per_group = 3 * ((d.S + 3) >> 2);
@@ -766,7 +789,7 @@ struct Solver {
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
                 const int sl = 4 * sq + q;
-                if (sl < d.S) w.Jt[(g * d.S + sl) * 3 + c] = acc[q];
+                if (sl < d.S) w.Pb[(g * d.S + sl) * 3 + c] = acc[q];
             }
         }
     }
@@ -913,7 +936,7 @@ struct Solver {
                 }
             }
             for (int q = 0; q < 3; ++q)
-                for (int g = 0; g < nbg; ++g) vpo[q] += w.Jt[(g * d.S + s) * 3 + q];
+                for (int g = 0; g < nbg; ++g) vpo[q] += w.Pb[(g * d.S + s) * 3 + q];
             real v[3] = {0, 0, 0};
             real Rs[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
             for (int i = 0; i < d.kw; ++i) {
@@ -1213,36 +1236,46 @@ struct Solver {
         // its own column.
         const int lane = cta.tid & 31, warp = cta.tid >> 5, nwarp = cta.nthr >> 5;
         const int t = lane % 3, grp = lane / 3;
-        const int nmg = (tm + 9) / 10, nch = nwarp / nmg;         // marker groups, joint shares
-        const int mg = warp % nmg, ch = warp / nmg;
-        const int ml = mg * 10 + grp;
-        const bool valid = lane < 30 && ml < tm;
-        if (ch < nch) {
-            const int mi = t0 + (valid ? ml : 0), sl = 3 * mi + t;
-            const real sc = (valid && w.vis[mi]) ? wd : real(0);
-            real Mt[9], Lc[9];
-            slot_mats(sl, Mt, Lc);
-            const real *Pslot = m.pd4 + size_t(sl) * 4;
-            const int src1 = lane - t + (t + 2) % 3, src2 = lane - t + (t + 1) % 3;   // lanes whose t is t-1, t-2 (mod 3)
+        // markers [p0, p0 + pm) of the tile, at most ten per warp
+        auto part = [&](int p0, int pm) {
+            const int nmg = (pm + 9) / 10, nch = nwarp / nmg;         // marker groups, joint shares
+            const int mg = warp % nmg, ch = warp / nmg;
+            const int ml = p0 + mg * 10 + grp;
+            const bool valid = lane < 30 && ml < p0 + pm;
+            if (ch < nch) {
+                const int mi = t0 + (valid ? ml : 0), sl = 3 * mi + t;
+                const real sc = (valid && w.vis[mi]) ? wd : real(0);
+                real Mt[9], Lc[9];
+                slot_mats(sl, Mt, Lc);
+                const real *Pslot = m.pd4 + size_t(sl) * 4;
+                const int src1 = lane - t + (t + 2) % 3, src2 = lane - t + (t + 1) % 3;   // lanes whose t is t-1, t-2 (mod 3)
 #pragma unroll 1
-            for (int ji = ch; ji < njl; ji += nch) {
-                const int a = w.jlist[ji];
-                real blk[9];
-                slot_pose_block(sl, a, Mt, Lc, Pslot, blk);
-                // lane t collects column t of the marker's block: own part + the parts of the two other vertices
-                real col3[3];
+                for (int ji = ch; ji < njl; ji += nch) {
+                    const int a = w.jlist[ji];
+                    real blk[9];
+                    slot_pose_block(sl, a, Mt, Lc, Pslot, blk);
+                    // lane t collects column t of the marker's block: own part + the parts of the two other vertices
+                    real col3[3];
 #pragma unroll
-                for (int r = 0; r < 3; ++r) {
-                    const real b0 = blk[3 * r], b1 = blk[3 * r + 1], b2 = blk[3 * r + 2];
-                    // (two selects each; written as nested conditionals the compiler turned them into three divergent
-                    // branches per row -- every warp holds all three values of t)
-                    const real own = sel3(t, b0, b1, b2);
-                    const real to1 = sel3(t, b1, b2, b0);
-                    const real to2 = sel3(t, b2, b0, b1);
-                    col3[r] = own + __shfl_sync(0xffffffffu, to1, src1) + __shfl_sync(0xffffffffu, to2, src2);
+                    for (int r = 0; r < 3; ++r) {
+                        const real b0 = blk[3 * r], b1 = blk[3 * r + 1], b2 = blk[3 * r + 2];
+                        // (two selects each; written as nested conditionals the compiler turned them into three divergent
+                        // branches per row -- every warp holds all three values of t)
+                        const real own = sel3(t, b0, b1, b2);
+                        const real to1 = sel3(t, b1, b2, b0);
+                        const real to2 = sel3(t, b2, b0, b1);
+                        col3[r] = own + __shfl_sync(0xffffffffu, to1, src1) + __shfl_sync(0xffffffffu, to2, src2);
+                    }
+                    if (valid) pose_col_store(ml, a, t, sc, col3[0], col3[1], col3[2]);
                 }
-                if (valid) pose_col_store(ml, a, t, sc, col3[0], col3[1], col3[2]);
             }
+        };
+        // (a float32 tile may hold more markers than ten per warp: every marker in one tile, with fewer than 384 threads)
+        if constexpr (sizeof(real) == 4) {
+#pragma unroll 1
+            for (int p0 = 0; p0 < tm; p0 += 10 * nwarp) part(p0, tm - p0 < 10 * nwarp ? tm - p0 : 10 * nwarp);
+        } else {
+            part(0, tm);
         }
 #else
         for (int gi = 0; gi < tm * njl; ++gi) {
@@ -1381,13 +1414,37 @@ struct Solver {
     }
 #endif
 
-    // ---- T3: A += Jf^T Jf, g -= Jf^T r over the tile's rows; in linearise mode the finished rows go out first, as they are
+    // ---- acc[8 p + q] += J[r][i0 + p] J[r][j0 + q] (q < 4) or J[r][j4 + q - 4] (q >= 4) for the R rows r of J from Jr on, in
+    //      order: one 4 x 8 register tile of T3
+    template <int R>
+    M2_D void jtj_rows(const real *Jr, int i0, int j0, int j4, real (&acc)[32]) const {
+        Vec4<real> av[R], bv[R], cv[R];
+#pragma unroll
+        for (int u = 0; u < R; ++u) {
+            av[u] = ld4(Jr + u * d.npad + i0);
+            bv[u] = ld4(Jr + u * d.npad + j0);
+            cv[u] = ld4(Jr + u * d.npad + j4);
+        }
+#pragma unroll
+        for (int u = 0; u < R; ++u) {
+            const real ai[4] = {av[u].x, av[u].y, av[u].z, av[u].w};
+            const real bj8[8] = {bv[u].x, bv[u].y, bv[u].z, bv[u].w, cv[u].x, cv[u].y, cv[u].z, cv[u].w};
+#pragma unroll
+            for (int p = 0; p < 4; ++p)
+#pragma unroll
+                for (int q = 0; q < 8; ++q) acc[8 * p + q] += ai[p] * bj8[q];
+        }
+    }
+
+    // ---- T3: A += Jf^T Jf (one pass: A = Jf^T Jf), g -= Jf^T r over the tile's rows; in linearise mode the finished rows go
+    //      out first, as they are
     M2_D void tile_normal_equations(int t0, int tm, int n) {
         const int trows = 3 * tm, ld = d.lda;
         if (lin_f >= 0 && job.lin_J) {
             real *Jo = job.lin_J + (size_t(lin_f) * 3 * d.M + 3 * t0) * n;
             CTA_FOR(idx, trows * n) { const int row = idx / n, cc = idx - row * n; Jo[idx] = w.Jf[row * d.npad + cc]; }
         }
+        int jr_skip = 0;        // threads [0, jr_skip): the warps with one register tile of J^T J more than the others
 #if M2_GPU
         if constexpr (sizeof(real) == 8) {
             // float64: J^T J on the tensor cores as well -- mma.sync m8n8k4 (DMMA), a warp per 16x16 block of the upper
@@ -1417,76 +1474,75 @@ struct Solver {
                 }
                 add_upper_block16(i0, j0, n, c);
             }
-        } else if (w.tc) {
-            // float32: split TF32 on the tensor cores (tc::jtj_block_tf32), a warp per 16x16 block of the upper
-            // triangle; A += (hi hi^T + cross terms)
-            const int warp = cta.tid >> 5, nwarp = cta.nthr >> 5;
-            const int nb16 = (n + 15) >> 4, ntile = nb16 * (nb16 + 1) / 2;
-            for (int tile = warp; tile < ntile; tile += nwarp) {
-                int ti, tj;
-                upper_block(tile, nb16, ti, tj);
-                const int i0 = 16 * ti, j0 = 16 * tj;
-                float hh[2][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}}, cr[2][4] = {{0, 0, 0, 0}, {0, 0, 0, 0}};
-                tc::jtj_block_tf32(w.Jf, d.npad, trows, d.npad, i0, j0, hh, cr);
-                real c[2][2][2];
-#pragma unroll
-                for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-                    for (int ni = 0; ni < 2; ++ni)
-#pragma unroll
-                        for (int e = 0; e < 2; ++e) c[mi][ni][e] = hh[ni][2 * mi + e] + cr[ni][2 * mi + e];
-                add_upper_block16(i0, j0, n, c);
-            }
         } else
 #endif
         {
-            const int nb = (n + kBS - 1) / kBS, nblk = nb * (nb + 1) / 2;
-            CTA_FOR(b, nblk) {
-                int bi, bj;
-                upper_block(b, nb, bi, bj);
-                real acc[kBS * kBS];
+            // float32 (and the host build): J^T J on the CUDA cores in register tiles of 4 x 8 entries of the upper
+            // triangle, a thread per tile; the tiles are numbered column block by column block, so the threads of a warp
+            // read few distinct eight-column vectors and consecutive four-row vectors of a row.  Each entry sums the rows in
+            // order.
+            const int nbi = (n + 3) >> 2, nbj = (n + 7) >> 3;
+            auto col_tiles = [nbi](int bj) { return 2 * bj + 2 < nbi ? 2 * bj + 2 : nbi; };   // row blocks 0 .. 2 bj + 1
+            int ntile = 0;
+            for (int bj = 0; bj < nbj; ++bj) ntile += col_tiles(bj);
+            // With few tiles (Step 1) S lanes of a warp share one tile, each a consecutive S-th of the rows, and their sums
+            // are added by shuffles: more warps, fewer rows each
+            int S = 1;
+#if M2_GPU
+            while (S < 4 && 2 * S * ntile <= cta.nthr) S *= 2;
+#endif
+            const int per = 32 / S, nitem = S == 1 ? ntile : (ntile + per - 1) / per * 32;   // tiles per warp, threads
+            CTA_FOR(it, nitem) {
+                const int lane = it & 31, part = S == 1 ? 0 : lane / per, tile = S == 1 ? it : (it >> 5) * per + lane % per;
+                int bi = tile < ntile ? tile : 0, bj = 0;
+                while (bi >= col_tiles(bj)) { bi -= col_tiles(bj); ++bj; }
+                const int i0 = 4 * bi, j0 = 8 * bj;
+                const int j4 = j0 + 4 < d.npad ? j0 + 4 : j0;     // (columns beyond the padded row: read, not written)
+                real acc[32];
 #pragma unroll
-                for (int q = 0; q < kBS * kBS; ++q) acc[q] = 0;
-                // four rows in flight: in the float64 / oversized layout the tile lives in the global workspace (L2), and a
-                // loop that waits for every row's two loads before its sixteen FMAs ran at a fourteenth of the FP64 rate
-                // (half of the float64 kernel's time).  Same products in the same order.
-                for (int row = 0; row < trows; row += 4) {
-                    Vec4<real> av[4], bv[4];
+                for (int q = 0; q < 32; ++q) acc[q] = 0;
+                // U rows at a time (their loads first, then their products), the last ones one by one.  (Four rows in
+                // flight hold 48 registers: in the global-workspace layout the multi-model kernel then spills.)
+                constexpr int U = BIG ? 2 : 4;
+                const int r0 = part * trows / S, r1 = (part + 1) * trows / S, full = r1 - (r1 - r0) % U;
+                const real *Jr = w.Jf + r0 * d.npad;
+#pragma unroll 1
+                for (int row = r0; row < full; row += U, Jr += U * d.npad) jtj_rows<U>(Jr, i0, j0, j4, acc);
+#pragma unroll 1
+                for (int row = full; row < r1; ++row, Jr += d.npad) jtj_rows<1>(Jr, i0, j0, j4, acc);
+#if M2_GPU
+                for (int o = 16; o >= per; o >>= 1)
 #pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        const real *Jr = w.Jf + (row + u < trows ? row + u : trows - 1) * d.npad;
-                        av[u] = ld4(Jr + bi * kBS);
-                        bv[u] = ld4(Jr + bj * kBS);
-                    }
+                    for (int q = 0; q < 32; ++q) acc[q] += __shfl_xor_sync(0xffffffffu, acc[q], o);
+#endif
+                // one pass: A = the product (closed_form_terms adds the rest); else A += the tile's part.  The mirror entry
+                // receives the same value.
+                if (part == 0 && tile < ntile) {
 #pragma unroll
-                    for (int u = 0; u < 4; ++u)
-                        if (row + u < trows) {
-                            const real ai[4] = {av[u].x, av[u].y, av[u].z, av[u].w}, bjv[4] = {bv[u].x, bv[u].y, bv[u].z, bv[u].w};
+                    for (int p = 0; p < 4; ++p)
 #pragma unroll
-                            for (int p = 0; p < kBS; ++p)
-#pragma unroll
-                                for (int q = 0; q < kBS; ++q) acc[p * kBS + q] += ai[p] * bjv[q];
+                        for (int q = 0; q < 8; ++q) {
+                            const int i = i0 + p, j = j0 + q;
+                            if (i <= j && j < n) {
+                                const real v = one_pass() ? acc[8 * p + q] : w.A[i * ld + j] + acc[8 * p + q];
+                                w.A[i * ld + j] = v;
+                                if (i < j) w.A[j * ld + i] = v;
+                            }
                         }
                 }
-#pragma unroll
-                for (int p = 0; p < kBS; ++p)
-#pragma unroll
-                    for (int q = 0; q < kBS; ++q) {
-                        const int i = bi * kBS + p, j = bj * kBS + q;
-                        if (j < n && i <= j) {
-                            w.A[i * ld + j] += acc[p * kBS + q];
-                            if (i < j) w.A[j * ld + i] += acc[p * kBS + q];
-                        }
-                    }
             }
+            const int extra = nitem % cta.nthr;
+            jr_skip = (extra + 31) & ~31;
         }
-        // J^T r, a thread per column: on the tensor-core paths the first (ntile mod nwarp) warps took one 16x16 block more,
-        // so the columns start at the warp after them (the same sums in the same order, on other threads)
+        // J^T r, a thread per column, starting at the first warp with one block of J^T J fewer (the same sums in the same
+        // order, on other threads)
         int jr_tid = cta.tid;
 #if M2_GPU
-        if (sizeof(real) == 8 || w.tc) {
+        if constexpr (sizeof(real) == 8) {
             const int nb16 = (n + 15) >> 4, nwarp = cta.nthr >> 5;
             jr_tid = (cta.tid + cta.nthr - 32 * ((nb16 * (nb16 + 1) / 2) % nwarp)) % cta.nthr;
+        } else {
+            jr_tid = (cta.tid + cta.nthr - jr_skip) % cta.nthr;
         }
 #endif
 #pragma unroll 1
@@ -1596,7 +1652,7 @@ struct Solver {
         const int n = c.n;
         joint_axes();
         CTA_FOR(mi, d.M) marker_local_jacobian(mi);
-        CTA_FOR(i, n * d.lda) w.A[i] = 0;
+        if (!one_pass()) CTA_FOR(i, n * d.lda) w.A[i] = 0;     // (one pass: A lies under the build scratch; T3 writes it)
         CTA_FOR(i, n) w.g[i] = 0;
         dtg_chains();
         M2_SYNC();

@@ -119,8 +119,8 @@ mosh2::Model<real> model_dims(const mosh2_model_desc &d, std::vector<double> *hc
 }
 
 // ---- workspace layout ------------------------------------------------------------------------------------------------------------
-// The workspace of model `m` carved behind `header` bytes of shared memory (mosh2::carve), with the tensor cores in use when the
-// model qualifies and the launch has at least 128 threads.  smem / gws: the ends of the shared and the global arena, in bytes.
+// The workspace of model `m` carved behind `header` bytes of shared memory (mosh2::carve).  smem / gws: the ends of the shared
+// and the global arena, in bytes.
 template <class real, bool BIG>
 struct Layout {
     mosh2::Dims d;
@@ -129,12 +129,11 @@ struct Layout {
 };
 
 template <class real, bool BIG>
-Layout<real, BIG> layout(const mosh2::Model<real> &m, unsigned header = mosh2::kSmemHeader, int threads = 1) {
+Layout<real, BIG> layout(const mosh2::Model<real> &m, unsigned header = mosh2::kSmemHeader) {
     Layout<real, BIG> L{};
     L.d = mosh2::make_dims(m);
     mosh2::Arena S{header}, G{0};
     mosh2::carve<real, BIG>(L.w, L.d, m, S, G);
-    L.w.tc = (L.w.tc_ok && threads >= 128) ? 1 : 0;
     L.smem = S.off;
     L.gws = G.off;
     return L;
@@ -263,19 +262,27 @@ constexpr unsigned multi_smem_header() { return mosh2::kSmemHeader + ((unsigned(
 // ---- the workspace plan of a job ----------------------------------------------------------------------------------------------
 constexpr size_t kMaxSmem = 227 * 1024;      // dynamic shared memory per block on sm_90
 
-// Chooses the layout of `m`'s workspace and sets m.tile_markers (and m.dev_no_tc).  Preference order: 20-marker tiles, then
-// 10-marker tiles, while the workspace fits the shared-memory budget; then (*big = 1) the layout that moves A, its factor, the
-// Jacobian tiles and the linear-block scratch to a per-CTA global workspace of *gws bytes.  *smem > kMaxSmem: the model does
-// not fit at all.  `header`: bytes in front of the workspace (a multi-model job keeps the chunk's Model record there).
+// Chooses the layout of `m`'s workspace and sets m.tile_markers.  Preference order, while the workspace fits the shared-memory
+// budget: in float32 every marker in one tile (one pass: the Jacobian is built once and A written once per linearisation),
+// then the fewest tiles of more than 20 markers; 20-marker tiles, then 10-marker tiles; then (*big = 1) the layout that moves
+// A, its factor, the Jacobian tiles and the linear-block scratch to a per-CTA global workspace of *gws bytes.  *smem >
+// kMaxSmem: the model does not fit at all.  `header`: bytes in front of the workspace (a multi-model job keeps the chunk's
+// Model record there).
 template <class real>
 void plan_workspace(mosh2::Model<real> &m, size_t *smem, size_t *gws, int *big, unsigned header = mosh2::kSmemHeader) {
-    const int tries[3][2] = {{20, 0}, {10, 0}, {10, 1}};   // markers per tile (a warp owns ten), big
-    const char *dev_tile = getenv("MOSH2_DEV_TILE");      // development aid: 10 = skip the 20-marker tile
+    std::vector<std::pair<int, int>> tries;                  // markers per tile, big
+    const char *dev_tile = getenv("MOSH2_DEV_TILE");      // development aid: 10 = only the 10-marker tile in shared memory
     const bool dev_big = getenv("MOSH2_DEV_BIG") != nullptr;   // development aid: force the global-workspace layout
-    for (int pass = dev_big ? 2 : ((dev_tile && atoi(dev_tile) == 10) ? 1 : 0); pass < 3; ++pass) {
-        m.tile_markers = tries[pass][0];
-        m.dev_no_tc = getenv("MOSH2_DEV_NO_TC") ? 1 : 0;      // development aid: J^T J on the CUDA cores
-        *big = tries[pass][1];
+    if (!dev_big && !(dev_tile && atoi(dev_tile) == 10)) {
+        if (sizeof(real) == 4)
+            for (int k = 1; (m.M + k - 1) / k > 20; ++k) tries.push_back({(m.M + k - 1) / k, 0});
+        tries.push_back({20, 0});
+    }
+    if (!dev_big) tries.push_back({10, 0});
+    tries.push_back({10, 1});
+    for (const auto &t : tries) {
+        m.tile_markers = t.first;
+        *big = t.second;
         size_t s, g;
         if (*big) { const Layout<real, true> L = layout<real, true>(m, header); s = L.smem; g = L.gws; }
         else { const Layout<real, false> L = layout<real, false>(m, header); s = L.smem; g = L.gws; }

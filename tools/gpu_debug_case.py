@@ -29,8 +29,8 @@ v8 = np.ascontiguousarray(vis, dtype=np.uint8)
 handle.mosh2_emu_solve(C.byref(h.desc), C.byref(opts), F, o64.ctypes.data_as(lib._f64p), v8.ctypes.data_as(lib._u8p), 0, 0,
                        lib.MOSH2_F64, C.byref(emu.c))
 print('emu f64 builds', emu.counters[:, 2].tolist())
-for envs in ({}, {'MOSH2_DEV_TILE': '10'}, {'MOSH2_DEV_NO_TC': '1'}):
-    for k in ('MOSH2_DEV_TILE', 'MOSH2_DEV_NO_TC'):
+for envs in ({}, {'MOSH2_DEV_TILE': '10'}, {'MOSH2_DEV_BIG': '1'}):
+    for k in ('MOSH2_DEV_TILE', 'MOSH2_DEV_BIG'):
         os.environ.pop(k, None)
     os.environ.update(envs)
     for prec in ('f64', 'f32'):
