@@ -26,6 +26,11 @@ every picked frame's model carries the given shape plus its own expressions ``be
 zero expressions.  The device's linear block then holds the expression directions instead of the shape's, and in the two
 detailed steps the jaw and the expressions are private unknowns of each frame, with the poseF / expr terms.  The expressions
 are returned in the debug details as ``opt_models_expression``.
+
+``face_with_free_shape`` (SMPL-X with face markers, ``optimize_betas`` and ``optimize_face``; the reference raises here): the
+union of the two objectives.  Each frame's model carries the free shape plus its own expressions, the canonical body the shape
+with zero expressions; the linear block holds the shape directions followed by the expression directions.  The shape columns
+stay shared (attachment, init, surface and beta terms as with a free shape), the expressions private to their frame.
 """
 from __future__ import annotations
 
@@ -276,11 +281,12 @@ class DeviceBackend:
 # ---------------------------------------------------------------------------------------------------------------------
 # the solver
 # ---------------------------------------------------------------------------------------------------------------------
-def face_flag(cfg, marker_meta, avail_labels) -> bool:
+def face_flag(cfg, marker_meta, avail_labels, face_with_free_shape: bool = False) -> bool:
     """Whether Stage I fits the jaw and the expressions (``moshpp.optimize_face``), by the reference's rules, without changing
     ``cfg``: off with a free shape when the face markers are excluded (chmosh.py:103-118), off without a face-type marker in the
     layout or without a face label in the picked frames (chmosh.py:127-137), ignored for models other than SMPL-X (only SMPL-X has
-    a jaw and expression components), and NotImplementedError with a free shape on SMPL-X (chmosh.py:287-291)."""
+    a jaw and expression components), and NotImplementedError with a free shape on SMPL-X (chmosh.py:287-291) unless
+    ``face_with_free_shape`` asks for the joint fit of the shape and every picked frame's expressions."""
     sm, mp = cfg.surface_model, cfg.moshpp
     if not bool(_get(mp, 'optimize_face', False)):
         return False
@@ -293,14 +299,16 @@ def face_flag(cfg, marker_meta, avail_labels) -> bool:
         return False
     if sm.type != 'smplx':
         return False
-    if free_betas:
-        raise NotImplementedError('optimize_face with optimize_betas: Stage I fits per-frame expressions only for a given shape '
-                                  '(betas_fname or v_template_fname) with optimize_betas off (chmosh.py:287-291)')
+    if free_betas and not face_with_free_shape:
+        raise NotImplementedError('optimize_face with optimize_betas: Stage I fits per-frame expressions with a free shape only '
+                                  'when asked to (face_with_free_shape=True); otherwise give the shape (betas_fname or '
+                                  'v_template_fname) with optimize_betas off (chmosh.py:287-291)')
     return True
 
 
 class StageI:
-    def __init__(self, stagei_frames, cfg, marker_meta, betas=None, v_template=None, backend=None):
+    def __init__(self, stagei_frames, cfg, marker_meta, betas=None, v_template=None, backend=None, *,
+                 face_with_free_shape: bool = False):
         sm, mp = cfg.surface_model, cfg.moshpp
         self.cfg, self.marker_meta = cfg, marker_meta
         self.backend = backend or DeviceBackend()
@@ -315,7 +323,7 @@ class StageI:
             elif not np.any([('finger' in t) and l in avail for l, t in marker_meta['marker_type'].items()]):
                 self.fingers = False
         self.free_betas = bool(mp.optimize_betas)
-        self.face = face_flag(cfg, marker_meta, avail)
+        self.face = face_flag(cfg, marker_meta, avail, face_with_free_shape)
         if _get(mp, 'head_marker_corr_fname', None) is not None:
             raise NotImplementedError('moshpp.head_marker_corr_fname (chmosh.py:250-264,364-372) is outside this build')
         self.model = model = _pack.load_surface_model(sm.fname, pose_hand_prior_fname=_get(mp, 'pose_hand_prior_fname'),
@@ -364,18 +372,21 @@ class StageI:
     def pack_for(self, detailed: bool, can_v=None):
         sm, mp = self.cfg.surface_model, self.cfg.moshpp
         toes = bool(_get(mp, 'optimize_toes', False))
-        if self.face:
+        if self.face and not self.free_betas:
             # the shape is given: the linear block is the expression directions alone, and Step 2 frees the jaw and them
             return _pack.build_pack(self.model, self.betas, self.ml, num_betas=self.nb, prior=self.prior,
                                     optimize_fingers=self.fingers, optimize_toes=toes, optimize_face=True,
                                     expr_start=self.es, num_expressions=self.ne, can_verts=can_v)
+        # the linear block is the shape directions, followed by the expression directions when the face is fitted with the
+        # shape (face_with_free_shape); the free lists keep a frame's own unknowns first and the shared shape columns last
         pk = _pack.build_pack(self.model, self.betas, self.ml, num_betas=self.nb, prior=self.prior,
                               dmpl_dirs=self.model.shapedirs[:, :, :self.nb], num_dmpls=self.nb,
-                              optimize_fingers=self.fingers, optimize_toes=toes,
-                              can_verts=can_v, jd_lin=self.jd_lin)
-        lin = [3 + pk.p_red + i for i in range(self.nb)] if self.free_betas else []
-        s1 = [int(i) for i in pk.free_step1 if i < 3 + pk.p_red]
-        s2 = [int(i) for i in pk.free_step2 if i < 3 + pk.p_red]
+                              optimize_fingers=self.fingers, optimize_toes=toes, optimize_face=self.face,
+                              expr_start=self.es, num_expressions=self.ne, can_verts=can_v, jd_lin=self.jd_lin)
+        lo = 3 + pk.p_red
+        lin = [lo + i for i in range(self.nb)] if self.free_betas else []
+        s1 = [int(i) for i in pk.free_step1 if i < lo]
+        s2 = [int(i) for i in pk.free_step2 if i < lo or i >= lo + self.nb]       # trans | pose ids | expressions
         pk.free_step1 = np.asarray(s1 + lin, dtype=np.int32)
         pk.free_step2 = np.asarray(s2 + lin, dtype=np.int32)
         return pk
@@ -407,8 +418,8 @@ class StageI:
         n_p = n_f - nb
         x = np.zeros((F, pk.nx))
         x[:, :3], x[:, 3:3 + pk.p_red] = self.trans, self.pose
-        if self.face:
-            x[:, 3 + pk.p_red:] = self.expr
+        if self.face:           # (the shape slots of the linear block stay zero: the pack's rest vertices carry the shape)
+            x[:, 3 + pk.p_red + pk.n_dmpl - pk.n_expr:] = self.expr
         opts = _lib.make_options(None, optimize_fingers=detailed and self.fingers and pk.finger_hi > pk.finger_lo,
                                  optimize_face=detailed and self.face)
         opts.wt_data, opts.wt_poseB, opts.wt_poseH = float(wts['data']), float(wts['poseB']), float(wts['poseH'])
@@ -632,9 +643,13 @@ class StageI:
 
 
 def mosh_stagei(stagei_frames: List[Dict[str, np.ndarray]], cfg, betas_fname=None, v_template_fname=None, *, marker_meta=None,
-                device: int = 0, backend=None) -> dict:
+                device: int = 0, backend=None, face_with_free_shape: bool = False) -> dict:
     """Stage I of MoSh++ on one H100.  Positional arguments as in the reference (chmosh.py:83-85).  The marker layout is read
-    from ``cfg.dirs.marker_layout.fname`` like the reference does (chmosh.py:120-125), or handed over loaded as ``marker_meta``."""
+    from ``cfg.dirs.marker_layout.fname`` like the reference does (chmosh.py:120-125), or handed over loaded as ``marker_meta``.
+
+    ``face_with_free_shape``: with ``optimize_betas`` and ``optimize_face`` on SMPL-X, fit the shape and the jaw and expressions
+    of every picked frame together instead of raising NotImplementedError (the reference's answer; its log suggests running
+    Stage I twice, for the shape without the face markers and then for the face with that shape).  Off by default."""
     if marker_meta is None:                                                                      # chmosh.py:120-125
         mc = cfg.mocap
         marker_meta = load_marker_layout(cfg.dirs.marker_layout.fname, exclude_markers=_get(mc, 'exclude_markers'),
@@ -647,7 +662,8 @@ def mosh_stagei(stagei_frames: List[Dict[str, np.ndarray]], cfg, betas_fname=Non
         assert str(betas_fname).endswith('.npz'), ValueError(f'invalid numpy betas_fname: {betas_fname}')
         betas = np.load(betas_fname)['betas']
     v_template = _read_vertices(v_template_fname) if v_template_fname else None
-    s = StageI(stagei_frames, cfg, marker_meta, betas=betas, v_template=v_template, backend=backend or DeviceBackend(device))
+    s = StageI(stagei_frames, cfg, marker_meta, betas=betas, v_template=v_template, backend=backend or DeviceBackend(device),
+               face_with_free_shape=face_with_free_shape)
     sse, dev = s.run()
     can_v = s.can(s.betas[:s.nb])
     d2 = ((s.ml[:, None, :] - can_v[None]) ** 2).sum(-1)                                        # chmosh.py:422-424: nearest vertex
