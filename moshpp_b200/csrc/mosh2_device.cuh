@@ -2029,55 +2029,75 @@ struct Solver {
 #if M2_GPU
         // Four warps (named barrier 2): every warp forms y_k = Linv_k^T z_k itself, the 128 threads share the rows i < k0 of
         // the update z_i -= L[k, i] y_k -- one round per block instead of four by a single warp (560 -> cycles per block
-        // are the dependent shared-memory round trips, not the arithmetic).
+        // are the dependent shared-memory round trips, not the arithmetic).  A round takes two blocks, k1 and the one below
+        // it, k0 = k1 - NB: every thread also applies y_k1 to z_k0 itself, then forms y_k0, so half as many rounds (and
+        // barriers) stand between the factorisation and dgn.  Every z_i receives the same updates in the same order as with
+        // one block per round: the result is the same bit for bit.
         if (cta.tid < 128) {
             const int tid = cta.tid;
             for (int i = tid; i < n; i += 128) w.tmp[i] = w.Lm[n * ld + i];     // z = L^-1 (ds*g), see above
             asm volatile("bar.sync 2, 128;" ::: "memory");
+            // y = Linv_k^T z for the block at k (every thread, redundantly)
+            auto block_y = [&](int k, const real (&zv)[NB], real (&y)[NB]) {
+                const real *Li = w.Linv + (k / NB) * NB * NB;
+#pragma unroll
+                for (int cc = 0; cc < NB; ++cc) {
+                    real sacc = 0;
+#pragma unroll
+                    for (int pp = cc; pp < NB; ++pp) sacc += Li[pp * NB + cc] * zv[pp];
+                    y[cc] = sacc;
+                }
+            };
+            // thread 0, after the round's barrier: y_k replaces z_k
+            auto store_y = [&](int k, int kb, const real (&y)[NB]) {
+                if (kb == NB) {
+                    Vec4<real> o0, o1;
+                    o0.x = y[0]; o0.y = y[1]; o0.z = y[2]; o0.w = y[3]; o1.x = y[4]; o1.y = y[5]; o1.z = y[6]; o1.w = y[7];
+                    *reinterpret_cast<Vec4<real> *>(w.tmp + k) = o0;
+                    *reinterpret_cast<Vec4<real> *>(w.tmp + k + 4) = o1;
+                } else {
+#pragma unroll
+                    for (int cc = 0; cc < NB; ++cc) if (cc < kb) w.tmp[k + cc] = y[cc];
+                }
+            };
 #pragma unroll 1
-            for (int k0 = ((n - 1) / NB) * NB; k0 >= 0; k0 -= NB) {
-                const int kb = (n - k0 < NB) ? n - k0 : NB;
-                const real *Li = w.Linv + (k0 / NB) * NB * NB;
-                real zv[NB], y[NB], Lr[NB][NB];
+            for (int k1 = ((n - 1) / NB) * NB; k1 >= 0; k1 -= 2 * NB) {
+                const int kb = (n - k1 < NB) ? n - k1 : NB;   // (only the top block can be short)
+                const int k0 = k1 - NB;                        // < 0: k1 is the first block and has no partner
+                real zv[NB], y1[NB], y0[NB];
                 {
-                    const Vec4<real> z0 = ld4(w.tmp + k0), z1 = ld4(w.tmp + k0 + 4);
+                    const Vec4<real> z0 = ld4(w.tmp + k1), z1 = ld4(w.tmp + k1 + 4);
                     zv[0] = z0.x; zv[1] = z0.y; zv[2] = z0.z; zv[3] = z0.w; zv[4] = z1.x; zv[5] = z1.y; zv[6] = z1.z; zv[7] = z1.w;
                 }
 #pragma unroll
                 for (int cc = 1; cc < NB; ++cc) if (cc >= kb) zv[cc] = real(0);
-#pragma unroll
-                for (int pp = 0; pp < NB; ++pp) {
-                    const Vec4<real> l0 = ld4(Li + pp * NB);
-                    Lr[pp][0] = l0.x; Lr[pp][1] = l0.y; Lr[pp][2] = l0.z; Lr[pp][3] = l0.w;
-                    if (pp >= 4) {
-                        const Vec4<real> l1 = ld4(Li + pp * NB + 4);
-                        Lr[pp][4] = l1.x; Lr[pp][5] = l1.y; Lr[pp][6] = l1.z; Lr[pp][7] = l1.w;
+                block_y(k1, zv, y1);
+                if (k0 >= 0) {
+                    {
+                        const Vec4<real> z0 = ld4(w.tmp + k0), z1 = ld4(w.tmp + k0 + 4);
+                        zv[0] = z0.x; zv[1] = z0.y; zv[2] = z0.z; zv[3] = z0.w; zv[4] = z1.x; zv[5] = z1.y; zv[6] = z1.z; zv[7] = z1.w;
                     }
-                }
 #pragma unroll
-                for (int cc = 0; cc < NB; ++cc) {          // y = Linv^T z (every thread, redundantly)
-                    real sacc = 0;
+                    for (int r = 0; r < NB; ++r) {
+                        real zi = zv[r];
 #pragma unroll
-                    for (int pp = cc; pp < NB; ++pp) sacc += Lr[pp][cc] * zv[pp];
-                    y[cc] = sacc;
-                }
-                for (int i = tid; i < k0; i += 128) {
-                    real zi = w.tmp[i];
+                        for (int cc = 0; cc < NB; ++cc) if (cc < kb) zi -= w.Lm[(k1 + cc) * ld + k0 + r] * y1[cc];
+                        zv[r] = zi;
+                    }
+                    block_y(k0, zv, y0);
+                    for (int i = tid; i < k0; i += 128) {
+                        real zi = w.tmp[i];
 #pragma unroll
-                    for (int cc = 0; cc < NB; ++cc) if (cc < kb) zi -= w.Lm[(k0 + cc) * ld + i] * y[cc];
-                    w.tmp[i] = zi;
+                        for (int cc = 0; cc < NB; ++cc) if (cc < kb) zi -= w.Lm[(k1 + cc) * ld + i] * y1[cc];
+#pragma unroll
+                        for (int cc = 0; cc < NB; ++cc) zi -= w.Lm[(k0 + cc) * ld + i] * y0[cc];
+                        w.tmp[i] = zi;
+                    }
                 }
                 asm volatile("bar.sync 2, 128;" ::: "memory");   // (every thread has read z_k before thread 0 replaces it by y_k)
                 if (tid == 0) {
-                    if (kb == NB) {
-                        Vec4<real> o0, o1;
-                        o0.x = y[0]; o0.y = y[1]; o0.z = y[2]; o0.w = y[3]; o1.x = y[4]; o1.y = y[5]; o1.z = y[6]; o1.w = y[7];
-                        *reinterpret_cast<Vec4<real> *>(w.tmp + k0) = o0;
-                        *reinterpret_cast<Vec4<real> *>(w.tmp + k0 + 4) = o1;
-                    } else {
-#pragma unroll
-                        for (int cc = 0; cc < NB; ++cc) if (cc < kb) w.tmp[k0 + cc] = y[cc];
-                    }
+                    store_y(k1, kb, y1);
+                    if (k0 >= 0) store_y(k0, NB, y0);
                 }
             }
             asm volatile("bar.sync 2, 128;" ::: "memory");
