@@ -230,6 +230,8 @@ def prepare_stageii(cfg, markers_latent, latent_labels, betas, marker_meta, v_te
     prior_fname = _get(mp, 'pose_body_prior_fname')
     if prior_fname and model.model_type == 'animal_horse':
         prior = _pack.create_horse_body_prior(prior_fname)                                         # bodymodel_loader.py:121-125
+    elif prior_fname and model.model_type == 'animal_dog':
+        prior = _pack.create_dog_body_prior(prior_fname)                                           # bodymodel_loader.py:126-131
     elif prior_fname and model.model_type != 'mano':
         prior = _pack.create_gmm_body_prior(prior_fname, exclude_hands=model.model_type in ('smplh', 'smplx'))
     dyn = bool(_get(mp, 'optimize_dynamics', False))
@@ -739,7 +741,8 @@ def mosh_stageii_batch(mocap_fnames, cfg, markers_latent: np.ndarray, latent_lab
 def kernel_shape_key(pk) -> tuple:
     """What two packs must share to be solved by one multi-model launch (mosh2_job_create_multi): sizes, free-variable
     counts, finger / face / joint-angle ranges, prior size and the hand-block structure of the hand-PCA matrix (the non-zero
-    column range of every row).  The tables themselves may differ."""
+    column range of every row).  The tables themselves may differ, the prior's pose ids (``prior_ids``) among them: every
+    thread block stages the tables of its own chunk's model."""
     hc = np.asarray(pk.hand_comps).reshape(pk.n_hand_red, pk.n_hand_full) if pk.n_hand_red else np.zeros((0, 0))
     rows = []
     for r in hc:

@@ -9,7 +9,7 @@ Jacobians, priors, dog-leg) lives only in ``csrc/`` -- there is no CPU solver in
 Reference behaviour restated here (file:line under /root/reference/src/moshpp):
   * model parametrisation / hand PCA ........ models/smpl_fast_derivatives.py:52-166,194-204
   * marker attachment (TransformedCoeffs) .... transformed_lm.py:45-113
-  * GMM body prior constants ................. prior/gmm_prior_ch.py:107-134
+  * GMM body prior constants ................. prior/gmm_prior_ch.py:107-134, prior/dog_body_prior.py:53-87
   * pose-id partitions, toes, fingers ........ chmosh.py:548-571,645-647,676-692
 """
 from __future__ import annotations
@@ -288,6 +288,43 @@ def create_horse_body_prior(pose_body_prior_fname: str) -> BodyPrior:
     return BodyPrior(means=np.ascontiguousarray(mu[None]), Q=np.ascontiguousarray((P @ P.T)[None]), neglogw=np.zeros(1))
 
 
+# SMAL dog (prior/dog_body_prior.py:56-58, chmosh.py:574-579): the joints its pose prior and Stage II see -- not 0 (the
+# root, optimised on its own), 2, 6 and 29; their pose ids in this order (93 of the 105)
+DOG_BODY_JOINTS = (1, 3, 4, 5, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22, 23, 24, 25, 26, 27, 28,
+                   30, 31, 32, 33, 34)
+DOG_BODY_IDS = np.array([3 * j + c for j in DOG_BODY_JOINTS for c in range(3)], dtype=np.int32)
+
+
+def create_dog_body_prior(pose_body_prior_fname: str) -> BodyPrior:
+    """MaxMixtureDog.get_gmm_prior (prior/dog_body_prior.py:53-87): the mixture of 'gmm_covs' / 'gmm_means' / 'gmm_weights'
+    restricted to DOG_BODY_IDS, with MaxMixtureComplete's residual as for SMPL (gmm_prior_ch.py:42-104).
+
+    The weight constant -log(w_k / ((2 pi)^(D/2) sqrt(det S_k) / min_j sqrt(det S_j))) is computed in the log domain:
+    -log w_k + (D/2) log 2 pi + (logdet S_k - min_j logdet S_j) / 2.  That is the reference's value whenever the determinants
+    are representable; at D = 93 a covariance with per-axis variances near 1e-4 has det = 0 in float64, where the direct form
+    gives 0 / 0.  A covariance that is not positive definite raises ValueError (the reference asserts the opposite of what its
+    message says, dog_body_prior.py:78-79, and so refuses every valid prior)."""
+    gmm = load_reference_pickle(pose_body_prior_fname)
+    ids = DOG_BODY_IDS
+    covars = np.asarray(gmm['gmm_covs'], dtype=np.float64)[:, :, ids][:, ids]
+    means = np.asarray(gmm['gmm_means'], dtype=np.float64)[:, ids]
+    weights = np.asarray(gmm['gmm_weights'], dtype=np.float64).ravel()
+    D = len(ids)
+    logdets = np.zeros(len(covars))
+    for k, c in enumerate(covars):
+        try:
+            np.linalg.cholesky(c)
+        except np.linalg.LinAlgError:
+            raise ValueError(f'dog pose prior {pose_body_prior_fname}: the covariance of component {k} is not positive '
+                             f'definite') from None
+        logdets[k] = np.linalg.slogdet(c)[1]
+    precs = np.stack([np.linalg.inv(c) for c in covars])
+    neglogw = -np.log(weights) + 0.5 * D * np.log(2 * np.pi) + 0.5 * (logdets - logdets.min())
+    Q = 0.5 * precs
+    Q = 0.5 * (Q + np.transpose(Q, (0, 2, 1)))
+    return BodyPrior(means=np.ascontiguousarray(means), Q=np.ascontiguousarray(Q), neglogw=np.ascontiguousarray(neglogw))
+
+
 def create_gmm_body_prior(pose_body_prior_fname: str, exclude_hands: bool = False) -> BodyPrior:
     gmm = load_reference_pickle(pose_body_prior_fname)
     npose = 63 if exclude_hands else 69
@@ -425,10 +462,14 @@ def pose_partitions(model_type: str, p_red: int, optimize_fingers: bool, optimiz
         finger = all_ids[3:]
     elif model_type == 'animal_horse':
         body = all_ids[3:84]                                 # tail, mouth and ears stay at rest (chmosh.py:572-573)
+    elif model_type == 'animal_dog':
+        if p_red < 3 * (DOG_BODY_JOINTS[-1] + 1):
+            raise ValueError(f'animal_dog: the pose prior covers joints up to {DOG_BODY_JOINTS[-1]}; this model has '
+                             f'{p_red // 3} joints')
+        body = [all_ids[i] for i in DOG_BODY_IDS]            # joints 2, 6 and 29 stay at rest (chmosh.py:574-579)
     else:
-        # animal_dog and object are listed by the reference but cannot run its Stage II: MaxMixtureDog asserts that a
-        # covariance determinant IS zero (prior/dog_body_prior.py:73-74) and RigidObjectModel has no `fullpose`
-        # (chmosh.py:719); they are not built here
+        # object is listed by the reference but cannot run its Stage II: RigidObjectModel has no `fullpose`
+        # (chmosh.py:719); it is not built here
         raise NotImplementedError(f'surface model type {model_type!r} is outside the Stage-II hot path of this build')
     step1 = root + body
     if len(body) and not optimize_toes:
@@ -528,6 +569,8 @@ def build_pack(model: SurfaceModel, betas: np.ndarray, markers_latent: np.ndarra
         pack.prior_k = prior.means.shape[0]
         pack.prior_d = d
         pack.prior_off = parts['body'][0]
+        if parts['body'] != list(range(pack.prior_off, pack.prior_off + d)):     # (the dog: joints with gaps)
+            pack.prior_ids = np.asarray(parts['body'], dtype=np.int32)
         pack.prior_means = prior.means
         pack.prior_Q = prior.Q
         pack.prior_neglogw = prior.neglogw

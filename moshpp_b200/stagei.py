@@ -336,6 +336,8 @@ class StageI:
         pf = _get(mp, 'pose_body_prior_fname')
         if pf and model.model_type == 'animal_horse':
             self.prior = _pack.create_horse_body_prior(pf)
+        elif pf and model.model_type == 'animal_dog':
+            self.prior = _pack.create_dog_body_prior(pf)
         elif pf and model.model_type != 'mano':
             self.prior = _pack.create_gmm_body_prior(pf, exclude_hands=model.model_type in ('smplh', 'smplx'))
         self.nb = int(sm.num_betas)

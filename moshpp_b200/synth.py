@@ -103,12 +103,13 @@ def skeleton(model_type: str):
         par = [-1] + [0 if p < 0 else 1 + p for p in hpar]
         rad = [0.03] + [0.009] * 15
         return pos, np.array(par), np.array(rad)
-    if model_type == 'animal_horse':
+    if model_type in ('animal_horse', 'animal_dog'):
         return _HORSE35, np.array(_HORSE35_PARENTS), np.array(_HORSE35_RADII)
     raise ValueError(model_type)
 
 
-# a quadruped with 35 joints: 28 body joints (pose ids 0..83 are optimised), then tail (3), mouth, ears (2), forelock
+# a quadruped with 35 joints: 28 body joints (pose ids 0..83 are optimised for the horse), then tail (3), mouth, ears (2),
+# forelock; the dog model uses the same tree (its prior and Stage II see every joint but 0, 2, 6 and 29)
 _HORSE35 = np.array([
     [-0.50, 1.10, 0.0], [-0.25, 1.15, 0.0], [0.00, 1.15, 0.0], [0.25, 1.15, 0.0], [0.50, 1.15, 0.0],
     [0.70, 1.35, 0.0], [0.85, 1.55, 0.0], [1.00, 1.65, 0.0],
@@ -125,7 +126,7 @@ _HORSE35_RADII = [0.20, 0.20, 0.21, 0.20, 0.18, 0.11, 0.09, 0.08, 0.07, 0.06, 0.
                   0.08, 0.065, 0.045, 0.04, 0.08, 0.065, 0.045, 0.04, 0.12, 0.12, 0.10, 0.10, 0.04, 0.03, 0.025, 0.04,
                   0.02, 0.02, 0.03]
 
-NUM_VERTS = {'smpl': 6890, 'smplh': 6890, 'smplx': 10475, 'mano': 778, 'animal_horse': 3889}
+NUM_VERTS = {'smpl': 6890, 'smplh': 6890, 'smplx': 10475, 'mano': 778, 'animal_horse': 3889, 'animal_dog': 3889}
 
 
 def _bone_segments(pos, par, rad):
@@ -206,7 +207,7 @@ def make_body_model(model_type: str, n_verts: Optional[int] = None, n_betas: int
         segs_body = [s for s in segs if s[0] not in (23, 24)]
     else:
         segs_body = segs
-    torso = {'mano': (), 'animal_horse': (0, 1, 2, 3, 4)}.get(model_type, (0, 3, 6, 9))
+    torso = {'mano': (), 'animal_horse': (0, 1, 2, 3, 4), 'animal_dog': (0, 1, 2, 3, 4)}.get(model_type, (0, 3, 6, 9))
     verts = _sample_capsules(segs_body, V - n_eye, rng, torso_joints=torso)
     verts = verts[rng.permutation(len(verts))]
     if n_eye:
@@ -322,6 +323,25 @@ def make_horse_prior(seed: int = SEED_MODEL + 4, dim: int = 105) -> Dict[str, np
     q, _ = np.linalg.qr(rng.standard_normal((dim, dim)))
     lam = np.exp(rng.uniform(np.log(1.0 / 0.6), np.log(1.0 / 0.08), dim))
     return {'pic': (q * lam) @ q.T, 'mean_pose': 0.1 * rng.standard_normal(dim)}
+
+
+def make_dog_prior(seed: int = SEED_MODEL + 5, n_comp: int = 8, dim: int = 105) -> Dict[str, np.ndarray]:
+    """The dog pose prior's file layout (prior/dog_body_prior.py:63-71): 'gmm_covs' K x 105 x 105, 'gmm_means' K x 105 and
+    'gmm_weights' K over the whole pose without the root.  Components with means near zero share one spectrum in other
+    orientations, each scaled by its own factor within 3 % of one; over 93 dimensions that spreads the determinants, and the
+    weights that balance them, over two orders of magnitude.  The normalised constants -log w' then lie within 0.5 of each
+    other, and the component a pose is held to changes along the synthetic motions (within the first ten frames of CD)."""
+    rng = np.random.default_rng(seed)
+    means = 0.01 * rng.standard_normal((n_comp, dim))
+    lam = np.exp(rng.uniform(np.log(0.2 ** 2), np.log(0.6 ** 2), dim))
+    covs = np.zeros((n_comp, dim, dim))
+    scale = np.zeros(n_comp)
+    for k in range(n_comp):
+        q, _ = np.linalg.qr(rng.standard_normal((dim, dim)))
+        scale[k] = np.exp(rng.uniform(np.log(0.97), np.log(1.03)))
+        covs[k] = (q * (scale[k] ** 2 * lam)) @ q.T
+    weights = np.exp(rng.uniform(np.log(0.7), np.log(1.0), n_comp)) * scale ** 93
+    return {'gmm_covs': covs, 'gmm_means': means, 'gmm_weights': weights / weights.sum()}
 
 
 def make_dmpl(verts: np.ndarray, seed: int = SEED_MODEL + 3, n_dmpl: int = 8) -> Dict[str, np.ndarray]:
@@ -495,11 +515,14 @@ def make_motion(p: _pack.StageIIPack, n_frames: int, seed: int, fps: float = 120
         f = rng.uniform(0.2, 2.0, 3)
         ph = rng.uniform(0, 2 * np.pi, 3)
         pose[:, i] = (a[None] * np.sin(2 * np.pi * f[None] * t[:, None] + ph[None])).sum(1) + rng.normal(0, 0.05 * amp)
-    if p.model_type in ('smpl', 'smplh', 'smplx', 'animal_horse'):
+    if p.model_type in ('smpl', 'smplh', 'smplx', 'animal_horse', 'animal_dog'):
         pose[:, 30:36] *= 0.0            # toes are frozen in Stage II unless optimize_toes
     if p.model_type == 'animal_horse':
         pose[:, 84:] = 0.0               # tail, mouth and ears are never optimised (chmosh.py:572-573)
         pose[:, 3:84] *= 0.6
+    if p.model_type == 'animal_dog':
+        pose[:, np.setdiff1d(np.arange(3, P), _pack.DOG_BODY_IDS)] = 0.0    # joints 2, 6, 29: never optimised (chmosh.py:574-579)
+        pose[:, 3:] *= 0.6
     if p.model_type == 'smplx':
         if p.face_hi > p.face_lo:
             pose[:, 69:75] = 0.0         # eyes are never optimised; the jaw is, with optimize_face
@@ -591,6 +614,8 @@ CONFIGS = {
     # (new configurations go last: the motion seed depends on the position)
     # the one animal variant whose Stage II runs in the reference
     'CH': dict(model_type='animal_horse', frames=60, n_body=36, n_finger=0, optimize_fingers=False, optimize_dynamics=False, mocap_ext='npz'),
+    # the SMAL dog: an 8-component max-mixture pose prior over 93 pose ids with gaps (prior/dog_body_prior.py:53-87)
+    'CD': dict(model_type='animal_dog', frames=60, n_body=36, n_finger=0, optimize_fingers=False, optimize_dynamics=False, mocap_ext='npz'),
 }
 
 
@@ -637,6 +662,11 @@ def make_case(out_dir: str, config: str = 'C2', *, frames: Optional[int] = None,
         if not os.path.exists(body_prior_fname):
             with open(body_prior_fname, 'wb') as f:
                 pickle.dump(make_horse_prior(), f, protocol=pickle.HIGHEST_PROTOCOL)
+    elif mt == 'animal_dog':
+        body_prior_fname = os.path.join(out_dir, 'pose_body_prior_dog.pkl')
+        if not os.path.exists(body_prior_fname):
+            with open(body_prior_fname, 'wb') as f:
+                pickle.dump(make_dog_prior(), f, protocol=pickle.HIGHEST_PROTOCOL)
     elif not os.path.exists(body_prior_fname):
         with open(body_prior_fname, 'wb') as f:
             pickle.dump(make_body_prior(), f, protocol=pickle.HIGHEST_PROTOCOL)
@@ -668,6 +698,8 @@ def make_case(out_dir: str, config: str = 'C2', *, frames: Optional[int] = None,
     prior = None
     if mt == 'animal_horse':
         prior = _pack.create_horse_body_prior(body_prior_fname)
+    elif mt == 'animal_dog':
+        prior = _pack.create_dog_body_prior(body_prior_fname)
     elif mt != 'mano':
         prior = _pack.create_gmm_body_prior(body_prior_fname, exclude_hands=mt in ('smplh', 'smplx'))
     dm_dirs = None
