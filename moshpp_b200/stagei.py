@@ -31,6 +31,11 @@ are returned in the debug details as ``opt_models_expression``.
 union of the two objectives.  Each frame's model carries the free shape plus its own expressions, the canonical body the shape
 with zero expressions; the linear block holds the shape directions followed by the expression directions.  The shape columns
 stay shared (attachment, init, surface and beta terms as with a free shape), the expressions private to their frame.
+
+``reference_options`` (off by default: either option raises): the head-marker correlation prior replaces the init terms of
+the correlated markers by ``corr (ml - init)[head_ids]``, dense over their latent unknowns in the shared block; the extra
+initial rigid adjustment is one dog-leg over every frame's root orientation and translation on the unweighted data term, its
+normal equations 6 x 6 blocks from the same device linearisation with no shared block (DESIGN.md section 10).
 """
 from __future__ import annotations
 
@@ -308,7 +313,7 @@ def face_flag(cfg, marker_meta, avail_labels, face_with_free_shape: bool = False
 
 class StageI:
     def __init__(self, stagei_frames, cfg, marker_meta, betas=None, v_template=None, backend=None, *,
-                 face_with_free_shape: bool = False):
+                 face_with_free_shape: bool = False, reference_options: bool = False):
         sm, mp = cfg.surface_model, cfg.moshpp
         self.cfg, self.marker_meta = cfg, marker_meta
         self.backend = backend or DeviceBackend()
@@ -324,8 +329,22 @@ class StageI:
                 self.fingers = False
         self.free_betas = bool(mp.optimize_betas)
         self.face = face_flag(cfg, marker_meta, avail, face_with_free_shape)
-        if _get(mp, 'head_marker_corr_fname', None) is not None:
-            raise NotImplementedError('moshpp.head_marker_corr_fname (chmosh.py:250-264,364-372) is outside this build')
+        self.reference_options = reference_options
+        # the head-marker correlation prior (chmosh.py:252-266): head_ids / head_corr stay None when it does not apply
+        self.head_ids, self.head_corr = None, None
+        corr_fname = _get(mp, 'head_marker_corr_fname', None)
+        if corr_fname is not None:
+            if not reference_options:
+                raise NotImplementedError('moshpp.head_marker_corr_fname (chmosh.py:252-266,360-373) applies only when asked to '
+                                          '(reference_options=True); otherwise set it to None')
+            head_meta = np.load(corr_fname)
+            head_labels = [str(l) for l in head_meta['mrk_labels']]
+            missing = [l for l in head_labels if l not in marker_meta['marker_vids']]
+            if missing:
+                logger.debug(f'not all of the head markers are in the layout, the head-marker correlation is not used: {missing}')
+            else:
+                self.head_ids = [self.labels.index(l) for l in head_labels]
+                self.head_corr = np.asarray(head_meta['corr'], dtype=np.float64)                # K x H
         self.model = model = _pack.load_surface_model(sm.fname, pose_hand_prior_fname=_get(mp, 'pose_hand_prior_fname'),
                                                       use_hands_mean=bool(sm.use_hands_mean), dof_per_hand=int(sm.dof_per_hand),
                                                       v_template=v_template, surface_model_type=sm.type)
@@ -403,6 +422,8 @@ class StageI:
             except (KeyError, AttributeError):
                 base = w['stagei_wt_init']
             out['init'][k] = base * anneal
+        if self.head_ids is not None:       # the body type's init weight, else the base one (chmosh.py:368-369)
+            out['init_head_corr'] = out['init'].get('body', w['stagei_wt_init'] * anneal)
         if self.face:                                                                               # chmosh.py:322-324
             out['poseF'], out['expr'] = w['stagei_wt_poseF'] * anneal, w['stagei_wt_expr'] * anneal
         return out
@@ -445,8 +466,18 @@ class StageI:
         w_init = np.zeros(M)
         for k, mask in self.marker_meta['marker_type_mask'].items():
             mask = np.asarray(mask, dtype=bool)
+            if self.head_ids is not None:
+                # with the head-marker correlation prior the correlated markers leave their types' init terms and the
+                # 'head' type has none (chmosh.py:362-367); a type left without markers reports 0
+                if k == 'head':
+                    continue
+                mask = mask.copy()
+                mask[self.head_ids] = False
             w_init[mask] = wts['init'][k]
             sse[f'init_{k}'] = float(((r_init[mask] * wts['init'][k]) ** 2).sum())
+        if self.head_ids is not None:                                                            # chmosh.py:368-369
+            r_hc = wts['init_head_corr'] * self.head_corr.dot(r_init[self.head_ids])            # K x 3
+            sse['init_head_corr'] = float((r_hc ** 2).sum())
         # betas (AliasedBetas: all shape coefficients of the canonical model, chmosh.py:379)
         if self.free_betas:
             sse['beta'] = float(((self.betas * wts['beta']) ** 2).sum())
@@ -526,6 +557,18 @@ class StageI:
             # betas prior
             A[:nb, :nb] += wts['beta'] ** 2 * np.eye(nb)
             g[:nb] -= wts['beta'] ** 2 * self.betas[:nb]
+        if self.head_ids is not None:
+            # head-marker correlation rows w corr (ml - init)[head_ids]: dense over the latent unknowns of the correlated
+            # markers (d/d ml[head_ids[j]] = w corr[:, j] (x) I) and, with a free shape, d/d betas = w corr (x) d r_init/d betas
+            wh = wts['init_head_corr']
+            Jh = np.zeros((len(self.head_corr), 3, ns))
+            for j, i in enumerate(self.head_ids):
+                Jh[:, :, nb + 3 * i:nb + 3 * i + 3] += wh * self.head_corr[:, j, None, None] * np.eye(3)
+            if nb:
+                Jh[:, :, :nb] = wh * np.einsum('kh,hib->kib', self.head_corr, Gi[self.head_ids])
+            Jh = Jh.reshape(-1, ns)
+            A[:ns, :ns] += Jh.T.dot(Jh)
+            g[:ns] -= Jh.T.dot(r_hc.reshape(-1))
         # surf rows
         with np.errstate(divide='ignore', invalid='ignore'):
             gs = np.nan_to_num(0.5 / np.sqrt(np.abs(xs))) * (xs != 0) * direction * wts['surf']
@@ -567,7 +610,52 @@ class StageI:
         _, _, _, A, g, (pk, free, n_p) = self.evaluate(True, wts, detailed)[:6]
         pose_ids = np.asarray([int(i) - 3 for i in free[3:n_p] if i < 3 + pk.p_red], dtype=np.int64)
         ne = n_p - 3 - len(pose_ids)                     # the expression columns follow the pose ids (optimize_face, Step 2)
-        p = self.get_x(pose_ids, nb, ne)
+        self._dogleg(A, g, self.get_x(pose_ids, nb, ne), lambda x: self.set_x(x, pose_ids, nb, ne),
+                     lambda: self.evaluate(False, wts, detailed)[0], lambda: self.evaluate(True, wts, detailed)[3:5],
+                     nb + 3 * self.M, n_p, e_3, maxiter, delta_0, e_1, e_2)
+
+    # ---- extra_initial_rigid_adjustment (chmosh.py:230-232): the unweighted data residual of every picked frame wrt its root
+    #      orientation and translation, the latent markers, the shape and the attachment fixed ---------------------------------
+    def evaluate_rigid(self, want_jac: bool):
+        """Data SSE, and with want_jac the block-diagonal normal equations of the unknowns [trans | pose[:3]] of every frame."""
+        F = self.F
+        self.stats['evaluations'] += 1
+        self.stats['linearisations'] += int(want_jac)
+        pk = self.pack_for(False, self.can(self.betas[:self.nb]))
+        pk.free_step1 = np.arange(6, dtype=np.int32)                     # columns 0..5 of x = [trans | pose | linear block]
+        x = np.zeros((F, pk.nx))
+        x[:, :3], x[:, 3:3 + pk.p_red] = self.trans, self.pose
+        if self.face:
+            x[:, 3 + pk.p_red + pk.n_dmpl - pk.n_expr:] = self.expr
+        opts = _lib.make_options(None)
+        opts.wt_data, opts.wt_poseB, opts.wt_poseH = 1.0, 0.0, 0.0
+        dev = self.backend.linearize(pk, opts, self.obs, self.vis, x, 1, want_jac)
+        total = float(dev['errs'][:, 0].sum())
+        if not want_jac:
+            return total
+        A = np.zeros((6 * F, 6 * F))
+        for f in range(F):
+            A[6 * f:6 * f + 6, 6 * f:6 * f + 6] = dev['A'][f]
+        self._last_total = total
+        return A, dev['g'].reshape(-1).copy()
+
+    def get_rigid_x(self):
+        return np.concatenate([self.trans, self.pose[:, :3]], axis=1).reshape(-1)
+
+    def set_rigid_x(self, x):
+        x = x.reshape(self.F, 6)
+        self.trans[:] = x[:, :3]
+        self.pose[:, :3] = x[:, 3:]
+
+    def minimize_rigid(self, maxiter, e_3=1e-3, delta_0=0.5, e_1=1e-15, e_2=1e-15):
+        """One dog-leg over all picked frames with one trust region; the normal equations have no shared block."""
+        A, g = self.evaluate_rigid(True)
+        self._dogleg(A, g, self.get_rigid_x(), self.set_rigid_x, lambda: self.evaluate_rigid(False),
+                     lambda: self.evaluate_rigid(True), 0, 6, e_3, maxiter, delta_0, e_1, e_2)
+
+    def _dogleg(self, A, g, p, set_x, sse_at, linearize, ns, n_p, e_3, maxiter, delta_0, e_1, e_2):
+        """The dog-leg iterations from the normal equations (A, g) at p, whose SSE is self._last_total.  ``set_x`` puts a
+        state vector into the solver, ``sse_at()`` evaluates the objective there, ``linearize()`` returns its (A, g)."""
         sse0 = self._last_total
         delta = delta_0
         done = np.linalg.norm(g, np.inf) < e_1
@@ -583,7 +671,7 @@ class StageI:
                     d_dl = (delta / np.linalg.norm(d_sd)) * d_sd
                 else:
                     if d_gn is None:
-                        d_gn = _solve_arrow(A, g, nb + 3 * self.M, n_p, self.F)
+                        d_gn = _solve_arrow(A, g, ns, n_p, self.F)
                     if np.linalg.norm(d_gn) <= delta:
                         d_dl = d_gn.copy()
                     else:
@@ -596,8 +684,8 @@ class StageI:
                 if np.linalg.norm(d_dl) <= e_2 * np.linalg.norm(p):
                     done = True
                 else:
-                    self.set_x(p + d_dl, pose_ids, nb, ne)
-                    sse1 = self.evaluate(False, wts, detailed)[0]
+                    set_x(p + d_dl)
+                    sse1 = sse_at()
                     rho = sse0 - sse1
                     if rho > 0:
                         with np.errstate(divide='ignore', invalid='ignore'):
@@ -608,7 +696,7 @@ class StageI:
                         if e_3 > 0.0 and (sse0 - sse1) / sse0 < e_3:
                             done = True
                         else:
-                            _, _, _, A, g, _ = self.evaluate(True, wts, detailed)[:6]
+                            A, g = linearize()
                             sse0 = sse1
                             if np.linalg.norm(g, np.inf) < e_1:
                                 done = True
@@ -622,19 +710,23 @@ class StageI:
                     break
             if not done and it >= maxiter:
                 done = True
-        self.set_x(p, pose_ids, nb, ne)
+        set_x(p)
         self.stats['minimisations'] += 1
 
     def run(self):
         cfg = self.cfg
-        if bool(_get(cfg.opt_settings, 'extra_initial_rigid_adjustment', False)):               # chmosh.py:230-232
-            raise NotImplementedError('extra_initial_rigid_adjustment is outside this build')
+        extra_rigid = bool(_get(cfg.opt_settings, 'extra_initial_rigid_adjustment', False))
+        if extra_rigid and not self.reference_options:                                           # chmosh.py:230-232
+            raise NotImplementedError('opt_settings.extra_initial_rigid_adjustment runs only when asked to '
+                                      '(reference_options=True)')
         ann = list(cfg.opt_settings.weights['stagei_wt_annealing'])
         # rigid alignment of every frame to its markers (chmosh.py:225-229)
         _, _, dev = self.evaluate(False, self.weights_for(ann[0]), False)
         for f in range(self.F):
             v = self.vis[f]
             self.pose[f, :3], self.trans[f] = rigid_fit(dev['markers_sim'][f][v], self.obs[f][v])
+        if extra_rigid:     # (e_3 is the reference's fixed 1e-3, not stagei_lr)
+            self.minimize_rigid(int(cfg.opt_settings.maxiter))
         sse = {}
         for tidx, a in enumerate(ann):
             detailed = tidx > len(ann) - 3                                                       # chmosh.py:311
@@ -645,13 +737,17 @@ class StageI:
 
 
 def mosh_stagei(stagei_frames: List[Dict[str, np.ndarray]], cfg, betas_fname=None, v_template_fname=None, *, marker_meta=None,
-                device: int = 0, backend=None, face_with_free_shape: bool = False) -> dict:
+                device: int = 0, backend=None, face_with_free_shape: bool = False, reference_options: bool = False) -> dict:
     """Stage I of MoSh++ on one H100.  Positional arguments as in the reference (chmosh.py:83-85).  The marker layout is read
     from ``cfg.dirs.marker_layout.fname`` like the reference does (chmosh.py:120-125), or handed over loaded as ``marker_meta``.
 
     ``face_with_free_shape``: with ``optimize_betas`` and ``optimize_face`` on SMPL-X, fit the shape and the jaw and expressions
     of every picked frame together instead of raising NotImplementedError (the reference's answer; its log suggests running
-    Stage I twice, for the shape without the face markers and then for the face with that shape).  Off by default."""
+    Stage I twice, for the shape without the face markers and then for the face with that shape).  Off by default.
+
+    ``reference_options``: honour ``moshpp.head_marker_corr_fname`` (the head-marker correlation prior, chmosh.py:252-266,
+    360-373) and ``opt_settings.extra_initial_rigid_adjustment`` (chmosh.py:230-232) as the reference does.  Off by default:
+    then either option in ``cfg`` raises NotImplementedError.  With both options off in ``cfg`` the keyword changes nothing."""
     if marker_meta is None:                                                                      # chmosh.py:120-125
         mc = cfg.mocap
         marker_meta = load_marker_layout(cfg.dirs.marker_layout.fname, exclude_markers=_get(mc, 'exclude_markers'),
@@ -665,7 +761,7 @@ def mosh_stagei(stagei_frames: List[Dict[str, np.ndarray]], cfg, betas_fname=Non
         betas = np.load(betas_fname)['betas']
     v_template = _read_vertices(v_template_fname) if v_template_fname else None
     s = StageI(stagei_frames, cfg, marker_meta, betas=betas, v_template=v_template, backend=backend or DeviceBackend(device),
-               face_with_free_shape=face_with_free_shape)
+               face_with_free_shape=face_with_free_shape, reference_options=reference_options)
     sse, dev = s.run()
     can_v = s.can(s.betas[:s.nb])
     d2 = ((s.ml[:, None, :] - can_v[None]) ** 2).sum(-1)                                        # chmosh.py:422-424: nearest vertex

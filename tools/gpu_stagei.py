@@ -2,7 +2,9 @@
 coefficients -- through moshpp_b200.stagei.mosh_stagei; with --oracle also the float64 oracle on the host cores (parity + time).
 --face80: SMPL-X with face markers at the reference's size (16 free betas, 80 expressions), the shape and every picked frame's
 jaw and expressions fitted together (face_with_free_shape).
-Usage: python tools/gpu_stagei.py [--oracle] [--frames 12] [--face80]"""
+--reference-options: with the head-marker correlation prior (a synthetic K x H file over the LFHD / RFHD / LBHD / RBHD
+markers) and the extra initial rigid adjustment, both through reference_options=True.
+Usage: python tools/gpu_stagei.py [--oracle] [--frames 12] [--face80] [--reference-options]"""
 import argparse
 import copy
 import json
@@ -25,6 +27,7 @@ def main():
     ap.add_argument('--frames', type=int, default=12)
     ap.add_argument('--config', default='C5')
     ap.add_argument('--face80', action='store_true')
+    ap.add_argument('--reference-options', action='store_true')
     a = ap.parse_args()
     d = tempfile.mkdtemp(prefix='mosh_stagei_')
     if a.face80:
@@ -33,6 +36,14 @@ def main():
     cfg = copy.deepcopy(case['cfg'])
     cfg.moshpp.optimize_betas = True
     kw = dict(face_with_free_shape=True) if a.face80 else {}
+    if a.reference_options:
+        head = [l for l in ('LFHD', 'RFHD', 'LBHD', 'RBHD') if l in case['marker_meta']['marker_vids']]
+        rng = np.random.default_rng(0)
+        corr = np.vstack([np.eye(len(head)) + rng.normal(0, 0.2, (len(head), len(head))), rng.normal(0, 0.5, (2, len(head)))])
+        cfg.moshpp.head_marker_corr_fname = os.path.join(d, 'ssm_head_marker_corr.npz')
+        np.savez(cfg.moshpp.head_marker_corr_fname, mrk_labels=np.asarray(head), corr=corr)
+        cfg.opt_settings.extra_initial_rigid_adjustment = True
+        kw['reference_options'] = True
     mocap = MocapSession(case['mocap_fname'], cfg.mocap.unit)
     frames = mocap.markers_asdict()
     pick = np.linspace(0, len(frames) - 1, a.frames).astype(int)
@@ -49,7 +60,9 @@ def main():
             'latent_err_vs_truth_mm': float(1e3 * np.abs(out['markers_latent'] - case['markers_latent']).max())}
     if a.face80:
         line['workload'] += ', face: jaw + 80 expressions per frame, shape free'
-    if a.oracle and not a.face80:
+    if a.reference_options:
+        line['workload'] += ', head-marker correlation prior + extra initial rigid adjustment'
+    if a.oracle and not (a.face80 or a.reference_options):
         from oracle import stagei as ostagei
         t0 = time.perf_counter()
         ref = ostagei.mosh_stagei(frames, cfg, marker_meta=case['marker_meta'])
