@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MOSH2_VERSION 107
+#define MOSH2_VERSION 108
 
 enum {
     MOSH2_OK = 0,
@@ -96,6 +96,11 @@ typedef struct mosh2_options {
     int32_t optimize_fingers, optimize_dynamics;
     double wt_poseF, wt_expr;  /* moshpp_conf.yaml: stageii_wt_poseF (annealed), stageii_wt_expr */
     int32_t optimize_face;
+    /* Geman-McClure data term (scan2mesh/robustifiers.py:33-100 GMOf), 0 = off (the reference's least squares).  sigma > 0
+     * (metres): every data row of a visible marker becomes wd psi(sim - obs), psi(e) = sigma e / sqrt(sigma^2 + e^2), one row
+     * per coordinate, and its Jacobian row is scaled by psi'(e) = (sigma^2 / (sigma^2 + e^2))^(3/2).  The data column of errs
+     * then reports the robust SSE.  The first-frame Procrustes start stays non-robust. */
+    double robust_sigma;
 } mosh2_options;
 
 /* Outputs, one row per input frame (rows of skipped frames are zero). */

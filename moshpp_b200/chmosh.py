@@ -516,17 +516,40 @@ def _read_capture(fname: str, cfg, latent_labels, labels_map, device_adapter: bo
     return dict(fname=fname, cfg=cfg, labels=labels, mocap=mocap, sel=sel, raw_cols=raw_cols, obs=obs, vis=vis, F=F)
 
 
+def check_robust_sigma(robust_data_sigma) -> Optional[float]:
+    """The ``robust_data_sigma`` keyword of the Stage-II entry points: None (the reference's least-squares data term) or a
+    finite sigma > 0 in metres (the Geman-McClure data term, include/mosh2.h ``mosh2_options.robust_sigma``)."""
+    if robust_data_sigma is None:
+        return None
+    s = float(robust_data_sigma)
+    if not (np.isfinite(s) and s > 0):
+        raise ValueError(f'robust_data_sigma must be a finite sigma > 0 (metres) or None, not {robust_data_sigma!r}')
+    return s
+
+
+def with_robust_sigma(opts, robust_data_sigma):
+    """``opts`` with the Geman-McClure data term at ``robust_data_sigma`` (``check_robust_sigma``): a copy, so that the
+    options of the subject cache stay as prepared; ``opts`` itself for None."""
+    s = check_robust_sigma(robust_data_sigma)
+    if s is None:
+        return opts
+    o = _lib.Options.from_buffer_copy(opts)
+    o.robust_sigma = s
+    return o
+
+
 def _subject(seqs, cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname, device: int,
-             subject_cache: bool = True) -> dict:
+             subject_cache: bool = True, robust_data_sigma=None) -> dict:
     """A subject of a launch: its captures ``seqs`` (``_read_capture``) with its pack, options, flags and device model from
     the subject cache, or with ``subject_cache=False`` prepared for this call alone (``model`` None: ``_solve_launch`` makes
-    it and closes it at the end)."""
+    it and closes it at the end).  ``robust_data_sigma``: the Geman-McClure data term of this call (``with_robust_sigma``)."""
     if subject_cache:
         pk, opts, flags, model, cache_hit = subject_for(cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname, device)
     else:
         pk, opts, flags = prepare_stageii(cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname)
         model, cache_hit = None, False
-    return dict(seqs=seqs, pk=pk, opts=opts, flags=flags, model=model, cache_hit=cache_hit, device=device)
+    return dict(seqs=seqs, pk=pk, opts=with_robust_sigma(opts, robust_data_sigma), flags=flags, model=model, cache_hit=cache_hit,
+                device=device, robust_data_sigma=check_robust_sigma(robust_data_sigma))
 
 
 def _resolve_schedule(pk, mode: str, counts, chunk_len, chunk_warmup, warmup_full, first_extra, precision, verify: bool,
@@ -656,6 +679,8 @@ def _solve_launch(subs, sched: dict, t0: float, laps: Optional[_Laps] = None):
             'b200': {'device_adapter': s['raw_cols'] is not None, 'status': r.status.copy(), 'counters': r.counters.copy(),
                      'pose_reduced': r.pose[solved], 'frame_ids': np.nonzero(solved)[0]},
         })
+        if sub.get('robust_data_sigma') is not None:
+            data['stageii_debug_details']['b200']['robust_data_sigma'] = sub['robust_data_sigma']
         outs.append(data)
     laps('assemble_ms')
     n_fb = int(((res.status & _lib.ST_GN_FALLBACK) != 0).sum())
@@ -672,7 +697,7 @@ def mosh_stageii(mocap_fname: str, cfg, markers_latent: np.ndarray, latent_label
                  chunk_len: Optional[int] = None, chunk_warmup: Optional[int] = None, warmup_full: Optional[int] = None,
                  first_extra: Optional[int] = None, precision: Optional[str] = None, verify: bool = True, boundary_tol=None,
                  sm_budget: int = NUM_SMS, labels_map='general', subject_cache: bool = True,
-                 device_adapter: bool = True) -> dict:
+                 device_adapter: bool = True, robust_data_sigma: Optional[float] = None) -> dict:
     """Stage II of MoSh++ on one H100.  Positional arguments as in the reference (chmosh.py:458-459).
 
     Keyword-only extras.  ``mode``: 'fast' (default) = float32, chunked in time with a verified warm-up -- within
@@ -686,13 +711,20 @@ def mosh_stageii(mocap_fname: str, cfg, markers_latent: np.ndarray, latent_label
     per-subject constants and their device copy for the next sequences of the same subject (keyed by the content of every
     input; nothing sequence-dependent is cached).  ``device_adapter``: the mocap input adapter (missing-sample rule, label
     order, units) runs on the GPU from the raw marker table of the file; False = on the host in front of the solve.
+    ``robust_data_sigma``: None (default) = the reference's least-squares data term; sigma > 0 (metres) = the Geman-McClure
+    data term of the reference's ``GMOf`` (scan2mesh/robustifiers.py), rows wd sigma e / sqrt(sigma^2 + e^2) per coordinate of
+    e = sim - obs, in every dog-leg of every frame (warm-up and boundary repair included) but not in the first frame's
+    Procrustes start.  ``stageii_errs['data']`` then reports the robust SSE, the value minimised; sigma is recorded in
+    ``b200['robust_data_sigma']`` (absent without it).
     """
     t0 = time.time()
     laps = _Laps()
     _check_mode(mode)
+    check_robust_sigma(robust_data_sigma)
     cap = _read_capture(mocap_fname, cfg, latent_labels, labels_map, device_adapter)
     laps('read_mocap_ms')
-    sub = _subject([cap], cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname, device, subject_cache)
+    sub = _subject([cap], cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname, device, subject_cache,
+                   robust_data_sigma)
     laps('prepare_ms')
     sched = _resolve_schedule(sub['pk'], mode, [cap['F']], chunk_len, chunk_warmup, warmup_full, first_extra, precision, verify,
                               boundary_tol, sm_budget)
@@ -710,7 +742,8 @@ def mosh_stageii_batch(mocap_fnames, cfg, markers_latent: np.ndarray, latent_lab
                        v_template_fname=None, *, device: int = 0, mode: str = 'fast', chunk_len: Optional[int] = None,
                        chunk_warmup: Optional[int] = None, warmup_full: Optional[int] = None, first_extra: Optional[int] = None,
                        precision: Optional[str] = None, verify: bool = True, boundary_tol=None, sm_budget: int = NUM_SMS,
-                       labels_map='general', subject_cache: bool = True, device_adapter: bool = True) -> list:
+                       labels_map='general', subject_cache: bool = True, device_adapter: bool = True,
+                       robust_data_sigma: Optional[float] = None) -> list:
     """Stage II of several captures of ONE subject (one Stage-I result, one ``cfg`` apart from ``mocap.fname``) in one launch.
 
     Returns one dictionary per capture, in the order of ``mocap_fnames``: what ``mosh_stageii`` returns for that capture with
@@ -724,10 +757,12 @@ def mosh_stageii_batch(mocap_fnames, cfg, markers_latent: np.ndarray, latent_lab
     check, totals), marked ``'shared': True`` -- the same for every capture of the call."""
     t0 = time.time()
     _check_mode(mode)
+    check_robust_sigma(robust_data_sigma)
     seqs = [_read_capture(fn, cfg, latent_labels, labels_map, device_adapter) for fn in mocap_fnames]
     if not seqs:
         raise ValueError('no captures given')
-    sub = _subject(seqs, cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname, device, subject_cache)
+    sub = _subject(seqs, cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname, device, subject_cache,
+                   robust_data_sigma)
     counts = [s['F'] for s in seqs]
     sched = _resolve_schedule(sub['pk'], mode, counts, chunk_len, chunk_warmup, warmup_full, first_extra, precision, verify,
                               boundary_tol, sm_budget)
@@ -771,7 +806,7 @@ def launch_groups(keys) -> list:
 def mosh_stageii_subjects(subjects, *, device: int = 0, mode: str = 'fast', chunk_len: Optional[int] = None,
                           chunk_warmup: Optional[int] = None, warmup_full: Optional[int] = None, first_extra: Optional[int] = None,
                           precision: Optional[str] = None, verify: bool = True, boundary_tol=None, sm_budget: int = NUM_SMS,
-                          labels_map='general', device_adapter: bool = True) -> list:
+                          labels_map='general', device_adapter: bool = True, robust_data_sigma: Optional[float] = None) -> list:
     """Stage II of the captures of SEVERAL subjects, with as few launches as their models allow.
 
     ``subjects``: dictionaries with ``cfg``, ``mocap_fnames`` and the subject's Stage-I outputs ``markers_latent``,
@@ -785,11 +820,18 @@ def mosh_stageii_subjects(subjects, *, device: int = 0, mode: str = 'fast', chun
     boundary tolerance) are equal share one multi-model job (mosh2_job_create_multi) and one verified launch
     (``launch_verified``); e.g. male and female SMPL-H subjects share a launch, a DMPL subject (float64 exact preset) does not
     share one with float32 SMPL-H subjects.  ``b200['batch']`` holds the figures of the capture's launch, marked
-    ``'shared': True``, and ``'launches'``, the number of launches of the call."""
+    ``'shared': True``, and ``'launches'``, the number of launches of the call.
+
+    ``robust_data_sigma`` (as in ``mosh_stageii``) applies to every subject; a subject dictionary may carry its own
+    ``robust_data_sigma``, which takes its place for that subject.  The value is part of the options, so subjects with
+    different values never share a launch."""
     global SUBJECT_CACHE_SIZE
     t0 = time.time()
     _check_mode(mode)
+    check_robust_sigma(robust_data_sigma)
     subjects = list(subjects)
+    for s in subjects:
+        check_robust_sigma(s.get('robust_data_sigma', robust_data_sigma))
     bound = SUBJECT_CACHE_SIZE
     SUBJECT_CACHE_SIZE = max(bound, len(subjects))      # (every model of the call stays open until its launch is done)
     try:
@@ -799,7 +841,7 @@ def mosh_stageii_subjects(subjects, *, device: int = 0, mode: str = 'fast', chun
             if not seqs:
                 raise ValueError('a subject without captures')
             subs.append(_subject(seqs, s['cfg'], s['markers_latent'], s['latent_labels'], s['betas'], s['marker_meta'],
-                                 s.get('v_template_fname'), device))
+                                 s.get('v_template_fname'), device, robust_data_sigma=s.get('robust_data_sigma', robust_data_sigma)))
         groups = launch_groups([subject_launch_key(sub['pk'], sub['opts'], mode) for sub in subs])
         out = [[] for _ in subs]
         for g, members in enumerate(groups):

@@ -468,6 +468,7 @@ void mosh2_default_options(mosh2_options *o) {
     o->delta_0 = 0.5; o->e3_first = 1e-3; o->e3 = 1e-2; o->maxiter = 100;
     o->optimize_fingers = 0; o->optimize_dynamics = 0;
     o->wt_poseF = 1.0; o->wt_expr = 1.0; o->optimize_face = 0;
+    o->robust_sigma = 0;       // the reference's least-squares data term
 }
 
 int mosh2_model_create(const mosh2_model_desc *d, int device, mosh2_model **out) {
@@ -516,6 +517,7 @@ int mosh2_job_create_batch(mosh2_model *m, const mosh2_options *opt, int32_t n_s
     if (total > 0x3fffffff) return fail(MOSH2_E_TOO_LARGE, "%lld frames in one job", total);
     const int32_t n_frames = int32_t(total);
     if (precision != MOSH2_F32 && precision != MOSH2_F64) return fail(MOSH2_E_INVALID, "precision must be MOSH2_F32 or MOSH2_F64");
+    if (!mosh2_host::robust_sigma_ok(*opt)) return fail(MOSH2_E_INVALID, "robust_sigma must be 0 (off) or a finite sigma > 0");
     *out = nullptr;
     CU(cudaSetDevice(m->device));
     if (const int rc = m->ensure(precision)) return rc;
@@ -745,6 +747,7 @@ int mosh2_job_linearize(mosh2_job *j, const mosh2_options *opt, int32_t step, in
     if (!j || !x || !out || (step != 1 && step != 2)) return fail(MOSH2_E_INVALID, "bad argument");
     if (j->n_chunks < j->n_frames) return fail(MOSH2_E_INVALID, "mosh2_job_linearize needs a job of one-frame chunks (chunk_len = 1)");
     if (j->d_models) return fail(MOSH2_E_INVALID, "mosh2_job_linearize does not take a multi-model job");
+    if (opt && !mosh2_host::robust_sigma_ok(*opt)) return fail(MOSH2_E_INVALID, "robust_sigma must be 0 (off) or a finite sigma > 0");
     CU(cudaSetDevice(j->model->device));
     if (opt) mosh2_host::apply_call_weights(j->opt, *opt);
     if (j->precision == MOSH2_F64) return linearize<double>(j, j->model->f64.m, step, build, x, out);

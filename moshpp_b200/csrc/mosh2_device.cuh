@@ -162,6 +162,7 @@ struct Options {
     int maxiter, optimize_fingers, optimize_dynamics;
     double wt_poseF, wt_expr;
     int optimize_face;
+    double robust_sigma;    // > 0: Geman-McClure data term (mosh2_options::robust_sigma), 0: least squares
 };
 
 template <class real>
@@ -794,6 +795,41 @@ struct Solver {
         }
     }
 
+    // ---- simulated marker mi from its three posed attachment vertices (transformed_lm.py:130-159)
+    M2_D void sim_marker(int mi, real mk[3]) const {
+        const real *v0 = w.vp + 9 * mi, *v1 = v0 + 3, *v2 = v0 + 6;
+        real e1[3] = {v1[0] - v0[0], v1[1] - v0[1], v1[2] - v0[2]};
+        real e2[3] = {v2[0] - v0[0], v2[1] - v0[1], v2[2] - v0[2]};
+        const real n1 = r_sqrt(e1[0] * e1[0] + e1[1] * e1[1] + e1[2] * e1[2]);
+        real f1[3] = {e1[0] / n1, e1[1] / n1, e1[2] / n1};
+        real nn[3];
+        cross3(e1, e2, nn);
+        const real n2 = r_sqrt(nn[0] * nn[0] + nn[1] * nn[1] + nn[2] * nn[2]);
+        real f2[3] = {nn[0] / n2, nn[1] / n2, nn[2] / n2};
+        real f3[3];
+        cross3(f1, f2, f3);
+        const real k1 = w.c_coefs[3 * mi], k2 = w.c_coefs[3 * mi + 1], k3 = w.c_coefs[3 * mi + 2];
+        for (int q = 0; q < 3; ++q) mk[q] = v0[q] + k1 * f1[q] + k2 * f2[q] + k3 * f3[q];
+    }
+
+    // ---- Geman-McClure data term (Options::robust_sigma > 0; scan2mesh/robustifiers.py:33-100 GMOf = SignedSqrt(GMOfInternal)):
+    //      the row of residual e = sim - obs is wd psi(e), psi(e) = sigma e / sqrt(sigma^2 + e^2), and its Jacobian row is the
+    //      least-squares one times psi'(e) = (sigma^2 / (sigma^2 + e^2))^(3/2).  psi' is recovered from the stored row alone:
+    //      with u = rm / (wd sigma) = e / sqrt(sigma^2 + e^2), psi' = (1 - u^2)^(3/2).  (In float32 1 - u^2 loses relative accuracy
+    //      as the marker saturates -- about 1e-5 at e = 10 sigma -- where psi' itself is 1e-3 and the row no longer matters.)
+    //      A row with e = 0 exactly gets psi' = 0, as the reference's SignedSqrt does (invisible rows are zero already).
+    M2_D bool robust() const { return job.opt.robust_sigma > 0; }
+    M2_D real data_row_gm(real e) const {
+        const real s = real(job.opt.robust_sigma);
+        return wd * (s * e / r_sqrt(s * s + e * e));
+    }
+    M2_D real data_dpsi_gm(real rm) const {
+        const real u = rm / (wd * real(job.opt.robust_sigma));
+        real t = real(1) - u * u;
+        t = t > real(0) ? t : real(0);
+        return rm != real(0) ? t * r_sqrt(t) : real(0);
+    }
+
     // ---- forward evaluation at state xs; leaves SSE terms in w.sc[0..6], argmin component in w.isc[0]
     //      `reuse`: the forward scratch of the previous evaluation already belongs to this state (the last trial step was
     //      accepted, so x = that trial point): only the terms that depend on the frame's observations, weights and targets
@@ -960,30 +996,36 @@ struct Solver {
         M2_TACC(3);
         }   // !reuse
         // simulated markers and data residual (transformed_lm.py:130-159); the prior products share the phase
-        if (reuse) {
+        if (robust()) {
+            // Geman-McClure data term: the same loops, rows wd psi(e) (data_row_gm)
+            if (reuse) {
+                CTA_FOR(mi, d.M) {
+                    const bool vis = w.vis[mi] != 0;
+                    for (int q = 0; q < 3; ++q) w.rm[3 * mi + q] = vis ? data_row_gm(w.mk[3 * mi + q] - w.obs[3 * mi + q]) : real(0);
+                }
+            } else
+                CTA_FOR(mi, d.M) {
+                    real mk[3];
+                    sim_marker(mi, mk);
+                    const bool vis = w.vis[mi] != 0;
+                    for (int q = 0; q < 3; ++q) {
+                        w.mk[3 * mi + q] = mk[q];
+                        w.rm[3 * mi + q] = vis ? data_row_gm(mk[q] - w.obs[3 * mi + q]) : real(0);
+                    }
+                }
+        } else if (reuse) {
             CTA_FOR(mi, d.M) {
                 const bool vis = w.vis[mi] != 0;
                 for (int q = 0; q < 3; ++q) w.rm[3 * mi + q] = vis ? (w.mk[3 * mi + q] - w.obs[3 * mi + q]) * wd : real(0);
             }
         } else
         CTA_FOR(mi, d.M) {
-            const real *v0 = w.vp + 9 * mi, *v1 = v0 + 3, *v2 = v0 + 6;
-            real e1[3] = {v1[0] - v0[0], v1[1] - v0[1], v1[2] - v0[2]};
-            real e2[3] = {v2[0] - v0[0], v2[1] - v0[1], v2[2] - v0[2]};
-            const real n1 = r_sqrt(e1[0] * e1[0] + e1[1] * e1[1] + e1[2] * e1[2]);
-            real f1[3] = {e1[0] / n1, e1[1] / n1, e1[2] / n1};
-            real nn[3];
-            cross3(e1, e2, nn);
-            const real n2 = r_sqrt(nn[0] * nn[0] + nn[1] * nn[1] + nn[2] * nn[2]);
-            real f2[3] = {nn[0] / n2, nn[1] / n2, nn[2] / n2};
-            real f3[3];
-            cross3(f1, f2, f3);
-            const real k1 = w.c_coefs[3 * mi], k2 = w.c_coefs[3 * mi + 1], k3 = w.c_coefs[3 * mi + 2];
+            real mk[3];
+            sim_marker(mi, mk);
             const bool vis = w.vis[mi] != 0;
             for (int q = 0; q < 3; ++q) {
-                const real mk = v0[q] + k1 * f1[q] + k2 * f2[q] + k3 * f3[q];
-                w.mk[3 * mi + q] = mk;
-                w.rm[3 * mi + q] = vis ? (mk - w.obs[3 * mi + q]) * wd : real(0);
+                w.mk[3 * mi + q] = mk[q];
+                w.rm[3 * mi + q] = vis ? (mk[q] - w.obs[3 * mi + q]) * wd : real(0);
             }
         }
         M2_SYNC();
@@ -1164,19 +1206,24 @@ struct Solver {
         }
     }
 
-    // ---- the three residual rows of marker `ml` of the tile (already weighted) in free-variable column `col`
-    M2_D void jf_store3(int ml, int col, real v0, real v1, real v2) {
+    // ---- the three residual rows of marker `ml` of the tile from marker t0 on (already weighted) in free-variable column
+    //      `col`; with the Geman-McClure data term each row times its psi' (data_dpsi_gm)
+    M2_D void jf_store3(int t0, int ml, int col, real v0, real v1, real v2) {
         real *J = w.Jf + 3 * ml * d.npad + col;
+        if (robust()) {
+            const real *r = w.rm + 3 * (t0 + ml);
+            v0 *= data_dpsi_gm(r[0]); v1 *= data_dpsi_gm(r[1]); v2 *= data_dpsi_gm(r[2]);
+        }
         J[0] = v0; J[d.npad] = v1; J[2 * d.npad] = v2;
     }
 
     // ---- column k (rows b0, b1, b2) of the finished 3x3 T1 block of marker `ml` of the tile and joint a: body joints go
     //      straight to their free column of the tile, weighted by sc (wd, or 0 for an invisible marker); hand joints go to
     //      the full-pose tile for the PCA chain (T2b)
-    M2_D void pose_col_store(int ml, int a, int k, real sc, real b0, real b1, real b2) {
+    M2_D void pose_col_store(int t0, int ml, int a, int k, real sc, real b0, real b1, real b2) {
         if (3 * a < m.body_dof) {
             const int col = w.colmap[3 + 3 * a + k];
-            if (col >= 0) jf_store3(ml, col, b0 * sc, b1 * sc, b2 * sc);
+            if (col >= 0) jf_store3(t0, ml, col, b0 * sc, b1 * sc, b2 * sc);
         } else {
             real *Jr = w.Jt + 3 * ml * d.NCt + (3 * a - m.body_dof) + k;
             Jr[0] = b0; Jr[d.NCt] = b1; Jr[2 * d.NCt] = b2;
@@ -1266,7 +1313,7 @@ struct Solver {
                         const real to2 = sel3(t, b2, b0, b1);
                         col3[r] = own + __shfl_sync(0xffffffffu, to1, src1) + __shfl_sync(0xffffffffu, to2, src2);
                     }
-                    if (valid) pose_col_store(ml, a, t, sc, col3[0], col3[1], col3[2]);
+                    if (valid) pose_col_store(t0, ml, a, t, sc, col3[0], col3[1], col3[2]);
                 }
             }
         };
@@ -1289,7 +1336,7 @@ struct Solver {
                 for (int q = 0; q < 9; ++q) blk[q] += part[q];
             }
             const real sc = w.vis[mi] ? wd : real(0);
-            for (int k = 0; k < 3; ++k) pose_col_store(ml, a, k, sc, blk[k], blk[3 + k], blk[6 + k]);
+            for (int k = 0; k < 3; ++k) pose_col_store(t0, ml, a, k, sc, blk[k], blk[3 + k], blk[6 + k]);
         }
 #endif
     }
@@ -1320,7 +1367,7 @@ struct Solver {
             }
             const int col = w.colmap[3 + d.PR + i];
             const real sc = w.vis[mi] ? wd : real(0);
-            if (col >= 0) jf_store3(ml, col, val[0] * sc, val[1] * sc, val[2] * sc);
+            if (col >= 0) jf_store3(t0, ml, col, val[0] * sc, val[1] * sc, val[2] * sc);
         }
     }
 
@@ -1329,7 +1376,7 @@ struct Solver {
         CTA_FOR(idx, tm * 3) {
             const int ml = idx / 3, q = idx - 3 * ml, col = w.colmap[q];
             const real v = w.vis[t0 + ml] ? wd : real(0);
-            if (col >= 0) jf_store3(ml, col, q == 0 ? v : real(0), q == 1 ? v : real(0), q == 2 ? v : real(0));
+            if (col >= 0) jf_store3(t0, ml, col, q == 0 ? v : real(0), q == 1 ? v : real(0), q == 2 ? v : real(0));
         }
         const int npadc = d.npad - n;
         CTA_FOR(idx, 3 * tm * npadc) w.Jf[(idx / npadc) * d.npad + n + idx % npadc] = 0;
@@ -1374,7 +1421,7 @@ struct Solver {
                 const int r = hb.r0 + 4 * rg + e;
                 if (r < hb.r1) {
                     const int col = w.colmap[3 + m.body_dof + r];
-                    if (col >= 0) jf_store3(ml, col, acc[e] * sc, acc[4 + e] * sc, acc[8 + e] * sc);
+                    if (col >= 0) jf_store3(t0, ml, col, acc[e] * sc, acc[4 + e] * sc, acc[8 + e] * sc);
                 }
             }
         }

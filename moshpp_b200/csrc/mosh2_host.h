@@ -208,14 +208,20 @@ inline mosh2::Options to_options(const mosh2_options &o) {
     q.num_train_markers = o.num_train_markers; q.delta_0 = o.delta_0; q.e3_first = o.e3_first; q.e3 = o.e3;
     q.maxiter = o.maxiter; q.optimize_fingers = o.optimize_fingers; q.optimize_dynamics = o.optimize_dynamics;
     q.wt_poseF = o.wt_poseF; q.wt_expr = o.wt_expr; q.optimize_face = o.optimize_face;
+    q.robust_sigma = o.robust_sigma;
     return q;
 }
 
-// The options a linearisation takes from its call (mosh2_job_linearize: Stage I anneals these weights between minimisations);
-// every other option stays as the job was created.
+// robust_sigma: 0 (off) or a finite sigma > 0
+inline bool robust_sigma_ok(const mosh2_options &o) {
+    return o.robust_sigma == 0 || (o.robust_sigma > 0 && o.robust_sigma < 1e300);
+}
+
+// The options a linearisation takes from its call (mosh2_job_linearize: Stage I anneals these weights between minimisations,
+// and leaves robust_sigma at 0); every other option stays as the job was created.
 inline void apply_call_weights(mosh2::Options &q, const mosh2_options &o) {
     q.wt_data = o.wt_data; q.wt_poseB = o.wt_poseB; q.wt_poseH = o.wt_poseH; q.wt_poseF = o.wt_poseF; q.wt_expr = o.wt_expr;
-    q.optimize_fingers = o.optimize_fingers;
+    q.optimize_fingers = o.optimize_fingers; q.robust_sigma = o.robust_sigma;
 }
 
 // Chunk table of a job that holds n_seq sequences back to back on its frame axis: kChunkRec ints per chunk -- first

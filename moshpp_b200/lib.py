@@ -13,7 +13,7 @@ import numpy as np
 
 from .pack import StageIIPack
 
-ABI_VERSION = 107          # MOSH2_VERSION of include/mosh2.h that the ctypes structs below encode
+ABI_VERSION = 108          # MOSH2_VERSION of include/mosh2.h that the ctypes structs below encode
 MOSH2_F32, MOSH2_F64 = 0, 1
 ST_SOLVED, ST_SKIPPED, ST_HAS_VELO, ST_HAS_EXTRAP, ST_GN_FALLBACK, ST_MAXITER, ST_SHORT_WARMUP = 1, 2, 4, 8, 16, 32, 64
 ERR_NAMES = ('data', 'poseB', 'velo', 'poseH', 'dmpl', 'extrap_dmpl', 'poseF', 'expr')   # column order of mosh2_result.errs
@@ -47,6 +47,7 @@ class Options(C.Structure):
         ('num_train_markers', C.c_double), ('delta_0', C.c_double), ('e3_first', C.c_double), ('e3', C.c_double),
         ('maxiter', C.c_int32), ('optimize_fingers', C.c_int32), ('optimize_dynamics', C.c_int32),
         ('wt_poseF', C.c_double), ('wt_expr', C.c_double), ('optimize_face', C.c_int32),
+        ('robust_sigma', C.c_double),
     ]
 
 
@@ -199,12 +200,13 @@ class DescHolder:
 
 
 def make_options(weights=None, *, maxiter: int = 100, optimize_fingers: bool = False,
-                 optimize_dynamics: bool = False, optimize_face: bool = False) -> Options:
-    """Stage-II weights (moshpp_conf.yaml:118-125) -> mosh2_options."""
+                 optimize_dynamics: bool = False, optimize_face: bool = False, robust_sigma: float = 0.0) -> Options:
+    """Stage-II weights (moshpp_conf.yaml:118-125) -> mosh2_options.  ``robust_sigma`` > 0 (metres): the Geman-McClure
+    data term (include/mosh2.h); 0: the reference's least squares."""
     o = Options(wt_data=400., wt_poseB=1.6, wt_poseH=1.0, wt_velo=2.5, wt_dmpl=1.0, wt_annealing=2.5,
                 wt_extrap_dmpl=6.0, num_train_markers=46., delta_0=0.5, e3_first=1e-3, e3=1e-2, maxiter=maxiter,
                 optimize_fingers=int(optimize_fingers), optimize_dynamics=int(optimize_dynamics),
-                wt_poseF=1.0, wt_expr=1.0, optimize_face=int(optimize_face))
+                wt_poseF=1.0, wt_expr=1.0, optimize_face=int(optimize_face), robust_sigma=float(robust_sigma))
     if weights is not None:
         g = (lambda k: weights[k])
         o.wt_data, o.wt_poseB, o.wt_poseH = float(g('stageii_wt_data')), float(g('stageii_wt_poseB')), float(g('stageii_wt_poseH'))
