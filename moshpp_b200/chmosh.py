@@ -517,7 +517,7 @@ def _read_capture(fname: str, cfg, latent_labels, labels_map, device_adapter: bo
 
 
 def check_robust_sigma(robust_data_sigma) -> Optional[float]:
-    """The ``robust_data_sigma`` keyword of the Stage-II entry points: None (the reference's least-squares data term) or a
+    """The ``robust_data_sigma`` keyword of the Stage-II entry points and of ``stagei.mosh_stagei``: None (the reference's least-squares data term) or a
     finite sigma > 0 in metres (the Geman-McClure data term, include/mosh2.h ``mosh2_options.robust_sigma``)."""
     if robust_data_sigma is None:
         return None

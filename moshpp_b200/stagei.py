@@ -36,6 +36,12 @@ stay shared (attachment, init, surface and beta terms as with a free shape), the
 the correlated markers by ``corr (ml - init)[head_ids]``, dense over their latent unknowns in the shared block; the extra
 initial rigid adjustment is one dog-leg over every frame's root orientation and translation on the unweighted data term, its
 normal equations 6 x 6 blocks from the same device linearisation with no shared block (DESIGN.md section 10).
+
+``robust_data_sigma`` (None by default: least squares): every data row of the four annealing steps and of the extra rigid
+adjustment becomes wd psi(e), the Geman-McClure row of Stage II (psi(e) = sigma e / sqrt(sigma^2 + e^2) per coordinate of a
+visible marker's e = sim - obs).  The device returns those rows and its own Jacobian columns robust already; the host scales the
+columns it adds through the attachment (latent markers, the shape's attachment part) by the same psi', recovered from the
+stored rows as the kernel does (``data_dpsi_gm``).  The Procrustes start and every other term stay least squares.
 """
 from __future__ import annotations
 
@@ -47,7 +53,7 @@ import numpy as np
 from . import lib as _lib
 from . import mesh_distance as _md
 from . import pack as _pack
-from .chmosh import _get, _read_vertices
+from .chmosh import _get, _read_vertices, check_robust_sigma
 
 logger = logging.getLogger('moshpp_b200')
 NUM_TRAIN_MARKERS = 46      # chmosh.py:100
@@ -236,6 +242,15 @@ def _solve_arrow(A, g, ns, n_p, F):
             return np.linalg.lstsq(A, g, rcond=None)[0]
 
 
+def data_dpsi_gm(r, wd, sigma):
+    """psi'(e) of the Geman-McClure data rows r = wd psi(e), recovered from the rows alone by the kernel's rule
+    (csrc/mosh2_device.cuh ``data_dpsi_gm``): u = r / (wd sigma) = e / sqrt(sigma^2 + e^2), psi' = (1 - u^2)^(3/2) clamped at
+    0, and 0 where the row is exactly 0 (e = 0, or an invisible marker)."""
+    u = r / (wd * sigma)
+    t = np.maximum(1.0 - u * u, 0.0)
+    return np.where(r != 0, t * np.sqrt(t), 0.0)
+
+
 class CanonicalBody:
     """can(betas) = can_0 + C betas[:nb]: the canonical mesh as an affine function of the free shape coefficients."""
 
@@ -313,8 +328,9 @@ def face_flag(cfg, marker_meta, avail_labels, face_with_free_shape: bool = False
 
 class StageI:
     def __init__(self, stagei_frames, cfg, marker_meta, betas=None, v_template=None, backend=None, *,
-                 face_with_free_shape: bool = False, reference_options: bool = False):
+                 face_with_free_shape: bool = False, reference_options: bool = False, robust_data_sigma=None):
         sm, mp = cfg.surface_model, cfg.moshpp
+        self.robust_sigma = check_robust_sigma(robust_data_sigma)           # None: the least-squares data term
         self.cfg, self.marker_meta = cfg, marker_meta
         self.backend = backend or DeviceBackend()
         self.labels = list(marker_meta['marker_vids'].keys())
@@ -448,6 +464,8 @@ class StageI:
         opts.wt_data, opts.wt_poseB, opts.wt_poseH = float(wts['data']), float(wts['poseB']), float(wts['poseH'])
         if self.face:
             opts.wt_poseF, opts.wt_expr = float(wts['poseF']), float(wts['expr'])
+        if self.robust_sigma is not None:
+            opts.robust_sigma = self.robust_sigma
         dev = self.backend.linearize(pk, opts, self.obs, self.vis, x, step, want_jac)
         sse = {'data': float(dev['errs'][:, 0].sum())}
         if pk.prior_k:
@@ -515,12 +533,17 @@ class StageI:
             Jf = dev['J'][f]                                     # 3M x n_f, weighted, zero rows where invisible
             r = dev['r'][f]
             wv = wts['data'] * self.vis[f].astype(np.float64)
+            # the weight of the rows through the attachment; with the robust data term each row also takes the psi' the
+            # device applied to its own columns of that row
+            wa = wv[:, None, None]
+            if self.robust_sigma is not None:
+                wa = wa * data_dpsi_gm(r, wts['data'], self.robust_sigma).reshape(M, 3, 1)
             Fp, _, _ = local_frames(dev['vp'][f, 0::3], dev['vp'][f, 1::3], dev['vp'][f, 2::3])   # rows f1, f2, f3 of the posed frames
             FpT = np.transpose(Fp, (0, 2, 1))                     # columns
             Jp = Jf[:, :n_p]
-            Jb = Jf[:, n_p:].reshape(M, 3, nb) + wv[:, None, None] * np.einsum('mij,mjb->mib', FpT, dk_db)
+            Jb = Jf[:, n_p:].reshape(M, 3, nb) + wa * np.einsum('mij,mjb->mib', FpT, dk_db)
             Jb = Jb.reshape(3 * M, nb)
-            Jm = wv[:, None, None] * np.einsum('mij,mjk->mik', FpT, Fcan)                          # 3x3 blocks d r_i / d ml_i
+            Jm = wa * np.einsum('mij,mjk->mik', FpT, Fcan)                                         # 3x3 blocks d r_i / d ml_i
             c0 = ns + f * n_p
             A[c0:c0 + n_p, c0:c0 + n_p] = dev['A'][f][:n_p, :n_p]
             g[c0:c0 + n_p] = dev['g'][f][:n_p]
@@ -629,6 +652,8 @@ class StageI:
             x[:, 3 + pk.p_red + pk.n_dmpl - pk.n_expr:] = self.expr
         opts = _lib.make_options(None)
         opts.wt_data, opts.wt_poseB, opts.wt_poseH = 1.0, 0.0, 0.0
+        if self.robust_sigma is not None:                   # (rows psi(e): the weight is 1)
+            opts.robust_sigma = self.robust_sigma
         dev = self.backend.linearize(pk, opts, self.obs, self.vis, x, 1, want_jac)
         total = float(dev['errs'][:, 0].sum())
         if not want_jac:
@@ -737,7 +762,8 @@ class StageI:
 
 
 def mosh_stagei(stagei_frames: List[Dict[str, np.ndarray]], cfg, betas_fname=None, v_template_fname=None, *, marker_meta=None,
-                device: int = 0, backend=None, face_with_free_shape: bool = False, reference_options: bool = False) -> dict:
+                device: int = 0, backend=None, face_with_free_shape: bool = False, reference_options: bool = False,
+                robust_data_sigma: Optional[float] = None) -> dict:
     """Stage I of MoSh++ on one H100.  Positional arguments as in the reference (chmosh.py:83-85).  The marker layout is read
     from ``cfg.dirs.marker_layout.fname`` like the reference does (chmosh.py:120-125), or handed over loaded as ``marker_meta``.
 
@@ -747,7 +773,17 @@ def mosh_stagei(stagei_frames: List[Dict[str, np.ndarray]], cfg, betas_fname=Non
 
     ``reference_options``: honour ``moshpp.head_marker_corr_fname`` (the head-marker correlation prior, chmosh.py:252-266,
     360-373) and ``opt_settings.extra_initial_rigid_adjustment`` (chmosh.py:230-232) as the reference does.  Off by default:
-    then either option in ``cfg`` raises NotImplementedError.  With both options off in ``cfg`` the keyword changes nothing."""
+    then either option in ``cfg`` raises NotImplementedError.  With both options off in ``cfg`` the keyword changes nothing.
+
+    ``robust_data_sigma``: None (default) = the reference's least-squares data term; sigma > 0 (metres) = the Geman-McClure
+    data term of Stage II (``chmosh.mosh_stageii``): every data row of the annealing steps and of the extra rigid adjustment
+    is wd sigma e / sqrt(sigma^2 + e^2) per coordinate of a visible marker's residual e = sim - obs, so that a swapped label or
+    a ghost marker in the picked frames pulls the shape and the latent markers with a bounded force.  The per-frame
+    Procrustes start and the init, head-correlation, shape, surface and pose terms stay least squares.
+    ``stagei_errs['data']`` then reports the robust SSE, the value minimised, and sigma is recorded in
+    ``stagei_debug_details['b200']['robust_data_sigma']`` (absent without it).  A sigma <= 0 or a non-finite one raises
+    ValueError."""
+    check_robust_sigma(robust_data_sigma)
     if marker_meta is None:                                                                      # chmosh.py:120-125
         mc = cfg.mocap
         marker_meta = load_marker_layout(cfg.dirs.marker_layout.fname, exclude_markers=_get(mc, 'exclude_markers'),
@@ -761,7 +797,8 @@ def mosh_stagei(stagei_frames: List[Dict[str, np.ndarray]], cfg, betas_fname=Non
         betas = np.load(betas_fname)['betas']
     v_template = _read_vertices(v_template_fname) if v_template_fname else None
     s = StageI(stagei_frames, cfg, marker_meta, betas=betas, v_template=v_template, backend=backend or DeviceBackend(device),
-               face_with_free_shape=face_with_free_shape, reference_options=reference_options)
+               face_with_free_shape=face_with_free_shape, reference_options=reference_options,
+               robust_data_sigma=robust_data_sigma)
     sse, dev = s.run()
     can_v = s.can(s.betas[:s.nb])
     d2 = ((s.ml[:, None, :] - can_v[None]) ** 2).sum(-1)                                        # chmosh.py:422-424: nearest vertex
@@ -772,6 +809,8 @@ def mosh_stagei(stagei_frames: List[Dict[str, np.ndarray]], cfg, betas_fname=Non
            'stagei_markers_sim_all': sims_all, 'stagei_markers_sim': [sims_all[f][s.vis[f]] for f in range(s.F)],
            'stagei_markers_obs': [s.obs[f][s.vis[f]] for f in range(s.F)], 'stagei_labels_obs': labels_obs,
            'b200': dict(s.stats)}
+    if s.robust_sigma is not None:
+        dbg['b200']['robust_data_sigma'] = s.robust_sigma
     if s.face:
         dbg['opt_models_expression'] = [e.copy() for e in s.expr]    # betas[es:es + ne] of each picked frame's model
     out = {'betas': s.betas.copy(), 'markers_latent': s.ml.copy(), 'latent_labels': s.labels, 'marker_meta': marker_meta,

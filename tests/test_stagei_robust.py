@@ -1,0 +1,509 @@
+"""Stage I with the Geman-McClure data term (``mosh_stagei(..., robust_data_sigma=sigma)``): every data row of the four
+annealing steps and of the extra rigid adjustment is wd psi(e), psi(e) = sigma e / sqrt(sigma^2 + e^2) per coordinate of a
+visible marker's e = sim - obs, its Jacobian row the least-squares one times psi'(e) = (sigma^2 / (sigma^2 + e^2))^(3/2).  The
+Procrustes start and the init, head-correlation, shape, surface and pose terms stay least squares.
+
+The float64 oracle of the robust objective, ``RobustData``, is a mixin over the oracle Stage-I solvers: the unchanged
+``oracle.StageISolver``, ``FaceOracle``, ``JointOracle`` and the ``ReferenceOptions`` mixin of the Stage-I test modules.
+
+CPU: the oracle against finite differences on rows of a swapped label and a ghost marker; the product on the host build of the
+device source against the oracle on corrupted picked frames (C2 with a free shape, CF with the face and a given shape, CF with
+``face_with_free_shape``, C2 with ``reference_options``); the keyword off and bad values; the recovery of the shape and the
+latent markers from corrupted picked frames, and what that does to a least-squares Stage II downstream; the head.  ``-m gpu``:
+one CUDA linearisation against the host build's, the CUDA library against the oracle, and the head with both stages robust."""
+import copy
+import ctypes as C
+import functools
+import json
+import os
+import pickle
+import shutil
+
+import numpy as np
+import pytest
+
+from conftest import EmuStageIBackend, dense_obs, stagei_case
+from moshpp_b200 import build, chmosh, lib
+from moshpp_b200 import stagei as product
+from oracle import stagei as oracle
+from test_robust_data import SIGMA, corrupt, gm_dpsi, gm_psi
+from test_stagei import _compare as _compare_body
+from test_stagei_face import FaceOracle, _compare as _compare_face, face_case
+from test_stagei_face_shape import JointOracle
+from test_stagei_reference_options import HEAD, ReferenceOptions, _assert_bit_identical, _check_stats, oracle_result, write_corr
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the float64 oracle of the robust objective
+# ---------------------------------------------------------------------------------------------------------------------
+class RobustData:
+    """Mixin over an oracle Stage-I solver: the data rows wd psi(e) and their Jacobian rows times psi'(e).
+
+    The oracle writes a data row as wd (obs - sim) = -wd e; psi is odd and psi' even, so wd psi(obs - sim) is the product's row
+    up to its sign, and the objective is the same.  Where the data rows sit: first in ``StageISolver.residual`` (also under
+    ``ReferenceOptions``, whose rows follow the solver's) and in ``rigid_residual`` (weight 1); in ``face_residual`` after the
+    rows of the other terms and before the poseF / expr rows of the detailed steps (``StageISolver.residual`` there runs with
+    no observations, so it has no data rows)."""
+    sigma = SIGMA
+
+    def _robust(self, out, want_jac, lo, wd, per_term):
+        nd = 3 * sum(len(i) for i in self.lm_ids)
+        r, J = out if want_jac else (out, None)
+        e = r[lo:lo + nd] / wd
+        r = r.copy()
+        r[lo:lo + nd] = wd * gm_psi(e, self.sigma)
+        if per_term is not None:
+            per_term['data'] = float((r[lo:lo + nd] ** 2).sum())
+        if not want_jac:
+            return r
+        J = J.copy()
+        J[lo:lo + nd] *= gm_dpsi(e, self.sigma)[:, None]
+        return r, J
+
+    def residual(self, x, want_jac, pose_ids, free_betas, wts, detailed, per_term=None):
+        out = super().residual(x, want_jac, pose_ids, free_betas, wts, detailed, per_term)
+        return self._robust(out, want_jac, 0, wts['data'], per_term)
+
+    def face_residual(self, x, want_jac, pose_ids, wts, detailed, per_term=None):
+        out = super().face_residual(x, want_jac, pose_ids, wts, detailed, per_term)
+        rows = len(out[0] if want_jac else out)
+        tail = self.n_frames * (len(self.face_ids) + len(self.expr_ids)) if detailed else 0
+        return self._robust(out, want_jac, rows - tail - 3 * sum(len(i) for i in self.lm_ids), wts['data'], per_term)
+
+    def rigid_residual(self, xr, want_jac):
+        return self._robust(super().rigid_residual(xr, want_jac), want_jac, 0, 1.0, None)
+
+
+class RobustBody(RobustData, oracle.StageISolver):
+    pass
+
+
+class RobustFace(RobustData, FaceOracle):
+    pass
+
+
+class RobustJoint(RobustData, JointOracle):
+    pass
+
+
+class RobustBodyRef(RobustData, ReferenceOptions, oracle.StageISolver):
+    def run(self):
+        # oracle.StageISolver.run refuses the extra rigid adjustment, which ReferenceOptions.rigid_adjust carries out
+        cfg = self.cfg
+        self.cfg = copy.deepcopy(cfg)
+        self.cfg.opt_settings.extra_initial_rigid_adjustment = False
+        try:
+            return super().run()
+        finally:
+            self.cfg = cfg
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# corrupted picked frames
+# ---------------------------------------------------------------------------------------------------------------------
+def dense(frames, labels):
+    obs, vis = np.zeros((len(frames), len(labels), 3)), np.zeros((len(frames), len(labels)), dtype=bool)
+    for f, fr in enumerate(frames):
+        for i, l in enumerate(labels):
+            if l in fr and not np.any(np.isnan(fr[l])):
+                obs[f, i], vis[f, i] = fr[l], True
+    return obs, vis
+
+
+def as_frames(obs, vis, labels):
+    return [{l: obs[f, i].copy() for i, l in enumerate(labels) if vis[f, i]} for f in range(len(obs))]
+
+
+def corrupt_frames(frames, meta, swap, ghost, spikes=()):
+    """The picked frames with ``corrupt`` applied (two labels swapped over ``swap``, a 0.3 m ghost over ``ghost``, 0.1 m
+    spikes), as label dictionaries with the missing labels left out; and which of them moved (frames x labels)."""
+    labels = list(meta['marker_vids'])
+    obs0, vis0 = dense(frames, labels)
+    obs, vis, _ = corrupt(obs0, vis0, swap=swap, ghost=ghost, spikes=list(spikes))
+    return as_frames(obs, vis, labels), np.abs(obs - obs0).max(axis=2) > 0
+
+
+def _emu(frames, cfg, meta, **kw):
+    return product.mosh_stagei(frames, cfg, marker_meta=meta, backend=EmuStageIBackend(), **kw)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# CPU: the oracle against finite differences
+# ---------------------------------------------------------------------------------------------------------------------
+def _fd(f, x0, J, cols, rows, h):
+    """The largest difference to central differences over ``rows`` of each column, relative to that column's largest entry."""
+    worst = 0.0
+    for c in cols:
+        xp, xm = x0.copy(), x0.copy()
+        xp[c] += h
+        xm[c] -= h
+        fd = (f(xp) - f(xm)) / (2 * h)
+        assert np.abs(J[rows, c]).max() > 0, c
+        worst = max(worst, np.abs(fd[rows] - J[rows, c]).max() / np.abs(J[rows, c]).max())
+    return worst
+
+
+def test_oracle_robust_jacobian_equals_finite_differences(cases, tmp_path):
+    """The robust data rows of an annealing step wrt the shape, the latent markers and the frames (a swapped label in frame
+    1, a ghost marker in frame 2), and the robust rows of the extra rigid adjustment wrt every frame's translation and root
+    orientation."""
+    case, cfg, frames = stagei_case(cases, 'C2', 3, frames=40, n_verts=1500, dropout=0.0)
+    meta = case['marker_meta']
+    frames, moved = corrupt_frames(frames, meta, swap=slice(1, 2), ghost=slice(2, 3))
+    cfg.opt_settings.extra_initial_rigid_adjustment = True
+    s = RobustBodyRef(frames, cfg, meta)
+    oracle.StageISolver.rigid_adjust(s)
+    wts = s.weights_for(0.5)
+    pose_ids = s.pose_ids_for(True)
+    rng = np.random.default_rng(0)
+    x0 = s.get_x(pose_ids, True)
+    nb, M = s.nb, s.n_markers
+    ids = np.arange(len(x0))
+    x0 = x0 + rng.normal(0, 0.02, x0.shape) * (ids >= nb + 3 * M) + rng.normal(0, 0.3, x0.shape) * (ids < nb)
+    r, J = s.residual(x0, True, pose_ids, True, wts, True)
+    nd = 3 * sum(len(i) for i in s.lm_ids)
+    e = oracle.StageISolver.residual(s, x0, False, pose_ids, True, wts, True)[:nd] / wts['data']       # (least squares: -e)
+    dpsi = gm_dpsi(e, SIGMA)
+    # rows of the corrupted labels (swapped in frame 1, the ghost in frame 2): psi' far below 1
+    off = np.cumsum([0] + [3 * len(i) for i in s.lm_ids])
+    bad = np.concatenate([off[f] + 3 * np.flatnonzero(moved[f, s.lm_ids[f]])[:, None] + np.arange(3) for f in range(s.n_frames)]).ravel()
+    assert moved[1].sum() == 2 and moved[2].sum() == 1 and len(bad) == 9
+    moved = np.flatnonzero(moved.any(0))
+    assert dpsi[bad].min() < 0.05 and dpsi.max() > 0.9            # saturated and unsaturated rows
+    per = 3 + len(pose_ids)
+    f1 = nb + 3 * M + per
+    cols = [nb + 3 * i + c for i in moved for c in (0, 2)] + [f1, f1 + 4, f1 + per + 1, f1 + per + 5, nb + 3 * M + 2]
+    res = lambda x: s.residual(x, False, pose_ids, True, wts, True)      # noqa: E731
+    # (the shape columns with a longer step: their differences lose more to rounding, as in the least-squares rows)
+    assert _fd(res, x0, J, [0, nb - 1], np.arange(nd), 2e-5) < 5e-8
+    assert _fd(res, x0, J, cols, np.arange(nd), 1e-6) < 5e-8
+    assert _fd(res, x0, J, cols[:6], bad, 1e-6) < 5e-8
+
+    xr = s.get_x(np.arange(3), False)[3 * M:] + rng.normal(0, 0.02, 6 * s.n_frames)
+    r, J = s.rigid_residual(xr, True)
+    assert product.data_dpsi_gm(r[bad], 1.0, SIGMA).min() < 0.05
+    assert _fd(lambda x: s.rigid_residual(x, False), xr, J, [0, 2, 3, 5, 6 + 4, 12 + 1], np.arange(nd), 1e-6) < 5e-8
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# CPU: the product on the host build of the device source against the oracle
+# ---------------------------------------------------------------------------------------------------------------------
+def test_free_shape_on_device_source_equals_oracle(cases):
+    """1. C2 (SMPL-H, free shape, the pose prior, fingers): a label swap in frame 1, a ghost marker and a spike in frame 2."""
+    case, cfg, frames = stagei_case(cases, 'C2', 4, frames=40, n_verts=1500, dropout=0.02)
+    cfg.opt_settings.maxiter = 6
+    meta = case['marker_meta']
+    frames, _ = corrupt_frames(frames, meta, swap=slice(1, 2), ghost=slice(2, 3), spikes=[2])
+    ref = oracle_result(RobustBody(frames, cfg, meta))
+    out = _emu(frames, cfg, meta, robust_data_sigma=SIGMA)
+    _compare_body(out, ref, 1e-9)
+    _check_stats(out, ref, 4)
+    assert out['stagei_debug_details']['b200']['robust_data_sigma'] == SIGMA
+
+
+def test_face_given_shape_on_device_source_equals_oracle(cases, tmp_path):
+    """2. CF (SMPL-X with face markers, the shape given): a label swap in frame 1, a ghost marker in frame 3."""
+    case, cfg, frames, fn = face_case(cases, tmp_path)
+    cfg.opt_settings.maxiter = 6
+    meta = case['marker_meta']
+    frames, _ = corrupt_frames(frames, meta, swap=slice(1, 2), ghost=slice(3, 4))
+    ref = oracle_result(RobustFace(frames, cfg, meta, np.load(fn)['betas']))
+    out = _emu(frames, cfg, meta, betas_fname=fn, robust_data_sigma=SIGMA)
+    _compare_face(out, ref, 1e-9)
+    _check_stats(out, ref, 4)
+
+
+def test_face_with_free_shape_on_device_source_equals_oracle(cases):
+    """3. CF with a free shape and the face (face_with_free_shape): a label swap in frame 1, a ghost and a spike in frame 2."""
+    case, cfg, frames = stagei_case(cases, 'CF', 4, frames=40, dropout=0.02)
+    cfg.opt_settings.maxiter = 6
+    meta = case['marker_meta']
+    frames, _ = corrupt_frames(frames, meta, swap=slice(1, 2), ghost=slice(2, 3), spikes=[2])
+    ref = oracle_result(RobustJoint(frames, cfg, meta))
+    out = _emu(frames, cfg, meta, face_with_free_shape=True, robust_data_sigma=SIGMA)
+    _compare_face(out, ref, 1e-9)
+    _check_stats(out, ref, 4)
+
+
+def test_reference_options_on_device_source_equal_oracle(cases, tmp_path):
+    """4. C2 with reference_options: the extra rigid adjustment (robust rows, weight 1) and the head-marker correlation prior."""
+    case, cfg, frames = stagei_case(cases, 'C2', 4, frames=40, n_verts=1500, dropout=0.02)
+    cfg.opt_settings.maxiter = 6
+    cfg.opt_settings.extra_initial_rigid_adjustment = True
+    cfg.moshpp.head_marker_corr_fname = write_corr(str(tmp_path / 'head_corr.npz'), HEAD)
+    meta = case['marker_meta']
+    frames, _ = corrupt_frames(frames, meta, swap=slice(2, 3), ghost=slice(1, 2))
+    ref = oracle_result(RobustBodyRef(frames, cfg, meta))
+    out = _emu(frames, cfg, meta, reference_options=True, robust_data_sigma=SIGMA)
+    _compare_body(out, ref, 1e-9)
+    _check_stats(out, ref, 5)
+    assert out['stagei_debug_details']['stagei_errs']['init_head_corr'] > 0
+
+
+def test_rigid_adjustment_rows_are_robust(cases, tmp_path):
+    """The extra rigid adjustment's SSE and normal equations on the device source against the oracle's robust rows (weight 1)."""
+    case, cfg, frames = stagei_case(cases, 'C2', 3, frames=40, n_verts=1500, dropout=0.02)
+    meta = case['marker_meta']
+    frames, _ = corrupt_frames(frames, meta, swap=slice(1, 2), ghost=slice(2, 3))
+    cfg.opt_settings.extra_initial_rigid_adjustment = True
+    s = product.StageI(frames, cfg, meta, backend=EmuStageIBackend(), reference_options=True, robust_data_sigma=SIGMA)
+    o = RobustBodyRef(frames, cfg, meta)
+    oracle.StageISolver.rigid_adjust(o)
+    s.pose[:], s.trans[:] = o.pose, o.trans
+    A, g = s.evaluate_rigid(True)
+    r, J = o.rigid_residual(o.get_x(np.arange(3), False)[3 * o.n_markers:], True)
+    assert abs(s._last_total - (r ** 2).sum()) <= 1e-10 * (r ** 2).sum()
+    assert np.abs(A - J.T.dot(J)).max() <= 1e-9 * np.abs(A).max()
+    assert np.abs(g + J.T.dot(r)).max() <= 1e-9 * np.abs(g).max()       # g = -J^T r (the oracle's rows and J: the sign of both flipped)
+    plain = product.StageI(frames, cfg, meta, backend=EmuStageIBackend(), reference_options=True)
+    plain.pose[:], plain.trans[:] = o.pose, o.trans
+    assert plain.evaluate_rigid(False) > 10 * s._last_total
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# CPU: the keyword
+# ---------------------------------------------------------------------------------------------------------------------
+def test_sigma_none_is_the_least_squares_result_bit_for_bit(cases):
+    case, cfg, frames = stagei_case(cases, 'C2', 3, frames=40, n_verts=1500, dropout=0.02)
+    cfg.opt_settings.maxiter = 3
+    meta = case['marker_meta']
+    frames, _ = corrupt_frames(frames, meta, swap=slice(1, 2), ghost=slice(2, 3))
+    a = _emu(frames, cfg, meta, robust_data_sigma=None)
+    b = _emu(frames, cfg, meta)
+    _assert_bit_identical(a, b)
+    assert pickle.dumps(a) == pickle.dumps(b)
+    assert 'robust_data_sigma' not in a['stagei_debug_details']['b200']
+    c = _emu(frames, cfg, meta, robust_data_sigma=SIGMA)
+    assert set(c['stagei_debug_details']['b200']) == set(b['stagei_debug_details']['b200']) | {'robust_data_sigma'}
+    assert np.abs(c['markers_latent'] - b['markers_latent']).max() > 1e-4
+
+
+@pytest.mark.parametrize('sigma', [0.0, -0.01, float('nan'), float('inf')])
+def test_bad_sigma_raises(cases, sigma):
+    case, cfg, frames = stagei_case(cases, 'C2', 3, frames=40, n_verts=1500, dropout=0.02)
+    with pytest.raises(ValueError, match='robust_data_sigma'):
+        product.mosh_stagei(frames, cfg, marker_meta=case['marker_meta'], backend=EmuStageIBackend(), robust_data_sigma=sigma)
+    with pytest.raises(ValueError, match='robust_data_sigma'):
+        product.StageI(frames, cfg, case['marker_meta'], backend=EmuStageIBackend(), robust_data_sigma=sigma)
+
+
+def test_dpsi_recovered_from_the_rows_is_the_closed_form():
+    """The host's psi' from the stored rows (the kernel's rule) against psi'(e) of the closed form; 0 on a zero row."""
+    wd, e = 7.5, np.r_[np.linspace(-0.6, 0.6, 241), 0.0, 1e-9]
+    got = product.data_dpsi_gm(wd * gm_psi(e, SIGMA), wd, SIGMA)
+    assert np.abs(got - gm_dpsi(e, SIGMA)).max() < 1e-12 and got[-2] == 0.0
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# CPU: recovery from corrupted picked frames, and Stage II downstream
+# ---------------------------------------------------------------------------------------------------------------------
+@pytest.fixture(scope='module')
+def recovery(cases):
+    """Stage I of a C2 subject on 12 frames picked from its 160-frame capture: least squares and robust, on the clean frames
+    and on the same frames with two labels swapped in frames 3 and 4 and a 0.3 m ghost replacing a label in frame 8."""
+    case, cfg, frames = stagei_case(cases, 'C2', 12, frames=160)
+    meta = case['marker_meta']
+    clean = as_frames(*dense(frames, list(meta['marker_vids'])), list(meta['marker_vids']))
+    bad, moved = corrupt_frames(frames, meta, swap=slice(3, 5), ghost=slice(8, 9))
+    out = dict(case=case, moved=moved)
+    for key, fr, sigma in (('l2_clean', clean, None), ('rb_clean', clean, SIGMA), ('l2_bad', bad, None), ('rb_bad', bad, SIGMA)):
+        out[key] = _emu(fr, cfg, meta, robust_data_sigma=sigma)
+    return out
+
+
+def _shape_errors(res, ref, nb):
+    """Largest latent-marker distance (mm) and largest shape-coefficient difference from ``ref``."""
+    dml = 1e3 * np.linalg.norm(res['markers_latent'] - ref['markers_latent'], axis=1).max()
+    return dml, np.abs(res['betas'][:nb] - ref['betas'][:nb]).max()
+
+
+def test_robust_stagei_recovers_the_clean_shape_and_latent_markers(recovery):
+    """Errors against the least-squares Stage I on the clean frames (the synthetic ground truth is itself recovered only
+    loosely).  Measured on the first run: the worst latent marker lands 48.5 mm (least squares) against 2.32 mm (robust) from
+    the clean solve, the worst shape coefficient 0.831 against 0.0385 (ratios 0.048 and 0.046).  On the clean frames the robust
+    and least-squares solves differ by 6.11 mm and 0.053 (the robust term weighs down the few rows the model fits worst, and
+    moves the latent markers along directions the frames pin down weakly).  The bounds below (1/10 of the least-squares
+    error; 10 mm and 0.1 on clean frames) are set from that run."""
+    nb = recovery['case']['cfg'].surface_model.num_betas
+    ref = recovery['l2_clean']
+    ml_l2, b_l2 = _shape_errors(recovery['l2_bad'], ref, nb)
+    ml_rb, b_rb = _shape_errors(recovery['rb_bad'], ref, nb)
+    ml_cl, b_cl = _shape_errors(recovery['rb_clean'], ref, nb)
+    print(f'\nlatent markers from the clean solve: L2 {ml_l2:.3g} mm, robust {ml_rb:.3g} mm; betas: L2 {b_l2:.3g}, robust {b_rb:.3g}; '
+          f'clean frames robust vs L2: {ml_cl:.3g} mm, {b_cl:.3g}')
+    assert ml_rb <= 0.1 * ml_l2 and b_rb <= 0.1 * b_l2
+    assert ml_cl < 10.0 and b_cl < 0.1
+    e = recovery['rb_bad']['stagei_debug_details']['stagei_errs']['data']
+    assert e < recovery['l2_bad']['stagei_debug_details']['stagei_errs']['data']
+
+
+def _stageii(handle, case, si):
+    """Least-squares Stage II (float64, the sequential pass, host build) of the case's clean capture with a Stage-I result."""
+    pk, opts, _ = chmosh.prepare_stageii(case['cfg'], si['markers_latent'], si['latent_labels'], si['betas'], si['marker_meta'])
+    obs, vis = dense_obs(case)
+    h = lib.DescHolder(pk)
+    res = lib.ResultArrays(len(obs), lib.pack_dims(pk))
+    o = np.ascontiguousarray(obs, dtype=np.float64)
+    v8 = np.ascontiguousarray(vis, dtype=np.uint8)
+    rc = handle.mosh2_emu_solve(C.byref(h.desc), C.byref(opts), len(obs), o.ctypes.data_as(lib._f64p), v8.ctypes.data_as(lib._u8p),
+                                C.byref(lib.make_schedule(0, 0)), lib.MOSH2_F64, C.byref(res.c))
+    assert rc == 0 and (res.status & lib.ST_SOLVED).all()
+    err = np.where(vis, np.linalg.norm(res.markers_sim - obs, axis=-1), 0.0)
+    return res, 1e3 * np.sqrt((err ** 2).sum(1) / vis.sum(1))            # per-frame RMS marker residual (mm)
+
+
+def test_robust_stagei_keeps_stageii_close_to_the_clean_one(recovery):
+    """Stage II (least squares) of the clean 160-frame capture with the clean, the corrupted least-squares and the corrupted
+    robust Stage I.  Measured on the first run: the mean per-frame RMS marker residual is 1.95 mm with the clean Stage I, 7.81 mm
+    with the corrupted least-squares one and 1.96 mm with the corrupted robust one; the worst body-pose difference from the
+    clean Stage I's solve is 0.603 rad (least squares) against 0.0463 rad (robust).  Bounds, set from that run: the robust
+    Stage I's residual within 1/20 and its pose within 0.15 of the least-squares Stage I's distance from the clean one."""
+    handle = C.CDLL(build.build_emu())
+    case = recovery['case']
+    ref, rms_ref = _stageii(handle, case, recovery['l2_clean'])
+    l2, rms_l2 = _stageii(handle, case, recovery['l2_bad'])
+    rb, rms_rb = _stageii(handle, case, recovery['rb_bad'])
+    bd = min(case['pack'].body_dof, 63)
+    dp_l2, dp_rb = np.abs(l2.pose[:, :bd] - ref.pose[:, :bd]).max(), np.abs(rb.pose[:, :bd] - ref.pose[:, :bd]).max()
+    print(f'\nmean RMS marker residual: clean {rms_ref.mean():.3g} mm, L2 {rms_l2.mean():.3g} mm, robust {rms_rb.mean():.3g} mm; '
+          f'worst body pose from the clean Stage I: L2 {dp_l2:.3g} rad, robust {dp_rb:.3g} rad')
+    assert abs(rms_rb.mean() - rms_ref.mean()) <= 0.05 * abs(rms_l2.mean() - rms_ref.mean())
+    assert dp_rb <= 0.15 * dp_l2
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the head: both stages robust through functools.partial
+# ---------------------------------------------------------------------------------------------------------------------
+def _head_setup(root):
+    from moshpp_b200 import synth
+    session = os.path.join(root, 'mocap', 'Synth DS', 'subject 01')
+    os.makedirs(session)
+    case = synth.make_case(os.path.join(root, 'models'), 'C2', frames=10, n_verts=1500)
+    cap = os.path.join(session, 'take_00.npz')
+    shutil.move(case['mocap_fname'], cap)
+    with open(os.path.join(session, 'settings.json'), 'w') as f:
+        json.dump({'gender': 'male'}, f)
+    sm = case['cfg'].surface_model
+    cfg = {'mocap.fname': cap, 'dirs.work_base_dir': os.path.join(root, 'work'), 'dirs.support_base_dir': os.path.join(root, 'support'),
+           'surface_model.type': 'smplh', 'surface_model.fname': sm.fname,
+           'moshpp.pose_body_prior_fname': case['cfg'].moshpp.pose_body_prior_fname,
+           'moshpp.pose_hand_prior_fname': case['cfg'].moshpp.pose_hand_prior_fname, 'moshpp.optimize_fingers': True,
+           'moshpp.stagei_frame_picker.num_frames': 4, 'moshpp.stagei_frame_picker.least_avail_markers': 0.8,
+           'opt_settings.maxiter': 3, 'moshpp.head_marker_corr_fname': None}
+    layout = os.path.join(root, 'work', 'SynthDS', 'SynthDS_smplh.json')
+    os.makedirs(os.path.dirname(layout))
+    product.write_marker_layout(layout, case['marker_meta'])
+    return cfg
+
+
+def test_head_with_robust_stagei(tmp_path):
+    """run_moshpp_once with Stage I bound to the robust data term: its pickle records sigma, and Stage II (here the float64
+    oracle) runs on it."""
+    from moshpp_b200 import mosh_head
+    from oracle import stageii as oracle_stageii
+
+    def stageii(mocap_fname, cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname=None):
+        out = oracle_stageii.mosh_stageii(mocap_fname, cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname)
+        out.pop('_pose_reduced')
+        out['stageii_debug_details'].pop('oracle_stats')
+        return out
+    cfg = _head_setup(str(tmp_path))
+    np.random.seed(0)
+    mp = mosh_head.run_moshpp_once(cfg, stagei_func=functools.partial(product.mosh_stagei, backend=EmuStageIBackend(),
+                                                                      robust_data_sigma=SIGMA), stageii_func=stageii)
+    with open(mp.stagei_fname, 'rb') as f:
+        s1 = pickle.load(f)
+    assert s1['stagei_debug_details']['b200']['robust_data_sigma'] == SIGMA
+    with open(mp.stageii_fname, 'rb') as f:
+        s2 = pickle.load(f)
+    assert np.isfinite(s2['fullpose']).all() and len(s2['fullpose']) == 10
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the CUDA path
+# ---------------------------------------------------------------------------------------------------------------------
+class DeviceLinearisation(product.DeviceBackend):
+    """The CUDA linearisation with the oracle's point-to-mesh distances (those of the host-build back end)."""
+    squared_distance = EmuStageIBackend.squared_distance
+
+
+def _corrupted_c2(cases):
+    case, cfg, frames = stagei_case(cases, 'C2', 4, frames=40, n_verts=1500, dropout=0.02)
+    frames, _ = corrupt_frames(frames, case['marker_meta'], swap=slice(1, 2), ghost=slice(2, 3), spikes=[2])
+    return case, cfg, frames
+
+
+@pytest.mark.gpu
+def test_gpu_linearisation_returns_the_robust_rows(cases):
+    """One detailed-step linearisation of corrupted C2 frames with a free shape: the CUDA rows, Jacobian, private blocks and
+    SSE equal the host build's, and the Jacobian is the least-squares one times the psi' recovered from the rows."""
+    case, cfg, frames = _corrupted_c2(cases)
+    meta = case['marker_meta']
+    emu = product.StageI(frames, cfg, meta, backend=EmuStageIBackend(), robust_data_sigma=SIGMA)
+    _, _, dev = emu.evaluate(False, emu.weights_for(1.0), False)
+    for f in range(emu.F):
+        v = emu.vis[f]
+        emu.pose[f, :3], emu.trans[f] = product.rigid_fit(dev['markers_sim'][f][v], emu.obs[f][v])
+    emu.pose[:, 3:66] += np.random.default_rng(4).normal(0, 0.05, (emu.F, 63))
+    got = {}
+    for name, be, sigma in (('emu', EmuStageIBackend(), SIGMA), ('gpu', DeviceLinearisation(), SIGMA), ('l2', DeviceLinearisation(), None)):
+        s = product.StageI(frames, cfg, meta, backend=be, robust_data_sigma=sigma)
+        s.pose[:], s.trans[:] = emu.pose, emu.trans
+        got[name] = s.evaluate(True, s.weights_for(0.25), True)
+    e, g, l2 = (got[k][2] for k in ('emu', 'gpu', 'l2'))
+    for k in ('r', 'J', 'A', 'g', 'errs'):
+        assert np.abs(g[k] - e[k]).max() <= 1e-10 * np.abs(e[k]).max(), k
+    for i in (3, 4):                                    # the whole normal equations, the host's attachment columns included
+        assert np.abs(got['gpu'][i] - got['emu'][i]).max() <= 1e-10 * np.abs(got['emu'][i]).max()
+    wd = emu.weights_for(0.25)['data']
+    dpsi = product.data_dpsi_gm(g['r'], wd, SIGMA)
+    assert dpsi.min() < 0.05 and dpsi.max() > 0.9
+    assert np.abs(g['J'] - l2['J'] * dpsi[..., None]).max() <= 1e-10 * np.abs(l2['J']).max()
+
+
+@pytest.mark.gpu
+def test_free_shape_on_the_gpu_equals_oracle(cases):
+    """C2 with a free shape on corrupted frames, through the CUDA linearisation.  With the oracle's point-to-mesh distances the
+    CUDA path equals the oracle as closely as the host build does, with the same counts.  With the CUDA distances (a float32
+    closest-part search) the whole path lands further off, measured 4.4e-6 in the shape on an H100."""
+    case, cfg, frames = _corrupted_c2(cases)
+    cfg.opt_settings.maxiter = 12
+    meta = case['marker_meta']
+    ref = oracle_result(RobustBody(frames, cfg, meta))
+    out = product.mosh_stagei(frames, cfg, marker_meta=meta, backend=DeviceLinearisation(), robust_data_sigma=SIGMA)
+    _compare_body(out, ref, 1e-9)
+    _check_stats(out, ref, 4)
+    full = product.mosh_stagei(frames, cfg, marker_meta=meta, robust_data_sigma=SIGMA)
+    print(f'\nCUDA path against the robust oracle: betas {np.abs(full["betas"] - ref["betas"]).max():.3g}, latent markers '
+          f'{np.abs(full["markers_latent"] - ref["markers_latent"]).max():.3g} m, counts {full["stagei_debug_details"]["b200"]}')
+    _compare_body(full, ref, 2e-5)
+    assert full['stagei_debug_details']['b200']['robust_data_sigma'] == SIGMA
+
+
+@pytest.mark.gpu
+def test_face_with_free_shape_on_the_gpu_equals_oracle(cases):
+    case, cfg, frames = stagei_case(cases, 'CF', 4, frames=40, dropout=0.02)
+    cfg.opt_settings.maxiter = 12
+    meta = case['marker_meta']
+    frames, _ = corrupt_frames(frames, meta, swap=slice(1, 2), ghost=slice(2, 3), spikes=[2])
+    ref = oracle_result(RobustJoint(frames, cfg, meta))
+    out = product.mosh_stagei(frames, cfg, marker_meta=meta, face_with_free_shape=True, robust_data_sigma=SIGMA)
+    _compare_face(out, ref, 1e-6)
+
+
+@pytest.mark.gpu
+def test_head_with_both_stages_robust_on_the_gpu(tmp_path):
+    """run_moshpp_once with Stage I and Stage II bound to the robust data term: both pickles record sigma, and Stage II runs
+    on the robust Stage I's shape and latent markers."""
+    from moshpp_b200 import mosh_head
+    cfg = _head_setup(str(tmp_path))
+    np.random.seed(0)
+    mp = mosh_head.run_moshpp_once(cfg, stagei_func=functools.partial(product.mosh_stagei, robust_data_sigma=SIGMA),
+                                   stageii_func=functools.partial(chmosh.mosh_stageii, robust_data_sigma=SIGMA))
+    with open(mp.stagei_fname, 'rb') as f:
+        s1 = pickle.load(f)
+    with open(mp.stageii_fname, 'rb') as f:
+        s2 = pickle.load(f)
+    assert s1['stagei_debug_details']['b200']['robust_data_sigma'] == SIGMA
+    assert s2['stageii_debug_details']['b200']['robust_data_sigma'] == SIGMA
+    assert len(s2['fullpose']) == 10 and np.isfinite(s2['fullpose']).all() and np.isfinite(s2['trans']).all()

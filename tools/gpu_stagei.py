@@ -4,7 +4,9 @@ coefficients -- through moshpp_b200.stagei.mosh_stagei; with --oracle also the f
 jaw and expressions fitted together (face_with_free_shape).
 --reference-options: with the head-marker correlation prior (a synthetic K x H file over the LFHD / RFHD / LBHD / RBHD
 markers) and the extra initial rigid adjustment, both through reference_options=True.
-Usage: python tools/gpu_stagei.py [--oracle] [--frames 12] [--face80] [--reference-options]"""
+--robust-data-sigma S: the Geman-McClure data term at sigma = S metres (robust_data_sigma); with --oracle the oracle is the
+robust one of tests/test_stagei_robust.py.
+Usage: python tools/gpu_stagei.py [--oracle] [--frames 12] [--face80] [--reference-options] [--robust-data-sigma S]"""
 import argparse
 import copy
 import json
@@ -28,6 +30,7 @@ def main():
     ap.add_argument('--config', default='C5')
     ap.add_argument('--face80', action='store_true')
     ap.add_argument('--reference-options', action='store_true')
+    ap.add_argument('--robust-data-sigma', type=float, default=None)
     a = ap.parse_args()
     d = tempfile.mkdtemp(prefix='mosh_stagei_')
     if a.face80:
@@ -44,6 +47,8 @@ def main():
         np.savez(cfg.moshpp.head_marker_corr_fname, mrk_labels=np.asarray(head), corr=corr)
         cfg.opt_settings.extra_initial_rigid_adjustment = True
         kw['reference_options'] = True
+    if a.robust_data_sigma is not None:
+        kw['robust_data_sigma'] = a.robust_data_sigma
     mocap = MocapSession(case['mocap_fname'], cfg.mocap.unit)
     frames = mocap.markers_asdict()
     pick = np.linspace(0, len(frames) - 1, a.frames).astype(int)
@@ -62,10 +67,18 @@ def main():
         line['workload'] += ', face: jaw + 80 expressions per frame, shape free'
     if a.reference_options:
         line['workload'] += ', head-marker correlation prior + extra initial rigid adjustment'
+    if a.robust_data_sigma is not None:
+        line['workload'] += f', Geman-McClure data term at sigma = {a.robust_data_sigma} m'
     if a.oracle and not (a.face80 or a.reference_options):
         from oracle import stagei as ostagei
         t0 = time.perf_counter()
-        ref = ostagei.mosh_stagei(frames, cfg, marker_meta=case['marker_meta'])
+        if a.robust_data_sigma is None:
+            ref = ostagei.mosh_stagei(frames, cfg, marker_meta=case['marker_meta'])
+        else:
+            sys.path.insert(0, os.path.join(ROOT, 'tests'))
+            from test_stagei_reference_options import oracle_result
+            from test_stagei_robust import RobustBody
+            ref = oracle_result(type('RobustAt', (RobustBody,), {'sigma': a.robust_data_sigma})(frames, cfg, case['marker_meta']))
         line['oracle_seconds'] = time.perf_counter() - t0
         line['oracle_stats'] = ref['stagei_debug_details']['oracle_stats']
         line['d_betas'] = float(np.abs(out['betas'] - ref['betas']).max())
