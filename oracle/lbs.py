@@ -54,7 +54,7 @@ class OracleModel:
             hc = dd['hands_components']
             self.hands_mean = np.zeros(hc.shape[1]) if use_hands_mean else dd['hands_mean']   # sic (line 114)
             self.selected_components = np.vstack((hc[:dof_per_hand]))
-        else:
+        else:                           # smpl and the animal models (animal_horse, animal_dog): an LBS body without hands
             self.body_dof = njoint_parms + 3
             self.selected_components = np.zeros((0, 0))
             self.hands_mean = np.zeros(0)

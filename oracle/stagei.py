@@ -18,8 +18,17 @@ constants of an evaluation).
 Built on lbs.py / markers.py / prior.py / rigid.py / dogleg.py / mesh_distance.py.  What cannot be pinned here, on top of
 chumpy's dog-leg and psbody.smpl's LBS (oracle/__init__.py): psbody.mesh's ``estimate_vertex_normals`` and AABB-tree
 nearest-part query (restated as area-weighted vertex normals and a brute-force closest-point search), and the order in
-which chumpy stacks the residual blocks (irrelevant to J^T J).  optimize_face in Stage I is not restated (the reference
-itself raises NotImplementedError when betas are optimised with it, chmosh.py:285-289).
+which chumpy stacks the residual blocks (irrelevant to J^T J).
+
+The keywords of the product's ``mosh_stagei``, on the one solver:
+  * ``moshpp.optimize_face`` (SMPL-X): every frame's jaw and expressions, free in the two detailed steps with their poseF /
+    expr terms (chmosh.py:136-151,163-170,283-297,322-324,396-401); with a free shape the reference raises (287-291),
+    ``face_with_free_shape=True`` fits the shape and the expressions together;
+  * ``reference_options=True``: the head-marker correlation prior (``init_head_corr``, chmosh.py:252-266,360-373) and the
+    extra initial rigid adjustment (230-232); without it the prior is not applied and the adjustment raises
+    NotImplementedError when the solver runs;
+  * ``robust_data_sigma``: the Geman-McClure data term (robust.py) in the annealing steps and the extra rigid adjustment.
+The dog (``animal_dog``) is a model type like the others: its max-mixture prior and pose ids are prior.py's.
 """
 from __future__ import annotations
 
@@ -32,8 +41,9 @@ from . import mesh_distance as md
 from .dogleg import minimize_dogleg
 from .lbs import LBS, OracleModel
 from .markers import TransformedCoeffs, _N, _skew, nrm, transformed_lms
-from .prior import HORSE_JANGLES_IDS, HORSE_JANGLES_SIGNS, HorsePosePrior, create_gmm_body_prior, horse_joint_angles
+from .prior import DOG_POSE_IDS, HORSE_JANGLES_IDS, HORSE_JANGLES_SIGNS, create_body_prior, horse_joint_angles
 from .rigid import perform_rigid_adjustment
+from .robust import gm_dpsi, gm_psi
 
 NUM_TRAIN_MARKERS = 46   # chmosh.py:100
 
@@ -106,14 +116,17 @@ def signed_surface_distance(samples, verts, faces, vn=None, want_jac=False):
 
 
 class StageISolver:
-    """The chumpy graph of chmosh.py:83-455 as explicit state + residual / Jacobian evaluation."""
+    """The chumpy graph of chmosh.py:83-455 as explicit state + residual / Jacobian evaluation, with the keywords of the
+    product's ``mosh_stagei`` (see ``mosh_stagei`` below)."""
 
-    def __init__(self, stagei_frames: List[Dict[str, np.ndarray]], cfg, marker_meta, betas=None, v_template=None):
+    def __init__(self, stagei_frames: List[Dict[str, np.ndarray]], cfg, marker_meta, betas=None, v_template=None, *,
+                 face_with_free_shape=False, reference_options=False, robust_data_sigma=None):
         sm, mp = cfg.surface_model, cfg.moshpp
         self.cfg = cfg
         self.marker_meta = marker_meta
         self.latent_labels = list(marker_meta['marker_vids'].keys())
         M = self.n_markers = len(self.latent_labels)
+        F = self.n_frames = len(stagei_frames)
         avail_labels = set(k for fr in stagei_frames for k in fr.keys())
         self.optimize_fingers = bool(mp.optimize_fingers)
         if self.optimize_fingers:                                                               # chmosh.py:130-141
@@ -121,22 +134,45 @@ class StageISolver:
                 self.optimize_fingers = False
             elif not np.any([('finger' in t) and l in avail_labels for l, t in marker_meta['marker_type'].items()]):
                 self.optimize_fingers = False
+        self.optimize_betas = bool(mp.optimize_betas)
+        # optimize_face: off with a free shape when the face markers are excluded (chmosh.py:103-118), off without a face-type
+        # marker in the layout or a face label in the frames (127-137); only SMPL-X has a jaw and expression components; with a
+        # free shape the reference raises when it runs (287-291), face_with_free_shape fits the shape and the expressions together
+        self.face = bool(mp.get('optimize_face', False)) and sm.type == 'smplx'
+        if self.face and self.optimize_betas and 'face' in (cfg.mocap.get('exclude_marker_types') or []):
+            self.face = False
+        if self.face and not np.any(['face' in t for t in marker_meta['marker_type_mask'].keys()]):
+            self.face = False
+        if self.face and not np.any([('face' in t) and l in avail_labels for l, t in marker_meta['marker_type'].items()]):
+            self.face = False
+        self.face_with_free_shape = face_with_free_shape
+        # every frame's model: the shape plus the frame's expressions at betas[betas_expr_start_id:][:num_expressions]; the
+        # canonical body keeps zero expressions
+        self.face_ids = [66, 67, 68] if self.face else []                                       # the jaw (line 293)
+        es = int(sm.betas_expr_start_id) if self.face else 0
+        self.expr_ids = np.arange(es, es + (int(sm.num_expressions) if self.face else 0))
+        self.expr = np.zeros((F, len(self.expr_ids)))
+        self.robust_sigma = robust_data_sigma           # None: the reference's least-squares data term
+        # reference_options: the head-marker correlation prior (chmosh.py:252-266; corr_ids / corr stay None when it does not
+        # apply) and the extra rigid adjustment (230-232, in run)
+        self.reference_options = reference_options
+        self.corr_ids, self.corr = None, None
+        corr_fname = mp.get('head_marker_corr_fname') if reference_options else None
+        if corr_fname is not None:
+            head = np.load(corr_fname)
+            if all(l in marker_meta['marker_vids'] for l in head['mrk_labels']):
+                self.corr_ids = [self.latent_labels.index(l) for l in head['mrk_labels']]
+                self.corr = np.asarray(head['corr'], dtype=np.float64)
         self.model = m = OracleModel(sm.fname, pose_hand_prior_fname=mp.pose_hand_prior_fname, use_hands_mean=sm.use_hands_mean,
                                      dof_per_hand=sm.dof_per_hand, v_template=v_template, surface_model_type=sm.type)
         with open(sm.fname, 'rb') as f:
             import pickle
             self.faces = np.asarray(pickle.load(f, encoding='latin-1')['f'], dtype=np.int64)
-        self.prior = None
-        if mp.pose_body_prior_fname and m.model_type == 'animal_horse':
-            self.prior = HorsePosePrior(mp.pose_body_prior_fname)
-        elif mp.pose_body_prior_fname and m.model_type != 'mano':
-            self.prior = create_gmm_body_prior(mp.pose_body_prior_fname, exclude_hands=m.model_type in ('smplh', 'smplx'))
+        self.prior = create_body_prior(m.model_type, mp.pose_body_prior_fname)
         self.nb = int(sm.num_betas)
-        self.optimize_betas = bool(mp.optimize_betas)
         self.betas = np.zeros(m.n_betas_model)
         if betas is not None:
             self.betas[:self.nb] = np.asarray(betas)[:self.nb]                                  # chmosh.py:169-172
-        F = self.n_frames = len(stagei_frames)
         self.pose = np.zeros((F, m.pose_size))
         self.trans = np.zeros((F, 3))
         self.full_lbs = LBS(m, None)
@@ -162,7 +198,7 @@ class StageISolver:
             self.lm_ids.append(np.asarray([self.latent_labels.index(l) for l in labs], dtype=np.int64))
             self.obs.append(np.vstack([fr[l] for l in labs]))
 
-        all_ids = list(range(m.pose_size))                                                      # chmosh.py:268-305
+        all_ids = list(range(m.pose_size))                                                      # chmosh.py:268-309
         self.root_ids, self.body_ids, self.finger_ids = all_ids[:3], [], []
         if sm.type == 'smpl':
             self.body_ids = all_ids[3:]
@@ -178,6 +214,8 @@ class StageISolver:
             self.finger_ids = all_ids[3:]
         elif sm.type == 'animal_horse':
             self.body_ids = all_ids[3:84]
+        elif sm.type == 'animal_dog':
+            self.body_ids = [all_ids[i] for i in DOG_POSE_IDS]
         else:
             raise NotImplementedError(sm.type)
         self.stats = dict(r_evals=0, j_evals=0, iterations=0, minimizations=0)
@@ -186,20 +224,26 @@ class StageISolver:
     def can_v(self):
         return self.full_lbs(np.zeros(self.model.pose_size), self.betas, np.zeros(3))
 
+    def frame_betas(self, f):
+        b = self.betas.copy()
+        b[self.expr_ids] = self.expr[f]
+        return b
+
     def pose_ids_for(self, detailed: bool):
         ids = self.root_ids + self.body_ids
         if len(self.body_ids) and not self.cfg.moshpp.optimize_toes:
-            ids = list(set(ids).difference(set(range(30, 36))))                                 # chmosh.py:391-392
-        if detailed and self.optimize_fingers:
-            ids = ids + self.finger_ids
+            ids = list(set(ids).difference(set(range(30, 36))))                                 # chmosh.py:389-390
+        if detailed:
+            ids = ids + (self.finger_ids if self.optimize_fingers else []) + self.face_ids      # chmosh.py:392-402
         return np.asarray(sorted(set(ids)), dtype=np.int64)
 
-    def markers_sim_all(self, tc=None, can_v=None):
-        can_v = self.can_v() if can_v is None else can_v
-        tc = TransformedCoeffs(can_v, self.ml) if tc is None else tc
+    def markers_sim_all(self):
+        can_v = self.can_v()
+        tc = TransformedCoeffs(can_v, self.ml)
+        lbs = LBS(self.model, tc.closest[:, :3].reshape(-1))
         out = []
         for f in range(self.n_frames):
-            v = LBS(self.model, tc.closest[:, :3].reshape(-1))(self.pose[f], self.betas, self.trans[f]).reshape(-1, 3, 3)
+            v = lbs(self.pose[f], self.frame_betas(f), self.trans[f]).reshape(-1, 3, 3)
             out.append(transformed_lms(tc, v[:, 0], v[:, 1], v[:, 2]))
         return out
 
@@ -211,50 +255,65 @@ class StageISolver:
             self.pose[f, :3] = rv
             self.trans[f] = T
 
-    # ---- residual vector and Jacobian for one annealing step ---------------------------------------------------
-    def layout(self, pose_ids, free_betas):
-        nb = self.nb if free_betas else 0
-        M, F, npi = self.n_markers, self.n_frames, len(pose_ids)
-        off_ml = nb
-        off_fr = nb + 3 * M
-        return nb, off_ml, off_fr, 3 + npi, off_fr + F * (3 + npi)
+    def rigid_residual(self, xr, want_jac):
+        """The objective of the extra rigid adjustment (chmosh.py:231): the data rows at weight 1 (robust with
+        robust_data_sigma) wrt xr = [trans | pose[:3]] of every frame, the rest fixed."""
+        fr = xr.reshape(self.n_frames, 6)
+        self.trans[:], self.pose[:, :3] = fr[:, :3], fr[:, 3:]
+        pose_ids = np.arange(3)
+        off = self.layout(pose_ids, False)[2]
+        rows = list(self.data_rows(want_jac, pose_ids, False, False, 1.0, self.can_v()))
+        r = np.concatenate([a for a, _ in rows])
+        return (r, np.vstack([J for _, J in rows])[:, off:]) if want_jac else r
 
-    def get_x(self, pose_ids, free_betas):
-        nb, off_ml, off_fr, per, n = self.layout(pose_ids, free_betas)
+    def extra_rigid_adjust(self):
+        """chmosh.py:230-232: one dog-leg over every frame's translation and root orientation."""
+        x0 = np.hstack([self.trans, self.pose[:, :3]]).reshape(-1)
+        xr, st = minimize_dogleg(self.rigid_residual, x0, e_3=1e-3, delta_0=0.5, maxiter=int(self.cfg.opt_settings.maxiter))
+        fr = xr.reshape(self.n_frames, 6)
+        self.trans[:], self.pose[:, :3] = fr[:, :3], fr[:, 3:]
+        self._count(st)
+
+    # ---- residual vector and Jacobian for one annealing step ---------------------------------------------------
+    def layout(self, pose_ids, free_betas, free_expr=False):
+        """The unknowns [betas[:nb] if free_betas | latent markers (3 M) | frame 0 | frame 1 | ...], a frame's block
+        [trans | pose[pose_ids] | expressions if free_expr (the face, detailed steps)]: (nb free, latent-marker offset, frame
+        offset, frame block size, total)."""
+        nb = self.nb if free_betas else 0
+        off_fr = nb + 3 * self.n_markers
+        per = 3 + len(pose_ids) + (len(self.expr_ids) if free_expr else 0)
+        return nb, nb, off_fr, per, off_fr + self.n_frames * per
+
+    def get_x(self, pose_ids, free_betas, free_expr=False):
+        nb, off_ml, off_fr, per, n = self.layout(pose_ids, free_betas, free_expr)
+        npi = len(pose_ids)
         x = np.zeros(n)
         x[:nb] = self.betas[:nb]
         x[off_ml:off_fr] = self.ml.reshape(-1)
-        for f in range(self.n_frames):
-            x[off_fr + f * per:off_fr + f * per + 3] = self.trans[f]
-            x[off_fr + f * per + 3:off_fr + (f + 1) * per] = self.pose[f, pose_ids]
+        fr = x[off_fr:].reshape(self.n_frames, per)
+        fr[:, :3] = self.trans
+        fr[:, 3:3 + npi] = self.pose[:, pose_ids]
+        fr[:, 3 + npi:] = self.expr[:, :per - 3 - npi]
         return x
 
-    def set_x(self, x, pose_ids, free_betas):
-        nb, off_ml, off_fr, per, n = self.layout(pose_ids, free_betas)
+    def set_x(self, x, pose_ids, free_betas, free_expr=False):
+        nb, off_ml, off_fr, per, n = self.layout(pose_ids, free_betas, free_expr)
+        npi = len(pose_ids)
         self.betas[:nb] = x[:nb]
         self.ml = x[off_ml:off_fr].reshape(-1, 3).copy()
-        for f in range(self.n_frames):
-            self.trans[f] = x[off_fr + f * per:off_fr + f * per + 3]
-            self.pose[f, pose_ids] = x[off_fr + f * per + 3:off_fr + (f + 1) * per]
+        fr = x[off_fr:].reshape(self.n_frames, per)
+        self.trans[:] = fr[:, :3]
+        self.pose[:, pose_ids] = fr[:, 3:3 + npi]
+        self.expr[:, :per - 3 - npi] = fr[:, 3 + npi:]
 
-    def residual(self, x, want_jac, pose_ids, free_betas, wts, detailed, per_term=None):
-        self.set_x(x, pose_ids, free_betas)
-        nbf, off_ml, off_fr, per, n = self.layout(pose_ids, free_betas)
-        M, F = self.n_markers, self.n_frames
-        m = self.model
-        can_v = self.can_v()
+    def data_rows(self, want_jac, pose_ids, free_betas, free_expr, wd, can_v):
+        """The data rows of every frame (chmosh.py:202-213,349), (obs - sim) wd or with robust_data_sigma wd psi(obs - sim),
+        each frame posed on its own betas: yields (r, J or None) per frame.  The shape columns come through the frame's model
+        and the marker attachment, the expression columns through the posed vertices only."""
+        nbf, off_ml, off_fr, per, n = self.layout(pose_ids, free_betas, free_expr)
+        M, npi = self.n_markers, len(pose_ids)
         tc = TransformedCoeffs(can_v, self.ml)                  # transformed_lm.py:59-113, re-made on every change
         tri = tc.closest[:, :3]
-        rs, Js = [], []
-
-        def block(name, r, J=None):
-            rs.append(r)
-            if per_term is not None:
-                per_term[name] = per_term.get(name, 0.0) + float((r ** 2).sum())
-            if want_jac:
-                Js.append(J)
-
-        # coefficients and their derivatives
         if want_jac:
             Fcan = np.zeros((M, 3, 3))
             dk_db = np.zeros((M, 3, nbf))
@@ -263,20 +322,25 @@ class StageISolver:
                 if nbf:
                     for t in range(3):
                         dk_db[i] += dk_dv[:, 3 * t:3 * t + 3].dot(self.Sdirs[tri[i, t]][:, :nbf])
-        # ---- data
-        lbs = LBS(m, tri.reshape(-1))
-        for f in range(F):
+        bids = np.concatenate([np.arange(nbf), self.expr_ids[:per - 3 - npi]])
+        lbs = LBS(self.model, tri.reshape(-1))
+        for f in range(self.n_frames):
             ids = self.lm_ids[f]
-            res = lbs(self.pose[f], self.betas, self.trans[f], want_jac, beta_ids=np.arange(nbf))
+            res = lbs(self.pose[f], self.frame_betas(f), self.trans[f], want_jac, beta_ids=bids)
             verts = (res[0] if want_jac else res).reshape(M, 3, 3)
-            if not want_jac:
+            if want_jac:
+                sim, loc = transformed_lms(tc, verts[:, 0], verts[:, 1], verts[:, 2], True)
+            else:
                 sim = transformed_lms(tc, verts[:, 0], verts[:, 1], verts[:, 2])
-                block('data', ((self.obs[f] - sim[ids]) * wts['data']).reshape(-1))
+            e = (self.obs[f] - sim[ids]).reshape(-1)
+            r = wd * e if self.robust_sigma is None else wd * gm_psi(e, self.robust_sigma)
+            if not want_jac:
+                yield r, None
                 continue
-            sim, loc = transformed_lms(tc, verts[:, 0], verts[:, 1], verts[:, 2], True)
             dv_pose = res[1].reshape(M, 3, 3, -1)
             dv_beta = res[2].reshape(M, 3, 3, -1)
             J = np.zeros((len(ids), 3, n))
+            c0 = off_fr + f * per
             for row, i in enumerate(ids):
                 e1, e2 = verts[i, 1] - verts[i, 0], verts[i, 2] - verts[i, 0]
                 f1 = e1 / np.linalg.norm(e1)
@@ -284,16 +348,44 @@ class StageISolver:
                 f2 = nn / np.linalg.norm(nn)
                 Fp = np.stack([f1, f2, np.cross(f1, f2)], axis=1)             # columns: posed frame
                 dpose = sum(loc[i, :, 3 * t:3 * t + 3].dot(dv_pose[i, t]) for t in range(3))
-                c0 = off_fr + f * per
+                db = sum(loc[i, :, 3 * t:3 * t + 3].dot(dv_beta[i, t]) for t in range(3))
                 J[row, :, c0:c0 + 3] = np.eye(3)
-                J[row, :, c0 + 3:c0 + per] = dpose[:, pose_ids]
+                J[row, :, c0 + 3:c0 + 3 + npi] = dpose[:, pose_ids]
+                J[row, :, c0 + 3 + npi:c0 + per] = db[:, nbf:]
                 J[row, :, off_ml + 3 * i:off_ml + 3 * i + 3] = Fp.dot(Fcan[i])
                 if nbf:
-                    J[row, :, :nbf] = sum(loc[i, :, 3 * t:3 * t + 3].dot(dv_beta[i, t]) for t in range(3)) + Fp.dot(dk_db[i])
-            block('data', ((self.obs[f] - sim[ids]) * wts['data']).reshape(-1), -J.reshape(-1, n) * wts['data'])
+                    J[row, :, :nbf] = db[:, :nbf] + Fp.dot(dk_db[i])
+            J = -J.reshape(-1, n) * wd
+            if self.robust_sigma is not None:
+                J *= gm_dpsi(e, self.robust_sigma)[:, None]
+            yield r, J
+
+    def residual(self, x, want_jac, pose_ids, free_betas, wts, detailed, per_term=None, *, free_expr=False, rows=None):
+        """r(x) and, if want_jac, J(x) at the unknowns ``x`` of ``layout``; the poseF / expr terms come with free_expr.
+        ``per_term`` collects every term's SSE, ``rows`` its rows (a slice of r)."""
+        self.set_x(x, pose_ids, free_betas, free_expr)
+        nbf, off_ml, off_fr, per, n = self.layout(pose_ids, free_betas, free_expr)
+        M, F = self.n_markers, self.n_frames
+        m = self.model
+        can_v = self.can_v()
+        rs, Js = [], []
+
+        def block(name, r, J=None):
+            if rows is not None:
+                end = sum(len(a) for a in rs) + len(r)
+                rows[name] = slice(rows[name].start if name in rows else end - len(r), end)
+            rs.append(r)
+            if per_term is not None:
+                per_term[name] = per_term.get(name, 0.0) + float((r ** 2).sum())
+            if want_jac:
+                Js.append(J)
+
+        # ---- data
+        for r, J in self.data_rows(want_jac, pose_ids, free_betas, free_expr, wts['data'], can_v):
+            block('data', r, J)
         # ---- pose prior(s)
+        col = {pid: c for c, pid in enumerate(pose_ids)}
         if len(self.body_ids) and self.prior is not None:
-            col = {pid: c for c, pid in enumerate(pose_ids)}
             for f in range(F):
                 xb = self.pose[f, self.body_ids]
                 r = self.prior.r(xb) * wts['poseB']
@@ -317,24 +409,45 @@ class StageISolver:
                             if pid in col:
                                 J[ri, off_fr + f * per + 3 + col[pid]] = 2.0 * sg * r[ri]
                     block('poseB_jangles', r, J)
-        # ---- init: latent markers against the initial guess riding on the current canonical body
+        # ---- init: latent markers against the initial guess riding on the current canonical body (chmosh.py:360-373); with
+        #      the head-marker correlation prior the types other than 'head' without the correlated markers, then init_head_corr
         t0 = self.tc0.closest[:, :3]
         if want_jac:
             init, loc0 = transformed_lms(self.tc0, can_v[t0[:, 0]], can_v[t0[:, 1]], can_v[t0[:, 2]], True)
         else:
             init = transformed_lms(self.tc0, can_v[t0[:, 0]], can_v[t0[:, 1]], can_v[t0[:, 2]])
+        diff = self.ml - init
+
+        def dinit_db(i):
+            return sum(loc0[i, :, 3 * t:3 * t + 3].dot(self.Sdirs[t0[i, t]][:, :nbf]) for t in range(3))
         for k, mask in self.marker_meta['marker_type_mask'].items():
-            mask = np.asarray(mask, dtype=bool)
-            r = ((self.ml - init)[mask] * wts['init'][k]).reshape(-1)
+            ids = np.flatnonzero(np.asarray(mask, dtype=bool))
+            if self.corr_ids is not None:
+                if k == 'head':
+                    continue
+                ids = np.setdiff1d(ids, self.corr_ids)
+            r = (diff[ids] * wts['init'][k]).reshape(-1)
             J = None
             if want_jac:
-                J = np.zeros((int(mask.sum()), 3, n))
-                for row, i in enumerate(np.nonzero(mask)[0]):
+                J = np.zeros((len(ids), 3, n))
+                for row, i in enumerate(ids):
                     J[row, :, off_ml + 3 * i:off_ml + 3 * i + 3] = np.eye(3)
                     if nbf:
-                        J[row, :, :nbf] = -sum(loc0[i, :, 3 * t:3 * t + 3].dot(self.Sdirs[t0[i, t]][:, :nbf]) for t in range(3))
+                        J[row, :, :nbf] = -dinit_db(i)
                 J = J.reshape(-1, n) * wts['init'][k]
             block(f'init_{k}', r, J)
+        if self.corr_ids is not None:
+            w, C = wts['head_corr'], self.corr
+            J = None
+            if want_jac:
+                J = np.zeros((len(C), 3, n))
+                for j, i in enumerate(self.corr_ids):
+                    for q in range(len(C)):
+                        J[q, :, off_ml + 3 * i:off_ml + 3 * i + 3] += C[q, j] * np.eye(3)
+                        if nbf:
+                            J[q, :, :nbf] -= C[q, j] * dinit_db(i)
+                J = J.reshape(-1, n) * w
+            block('init_head_corr', (C.dot(diff[self.corr_ids]) * w).reshape(-1), J)
         # ---- betas
         if free_betas:
             J = None
@@ -354,9 +467,8 @@ class StageISolver:
             block('surf', (d - self.m2b) * wts['surf'], J * wts['surf'])
         else:
             block('surf', (signed_surface_distance(self.ml, can_v, self.faces) - self.m2b) * wts['surf'])
-        # ---- fingers
+        # ---- fingers, then the jaw and the expressions of every frame (detailed steps)
         if detailed and self.optimize_fingers:
-            col = {pid: c for c, pid in enumerate(pose_ids)}
             for f in range(F):
                 r = self.pose[f, self.finger_ids] * wts['poseH']
                 J = None
@@ -366,6 +478,19 @@ class StageISolver:
                         if pid in col:
                             J[ri, off_fr + f * per + 3 + col[pid]] = wts['poseH']
                 block('poseH', r, J)
+        if free_expr:
+            for name in ('poseF', 'expr'):
+                for f in range(F):
+                    c0 = off_fr + f * per
+                    if name == 'poseF':
+                        r, cols = self.pose[f, self.face_ids] * wts[name], [c0 + 3 + col[p] for p in self.face_ids]
+                    else:
+                        r, cols = self.expr[f] * wts[name], list(range(c0 + 3 + len(pose_ids), c0 + per))
+                    J = None
+                    if want_jac:
+                        J = np.zeros((r.size, n))
+                        J[np.arange(r.size), cols] = wts[name]
+                    block(name, r, J)
         r = np.concatenate(rs)
         if want_jac:
             return r, np.vstack(Js)
@@ -383,45 +508,64 @@ class StageISolver:
             except (KeyError, AttributeError):
                 base = w['stagei_wt_init']
             out['init'][k] = base * anneal
+        if self.face:                                                                           # chmosh.py:322-324
+            out['poseF'], out['expr'] = w['stagei_wt_poseF'] * anneal, w['stagei_wt_expr'] * anneal
+        if self.corr_ids is not None:                                                           # chmosh.py:368-369
+            out['head_corr'] = out['init'].get('body', w['stagei_wt_init'] * anneal)
         return out
+
+    def _count(self, st):
+        self.stats['r_evals'] += st.r_evals
+        self.stats['j_evals'] += st.j_evals
+        self.stats['iterations'] += st.iterations
+        self.stats['minimizations'] += 1
 
     def run(self):
         cfg = self.cfg
+        if self.face and self.optimize_betas and not self.face_with_free_shape:
+            raise NotImplementedError('optimize_face with optimize_betas (chmosh.py:287-291): face_with_free_shape=True')
+        extra_rigid = bool(cfg.opt_settings.get('extra_initial_rigid_adjustment', False))
+        if extra_rigid and not self.reference_options:
+            raise NotImplementedError('extra_initial_rigid_adjustment needs reference_options=True')
         self.rigid_adjust()
+        if extra_rigid:
+            self.extra_rigid_adjust()
         free_betas = self.optimize_betas
-        if cfg.opt_settings.extra_initial_rigid_adjustment:                                    # chmosh.py:230-232
-            raise NotImplementedError('extra_initial_rigid_adjustment is not restated')
         ann = list(cfg.opt_settings.weights['stagei_wt_annealing'])
         errs = {}
         for tidx, a in enumerate(ann):
             detailed = tidx > len(ann) - 3                                                      # chmosh.py:311
             wts = self.weights_for(a)
             pose_ids = self.pose_ids_for(detailed)
+            free_expr = detailed and self.face
+            # (the keyword only where it is set: subclasses may override residual with the arguments before it)
+            kw = {'free_expr': True} if free_expr else {}
 
             def obj(x, want_jac):
-                return self.residual(x, want_jac, pose_ids, free_betas, wts, detailed)
+                return self.residual(x, want_jac, pose_ids, free_betas, wts, detailed, **kw)
 
-            x, st = minimize_dogleg(obj, self.get_x(pose_ids, free_betas), e_3=float(cfg.opt_settings.stagei_lr), delta_0=0.5,
-                                    maxiter=int(cfg.opt_settings.maxiter))
-            self.set_x(x, pose_ids, free_betas)
-            self.stats['r_evals'] += st.r_evals
-            self.stats['j_evals'] += st.j_evals
-            self.stats['iterations'] += st.iterations
-            self.stats['minimizations'] += 1
+            x, st = minimize_dogleg(obj, self.get_x(pose_ids, free_betas, free_expr), e_3=float(cfg.opt_settings.stagei_lr),
+                                    delta_0=0.5, maxiter=int(cfg.opt_settings.maxiter))
+            self.set_x(x, pose_ids, free_betas, free_expr)
+            self._count(st)
             errs = {}
-            self.residual(x, False, pose_ids, free_betas, wts, detailed, per_term=errs)
+            self.residual(x, False, pose_ids, free_betas, wts, detailed, errs, **kw)
         return errs
 
 
-def mosh_stagei(stagei_frames: List[Dict[str, np.ndarray]], cfg, betas_fname=None, v_template_fname=None, *, marker_meta=None) -> dict:
-    """Same inputs and return layout as the reference (chmosh.py:83-85,436-455); ``marker_meta`` is what
-    ``marker_layout_load(cfg.dirs.marker_layout.fname, ...)`` returns (chmosh.py:121-125; layout tooling is out of scope)."""
+def mosh_stagei(stagei_frames: List[Dict[str, np.ndarray]], cfg, betas_fname=None, v_template_fname=None, *, marker_meta=None,
+                face_with_free_shape=False, reference_options=False, robust_data_sigma=None) -> dict:
+    """Same inputs and return layout as the reference (chmosh.py:83-85,436-455), with the keywords of the product's
+    ``mosh_stagei``; ``marker_meta`` is what ``marker_layout_load(cfg.dirs.marker_layout.fname, ...)`` returns
+    (chmosh.py:121-125; layout tooling is out of scope).  With the face fitted the expressions of every picked frame are
+    ``stagei_debug_details['opt_models_expression']``."""
     betas = np.load(betas_fname)['betas'] if betas_fname is not None else None
     v_template = None
     if v_template_fname is not None:
         from moshpp_b200.chmosh import _read_vertices       # host IO helper shared with the product
         v_template = _read_vertices(v_template_fname)
-    s = StageISolver(stagei_frames, cfg, marker_meta, betas=betas, v_template=v_template)
+    s = StageISolver(stagei_frames, cfg, marker_meta, betas=betas, v_template=v_template, face_with_free_shape=face_with_free_shape,
+                     reference_options=reference_options, robust_data_sigma=robust_data_sigma)
     errs = s.run()
     can_v = s.can_v()
     _, closest = NearestNeighbors(algorithm='kd_tree', n_neighbors=1).fit(can_v).kneighbors(s.ml)      # chmosh.py:422-424
@@ -429,5 +573,7 @@ def mosh_stagei(stagei_frames: List[Dict[str, np.ndarray]], cfg, betas_fname=Non
     dbg = {'opt_models_trans': [t.copy() for t in s.trans], 'opt_models_pose': [p.copy() for p in s.pose], 'stagei_errs': errs,
            'stagei_markers_sim_all': sims_all, 'stagei_markers_sim': [sims_all[f][s.lm_ids[f]] for f in range(s.n_frames)],
            'stagei_markers_obs': s.obs, 'stagei_labels_obs': s.labels_obs, 'oracle_stats': dict(s.stats)}
+    if s.face:
+        dbg['opt_models_expression'] = [e.copy() for e in s.expr]
     return {'betas': s.betas.copy(), 'markers_latent': s.ml.copy(), 'latent_labels': s.latent_labels, 'marker_meta': marker_meta,
             'markers_latent_vids': {l: int(c[0]) for l, c in zip(s.latent_labels, closest.tolist())}, 'stagei_debug_details': dbg}

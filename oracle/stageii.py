@@ -18,7 +18,12 @@ full per-frame schedule and the earlier ones with one Step-2 iteration (DESIGN.m
 
 DMPL with SMPL-X is rejected by the reference (chmosh.py:508-509); BASELINE config 3 asks for it, so
 ``allow_smplx_dmpl=True`` lifts the assert and defines it by SURVEY.md Appendix A (extra beta
-columns that also move the joints).  optimize_face is not restated (SURVEY.md 8(f-4)).
+columns that also move the joints).  optimize_face is restated: the jaw joins Step 2 with its poseF term and the expression
+coefficients are free with their expr term (chmosh.py:560-566,685-689).
+
+Model types: the SMPL families, MANO, the horse and the dog (an LBS body without hands, its max-mixture prior over the pose
+ids of chmosh.py:574-579).  ``robust_data_sigma``: the product's Geman-McClure data term (robust.py); None, the default, is
+the reference's least-squares term.
 """
 from __future__ import annotations
 
@@ -31,8 +36,9 @@ import numpy as np
 from .dogleg import minimize_dogleg
 from .lbs import LBS, OracleModel
 from .markers import TransformedCoeffs, transformed_lms
-from .prior import HORSE_JANGLES_IDS, HORSE_JANGLES_SIGNS, HorsePosePrior, create_gmm_body_prior, horse_joint_angles
+from .prior import DOG_POSE_IDS, HORSE_JANGLES_IDS, HORSE_JANGLES_SIGNS, create_body_prior, horse_joint_angles
 from .rigid import perform_rigid_adjustment
+from .robust import gm_dpsi, gm_psi
 
 NUM_TRAIN_MARKERS = 46   # chmosh.py:460
 
@@ -72,7 +78,11 @@ class _Objective:
         for name, payload in self.terms:
             if name == 'data':
                 wt = payload
-                r = ((ev['markers'][self.vis] - self.obs) * wt).reshape(-1)
+                if s.robust_sigma is None:
+                    r = ((ev['markers'][self.vis] - self.obs) * wt).reshape(-1)
+                else:
+                    e = (ev['markers'][self.vis] - self.obs).reshape(-1)
+                    r = wt * gm_psi(e, s.robust_sigma)
                 if want_jac:
                     J = np.zeros((r.size, self.n))
                     dm_pose = ev['dm_pose'][self.vis].reshape(-1, s.model.pose_size)
@@ -80,6 +90,8 @@ class _Objective:
                     J[:, 3:3 + npi] = dm_pose[:, self.pose_ids] * wt
                     if self.free_dmpl:
                         J[:, 3 + npi:] = ev['dm_beta'][self.vis].reshape(-1, s.nd) * wt
+                    if s.robust_sigma is not None:
+                        J *= gm_dpsi(e, s.robust_sigma)[:, None]
             elif name == 'poseB':
                 wt = payload
                 xb = s.pose[s.body_ids]
@@ -163,7 +175,10 @@ class _Objective:
         for name, payload in self.terms:
             s = self.s
             if name == 'data':
-                out[name] = float((((ev['markers'][self.vis] - self.obs) * payload) ** 2).sum())
+                e = ev['markers'][self.vis] - self.obs
+                if s.robust_sigma is not None:
+                    e = gm_psi(e, s.robust_sigma)
+                out[name] = float(((e * payload) ** 2).sum())
             elif name == 'poseB':
                 out[name] = float(((s.prior.r(s.pose[s.body_ids]) * payload) ** 2).sum())
             elif name == 'poseB_jangles':
@@ -187,10 +202,11 @@ class StageIISolver:
     """State of ``opt_model`` + everything chmosh.py:488-579 sets up before the frame loop."""
 
     def __init__(self, cfg, markers_latent, latent_labels, betas, marker_meta, mode='lean',
-                 allow_smplx_dmpl=True):
+                 allow_smplx_dmpl=True, robust_data_sigma=None):
         sm, mp = cfg.surface_model, cfg.moshpp
         self.cfg = cfg
         self.mode = mode
+        self.robust_sigma = robust_data_sigma          # None: the reference's least-squares data term
         self.latent_labels = list(latent_labels)
         self.optimize_fingers = bool(mp.optimize_fingers)
         self.optimize_face = bool(mp.optimize_face)
@@ -210,12 +226,7 @@ class StageIISolver:
                                  surface_model_type=sm.type)
         m = self.model
         assert m.model_type == sm.type
-        self.prior = None
-        if mp.pose_body_prior_fname and m.model_type == 'animal_horse':
-            self.prior = HorsePosePrior(mp.pose_body_prior_fname)                                 # bodymodel_loader.py:121-125
-        elif mp.pose_body_prior_fname and m.model_type != 'mano':
-            self.prior = create_gmm_body_prior(mp.pose_body_prior_fname,
-                                               exclude_hands=m.model_type in ('smplh', 'smplx'))  # bodymodel_loader.py:126-129
+        self.prior = create_body_prior(m.model_type, mp.pose_body_prior_fname)
         self.betas = np.zeros(m.n_betas_model)
         self.betas[:sm.num_betas] = np.asarray(betas)[:sm.num_betas]                            # chmosh.py:499-500
         self.pose = np.zeros(m.pose_size)
@@ -281,6 +292,8 @@ class StageIISolver:
             self.finger_ids = all_ids[3:]
         elif sm.type == 'animal_horse':
             self.body_ids = all_ids[3:84]                                                       # line 572-573
+        elif sm.type == 'animal_dog':
+            self.body_ids = [all_ids[i] for i in DOG_POSE_IDS]                                  # lines 574-579
         else:
             raise NotImplementedError(sm.type)
         ids = self.root_ids + self.body_ids
@@ -450,15 +463,17 @@ def frames_from_mocap(markers, labels, latent_labels):
 
 
 def mosh_stageii(mocap_fname, cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname=None,
-                 *, mode='lean', chunk=None, max_frames=None, allow_smplx_dmpl=True, mocap=None, on_frame=None) -> dict:
-    """Same signature and return layout as the reference (chmosh.py:458-459, 726-741)."""
+                 *, mode='lean', chunk=None, max_frames=None, allow_smplx_dmpl=True, mocap=None, on_frame=None,
+                 robust_data_sigma=None) -> dict:
+    """Same signature and return layout as the reference (chmosh.py:458-459, 726-741).  ``robust_data_sigma`` (metres; the
+    product's keyword): the data rows Geman-McClure robustified (robust.py) instead of least squares."""
     if mocap is None:
         # host IO adapter (outside the oracle's scope, SURVEY.md 8(f-1)); shared with the product
         from moshpp_b200.mocap_interface import MocapSession
         mocap = MocapSession(mocap_fname, mocap_unit=cfg.mocap.unit, mocap_rotate=cfg.mocap.rotate,
                              only_subjects=[cfg.mocap.subject_name] if cfg.mocap.multi_subject else None)
     solver = StageIISolver(cfg, markers_latent, latent_labels, betas, marker_meta, mode=mode,
-                           allow_smplx_dmpl=allow_smplx_dmpl)
+                           allow_smplx_dmpl=allow_smplx_dmpl, robust_data_sigma=robust_data_sigma)
     n = len(mocap.markers)
     sel = list(range(cfg.mocap.start_fidx, n if cfg.mocap.end_fidx == -1 else cfg.mocap.end_fidx, cfg.mocap.ds_rate))
     if max_frames is not None:

@@ -6,7 +6,6 @@ CPU: the prior constants against the reference's formula, the pose partitions ag
 the other families unchanged, and the device source (single-thread host build) against the float64 oracle in Stage II and
 Stage I.  ``-m gpu``: the CUDA library against the same oracle, the normal equations of a dog frame in both workspace layouts,
 the workspace at the reference's marker counts, and launches that mix the dog with other models."""
-import contextlib
 import copy
 import ctypes as C
 import dataclasses
@@ -20,9 +19,8 @@ from conftest import EmuStageIBackend, dense_obs, gpu_solve, run_oracle, stagei_
 from moshpp_b200 import chmosh, lib, synth
 from moshpp_b200 import pack as _pack
 from moshpp_b200 import stagei as product
-from oracle import prior as oracle_prior
 from oracle import stagei as oracle_stagei
-from oracle import stageii as oracle_stageii
+from oracle.prior import dog_oracle_prior
 
 DOG = dict(frames=10, n_verts=1500)
 DOG_JOINTS = [1, 3, 4, 5, 7, 8, 9, 10, 11, 12, 13, 14, 15, 16, 17, 18, 19, 20, 21, 22, 23, 24, 25, 26, 27, 28, 30, 31, 32, 33, 34]
@@ -45,80 +43,6 @@ def _direct_neglogw(covs, weights):
     return -np.log(weights / ((2 * np.pi) ** (D / 2.) * (sqrdets / sqrdets.min())))
 
 
-
-# ---- the float64 oracle of the dog ---------------------------------------------------------------------------------------
-# The oracle package restates the reference for the SMPL families, MANO and the horse.  The dog's branch is restated here on
-# top of it: the prior of MaxMixtureDog.get_gmm_prior (prior/dog_body_prior.py:53-87) as the oracle's MaxMixtureComplete, and
-# the pose ids of chmosh.py:304-309,574-579.  The oracle's solvers are built for the model as an LBS body without hands (the
-# parametrisation of every animal model) and then given the dog's prior and pose-id partitions.
-
-DOG_POSE_IDS = np.arange(0, 105).reshape([-1, 3])[DOG_JOINTS].reshape(-1)
-
-
-def dog_oracle_prior(prior_pklpath) -> oracle_prior.MaxMixtureComplete:
-    """MaxMixtureDog.get_gmm_prior, with the check its message describes: the reference asserts that some determinant IS zero
-    (lines 78-79), while the message and the division on line 83 mean the opposite."""
-    with open(prior_pklpath, 'rb') as f:
-        gmm = pickle.load(f, encoding='latin-1')
-    npose = len(DOG_POSE_IDS)
-    covars = gmm['gmm_covs'][:, :, DOG_POSE_IDS][:, DOG_POSE_IDS]
-    means = gmm['gmm_means'][:, DOG_POSE_IDS]
-    weights = gmm['gmm_weights'][:]
-    precs = np.asarray([np.linalg.inv(cov) for cov in covars])
-    chols = np.asarray([np.linalg.cholesky(prec) for prec in precs])
-    sqrdets = np.array([(np.sqrt(np.linalg.det(c))) for c in covars])
-    if np.any(sqrdets == 0.0):
-        raise ValueError(f'Encountered zeros in the determinant of the covariance matrix:  {sqrdets}')
-    const = (2 * np.pi) ** (npose / 2.)
-    weights = weights / (const * (sqrdets / sqrdets.min()))
-    return oracle_prior.MaxMixtureComplete(means=means, precs=chols, weights=weights)
-
-
-def _lbs_body_cfg(cfg):
-    c = copy.deepcopy(cfg)
-    c.surface_model.type = 'smpl'               # (an LBS body without hands: body_dof = 3 nJ, no hand PCA)
-    c.moshpp.pose_body_prior_fname = None
-    return c
-
-
-def _dog_ids(solver, n_pose, toes):
-    solver.model.model_type = 'animal_dog'
-    all_ids = list(range(n_pose))
-    solver.body_ids = [all_ids[i] for i in DOG_POSE_IDS]                               # chmosh.py:304-309,574-579
-    solver.finger_ids = []
-    ids = all_ids[:3] + solver.body_ids
-    if not toes:
-        ids = list(set(ids).difference(set(all_ids[30:36])))                          # chmosh.py:389-390,645-647
-    return sorted(ids)
-
-
-class DogStageIISolver(oracle_stageii.StageIISolver):
-    def __init__(self, cfg, *args, **kw):
-        super().__init__(_lbs_body_cfg(cfg), *args, **kw)
-        self.cfg = cfg
-        self.prior = dog_oracle_prior(cfg.moshpp.pose_body_prior_fname) if cfg.moshpp.pose_body_prior_fname else None
-        self.step1_ids = self.step2_ids = _dog_ids(self, self.model.pose_size, bool(cfg.moshpp.optimize_toes))
-
-
-class DogStageISolver(oracle_stagei.StageISolver):
-    def __init__(self, frames, cfg, *args, **kw):
-        super().__init__(frames, _lbs_body_cfg(cfg), *args, **kw)
-        self.cfg = cfg
-        self.prior = dog_oracle_prior(cfg.moshpp.pose_body_prior_fname) if cfg.moshpp.pose_body_prior_fname else None
-        _dog_ids(self, self.model.pose_size, bool(cfg.moshpp.optimize_toes))
-
-
-@contextlib.contextmanager
-def dog_oracle():
-    """The oracle's Stage-I and Stage-II drivers (and everything that builds their solvers) on the dog's solvers."""
-    with mock.patch.object(oracle_stageii, 'StageIISolver', DogStageIISolver), \
-            mock.patch.object(oracle_stagei, 'StageISolver', DogStageISolver):
-        yield
-
-
-def run_dog_oracle(case, **kw):
-    with dog_oracle():
-        return run_oracle(case, **kw)
 
 # ---- the prior constants ------------------------------------------------------------------------------------------------
 
@@ -271,7 +195,7 @@ def _check_f64(case, res, out, tol_pose, tol_trans, rtol, atol):
 
 def test_f64_device_source_equals_oracle(cases, emu):
     case = _dog(cases)
-    out = run_dog_oracle(case)
+    out = run_oracle(case)
     res = emu(case, precision=lib.MOSH2_F64)
     _check_f64(case, res, out, 1e-9, 1e-10, 1e-8, 1e-12)
     assert res.counters[out['stageii_debug_details']['frame_ids'], 3].sum() == out['stageii_debug_details']['oracle_stats']['minimizations']
@@ -280,7 +204,7 @@ def test_f64_device_source_equals_oracle(cases, emu):
 def test_solve_moves_between_mixture_components(cases):
     """The fixture exercises the max-mixture selection: the component of the solved poses changes within the case."""
     case = _dog(cases)
-    out = run_dog_oracle(case)
+    out = run_oracle(case)
     pr = dog_oracle_prior(case['cfg'].moshpp.pose_body_prior_fname)
     comp = [pr.select(x)[0] for x in out['_pose_reduced'][:, _pack.DOG_BODY_IDS]]
     assert len(set(comp)) > 1, comp
@@ -348,8 +272,7 @@ def test_prior_ids_are_read_per_model_in_a_multi_model_job(cases):
 def _stagei(cases, backend, tol):
     case, cfg, frames = stagei_case(cases, 'CD', 4, **DOG)
     cfg.opt_settings.maxiter = 3
-    with dog_oracle():
-        ref = oracle_stagei.mosh_stagei(frames, cfg, marker_meta=case['marker_meta'])
+    ref = oracle_stagei.mosh_stagei(frames, cfg, marker_meta=case['marker_meta'])
     out = product.mosh_stagei(frames, cfg, marker_meta=case['marker_meta'], backend=backend)
     assert np.abs(out['betas'] - ref['betas']).max() < tol
     assert np.abs(out['markers_latent'] - ref['markers_latent']).max() < tol
@@ -383,7 +306,7 @@ def _ne():
 
 def _errors(case, pk, opts, step, obs, vis, x, out, precision, tc=False):
     ne = _ne()
-    with mock.patch.dict(ne.TWIN_F32, {'CD': DOG_F32}), dog_oracle():
+    with mock.patch.dict(ne.TWIN_F32, {'CD': DOG_F32}):
         return ne.normal_equation_errors(case, 'CD', pk, opts, step, obs, vis, x, out, precision, tc=tc)
 
 
@@ -458,7 +381,7 @@ def test_workspace_plan_fits(cases, n_markers):
 @pytest.mark.gpu
 def test_f64_kernel_equals_oracle(cases):
     case = _dog(cases)
-    out = run_dog_oracle(case)
+    out = run_oracle(case)
     res = gpu_solve(case, precision='f64')
     _check_f64(case, res, out, 1e-8, 1e-9, 1e-7, 1e-10)
     mk = np.concatenate(out['stageii_debug_details']['markers_sim'])
@@ -471,7 +394,7 @@ def test_f64_kernel_equals_oracle(cases):
 def test_f32_kernel_within_stated_tolerance(cases):
     """The float32 bounds of tests/test_gpu_parity.py for the horse (BASELINE.md section 4)."""
     case = _dog(cases)
-    out = run_dog_oracle(case)
+    out = run_oracle(case)
     res = gpu_solve(case, precision='f32')
     dbg = out['stageii_debug_details']
     fid = dbg['frame_ids']
@@ -490,7 +413,7 @@ def test_drop_in_callable_with_the_dog_model(cases):
     out = chmosh.mosh_stageii(mocap_fname=case['mocap_fname'], cfg=case['cfg'], markers_latent=case['markers_latent'],
                               latent_labels=case['latent_labels'], betas=case['betas'], marker_meta=case['marker_meta'],
                               precision='f64', chunk_len=0)
-    ref = run_dog_oracle(case)
+    ref = run_oracle(case)
     assert np.abs(out['fullpose'] - ref['fullpose']).max() < 1e-8 and np.abs(out['trans'] - ref['trans']).max() < 1e-9
     e, r = out['stageii_debug_details']['stageii_errs'], ref['stageii_debug_details']['stageii_errs']
     assert set(e) == set(r) == {'data', 'poseB', 'velo'}
@@ -532,7 +455,7 @@ def test_kernel_normal_equations_equal_float64(cases, dog_states, step, precisio
 @pytest.mark.parametrize('precision', ['f64', 'f32'])
 def test_kernel_solve_in_the_global_workspace_layout_equals_oracle(cases, precision, monkeypatch):
     case = _dog(cases)
-    out = run_dog_oracle(case)
+    out = run_oracle(case)
     monkeypatch.setenv('MOSH2_DEV_BIG', '1')
     res = gpu_solve(case, precision=precision)
     monkeypatch.delenv('MOSH2_DEV_BIG')

@@ -11,7 +11,7 @@ apiece.  This module covers that size:
     normal equations of Steps 1 and 2 against the float64 oracle, the Gauss-Newton solve at every n above the sizes the
     other modules reach, up to n2 + 8, and at the normal equations the linearisation exports;
   * on the H100: the drop-in float64 Stage II against the sequential float64 oracle, and Stage I with optimize_face (one
-    linearisation against FaceOracle at a given state, and a short run against the oracle).
+    linearisation against the oracle's rows at a given state, and a short run against the oracle).
 
 Float32 bounds: 4x the maxima of the float32 host build over the same inputs, as ``TWIN_F32`` of
 tests/test_gpu_normal_equations.py and ``TOL`` of tests/test_gpu_same_state.py were set.  The host build's maxima were
@@ -28,6 +28,7 @@ import pytest
 from conftest import EmuStageIBackend, dense_obs, gpu_solve, run_oracle
 from moshpp_b200 import chmosh, lib, synth
 from moshpp_b200 import stagei as product
+from oracle import stagei as oracle
 from test_gpu_gauss_newton import (THREADS, _bind, _maxima, expected_ok, layout_desc, solve_errors, spd_system,
                                    KAPPA)
 from test_gpu_normal_equations import (PREC, _prepare, emu_lin, gpu_linearize, lin_inputs,  # noqa: F401 (emu_lin: a fixture)
@@ -35,7 +36,7 @@ from test_gpu_normal_equations import (PREC, _prepare, emu_lin, gpu_linearize, l
 import test_gpu_normal_equations as ne
 import test_gpu_same_state as ss
 from test_gpu_same_state import same_state_errors
-from test_stagei_face import FaceOracle, _compare, face_oracle_stagei
+from test_stagei_face import _compare
 
 FACE80 = 'CF80'
 # float32 normal equations of the 80-expression family: 4x the host build's maxima (see the module docstring)
@@ -348,7 +349,7 @@ def face80_stagei_case(cases, tmp_path, n_pick=3):
 
 
 def _stagei_linearisation(backend, cases, tmp_path):
-    """One Step-2 linearisation at a given state (non-zero jaw and expressions) against FaceOracle's J, r, A and g."""
+    """One Step-2 linearisation at a given state (non-zero jaw and expressions) against the oracle's J, r, A and g."""
     case, cfg, frames, _ = face80_stagei_case(cases, tmp_path)
     s = product.StageI(frames, cfg, case['marker_meta'], betas=case['betas'], backend=backend)
     assert s.face and s.ne == 80
@@ -367,31 +368,32 @@ def _stagei_linearisation(backend, cases, tmp_path):
     opts.wt_poseF, opts.wt_expr = wts['poseF'], wts['expr']
     dev = backend.linearize(pk, opts, s.obs, s.vis, x, 2, True)
 
-    o = FaceOracle(frames, cfg, case['marker_meta'], case['betas'])
+    o = oracle.StageISolver(frames, cfg, case['marker_meta'], case['betas'])
     ids = o.pose_ids_for(True)
     o.pose[:], o.trans[:], o.expr[:] = s.pose, s.trans, s.expr
-    off_ml, off_fr, per0, per, n = o.face_layout(ids, True)
+    _, off_ml, off_fr, per, n = o.layout(ids, False, True)
     assert per == len(pk.free_step2)
     free = [0, 1, 2] + [3 + int(i) for i in ids]
     assert list(pk.free_step2[:len(free)]) == free
     M, F = o.n_markers, s.F
     col = {l: i for i, l in enumerate(s.labels)}
-    r_all, J_all = o.face_residual(o.get_face_x(ids, True), True, ids, o.weights_for(0.25), True)
-    # FaceOracle's rows: the base terms (no data rows), every frame's data rows, then poseF (3 per frame) and expr (80 per frame)
+    at = {}
+    r_all, J_all = o.residual(o.get_x(ids, False, True), True, ids, False, o.weights_for(0.25), True, free_expr=True,
+                              rows=at)
+    # the oracle's rows of every frame: its data rows, its poseF rows (3 per frame) and its expr rows (80 per frame)
     nv = [len(i) for i in o.lm_ids]
-    face_rows = r_all.shape[0] - F * (3 + 80)
-    data0 = face_rows - 3 * sum(nv)
-    sel = np.r_[np.arange(3), per0 + np.arange(80)]          # translation and expressions: data and expr terms only
+    data0, poseF0, expr0 = at['data'].start, at['poseF'].start, at['expr'].start
+    sel = np.r_[np.arange(3), 3 + len(ids) + np.arange(80)]          # translation and expressions: data and expr terms only
     for f in range(F):
         rows = np.arange(data0 + 3 * sum(nv[:f]), data0 + 3 * sum(nv[:f + 1]))
         cols = slice(off_fr + f * per, off_fr + (f + 1) * per)
         slots = (3 * np.asarray([col[l] for l in np.asarray(o.latent_labels)[o.lm_ids[f]]])[:, None] + np.arange(3)).ravel()
         Jref, rref = np.zeros((3 * M, per)), np.zeros(3 * M)
-        Jref[slots] = -J_all[rows][:, cols]            # FaceOracle's r = obs - sim, the kernel's r = sim - obs
+        Jref[slots] = -J_all[rows][:, cols]            # the oracle's r = obs - sim, the kernel's r = sim - obs
         rref[slots] = -r_all[rows]
         assert np.abs(dev['J'][f] - Jref).max() <= 1e-9 * np.abs(Jref).max(), f
         assert np.abs(dev['r'][f] - rref).max() <= 1e-9 * np.abs(rref).max(), f
-        own = np.r_[rows, face_rows + 3 * f + np.arange(3), face_rows + 3 * F + 80 * f + np.arange(80)]
+        own = np.r_[rows, poseF0 + 3 * f + np.arange(3), expr0 + 80 * f + np.arange(80)]
         Jf, rf = J_all[own][:, cols], r_all[own]
         A_ref, g_ref = Jf.T @ Jf, -Jf.T @ rf
         d = np.sqrt(np.diag(A_ref))[sel]
@@ -413,7 +415,7 @@ def test_kernel_face80_stagei_linearisation_equals_oracle(cases, tmp_path):
 def test_face80_stagei_on_the_gpu_equals_oracle(cases, tmp_path):
     case, cfg, frames, fn = face80_stagei_case(cases, tmp_path)
     cfg.opt_settings.maxiter = 4
-    ref = face_oracle_stagei(frames, cfg, fn, case['marker_meta'])
+    ref = oracle.mosh_stagei(frames, cfg, betas_fname=fn, marker_meta=case['marker_meta'])
     out = product.mosh_stagei(frames, cfg, betas_fname=fn, marker_meta=case['marker_meta'])
     _compare(out, ref, 1e-6)
     assert np.stack(out['stagei_debug_details']['opt_models_expression']).shape == (len(frames), 80)

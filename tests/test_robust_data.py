@@ -2,79 +2,28 @@
 (scan2mesh/robustifiers.py:33-100) on every coordinate of every data row, psi(e) = sigma e / sqrt(sigma^2 + e^2), Jacobian rows
 scaled by psi'(e) = (sigma^2 / (sigma^2 + e^2))^(3/2).
 
-The float64 oracle of the robust objective lives here, on top of the unchanged ``oracle`` package: its frame objective
-(``oracle.stageii._Objective``) with the data rows robustified, swapped in for the oracle's Stage-II driver.
+The float64 oracle is ``oracle.stageii`` with ``robust_data_sigma``; its closed form is ``oracle.robust``.
 
 CPU: the closed form against golden vectors of the unmodified reference (tests/golden/ref_gmof.npz, written by
 tests/golden/make_gmof_vectors.py), the oracle's Jacobian
 against finite differences, the device source (single-thread host build) against the oracle on corrupted captures, the
 recovery of a corrupted capture, and the plumbing of the keyword.  ``-m gpu``: the CUDA library against the oracle, the
 default fast mode on a corrupted 500-frame capture, and the batch / subjects entry points against per-capture calls."""
-import contextlib
 import copy
 import ctypes as C
 import os
-from unittest import mock
 
 import numpy as np
 import pytest
 
-from conftest import dense_obs
+from conftest import dense_obs, run_oracle
 from moshpp_b200 import build, chmosh, lib
 from moshpp_b200.mocap_interface import MocapSession
 from oracle import stageii as oracle_stageii
+from oracle.robust import gm_dpsi, gm_psi
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SIGMA = 0.03        # metres: a few times the marker noise, well below a swapped label or a ghost marker
-
-
-# ---- the closed form the kernel evaluates (mosh2_device.cuh: data_row_gm / data_dpsi_gm), restated in float64 --------------
-def gm_psi(x, sigma):
-    """GMOf(x, sigma) = SignedSqrt(GMOfInternal(x, sigma)) = sigma x / sqrt(sigma^2 + x^2)."""
-    x = np.asarray(x, dtype=np.float64)
-    return sigma * x / np.sqrt(sigma * sigma + x * x)
-
-
-def gm_dpsi(x, sigma):
-    """d GMOf / dx = (sigma^2 / (sigma^2 + x^2))^(3/2); 0 at x = 0, where the reference's SignedSqrt masks its derivative."""
-    x = np.asarray(x, dtype=np.float64)
-    t = sigma * sigma / (sigma * sigma + x * x)
-    return np.where(x != 0, t * np.sqrt(t), 0.0)
-
-
-# ---- the float64 oracle of the robust objective ---------------------------------------------------------------------------
-class RobustObjective(oracle_stageii._Objective):
-    """The oracle's frame objective with the data rows wt psi(e) and their Jacobian rows scaled by psi'(e).  The data term is
-    the first term of every objective the oracle builds (``StageIISolver.frame_terms``)."""
-    sigma = None
-
-    def __call__(self, x, want_jac):
-        out = super().__call__(x, want_jac)
-        r, J = out if want_jac else (out, None)
-        name, wt = self.terms[0]
-        assert name == 'data'
-        nd = 3 * len(self.vis)
-        e = r[:nd] / wt
-        r = r.copy()
-        r[:nd] = wt * gm_psi(e, self.sigma)
-        if not want_jac:
-            return r
-        J = J.copy()
-        J[:nd] *= gm_dpsi(e, self.sigma)[:, None]
-        return r, J
-
-    def term_sse(self):
-        out = super().term_sse()
-        e = (self.s.evaluate(False)['markers'][self.vis] - self.obs).reshape(-1)
-        out['data'] = float(((self.terms[0][1] * gm_psi(e, self.sigma)) ** 2).sum())
-        return out
-
-
-@contextlib.contextmanager
-def robust_oracle(sigma):
-    """The oracle's Stage-II driver with the Geman-McClure data term at ``sigma``."""
-    with mock.patch.object(oracle_stageii, '_Objective', type('RobustObjectiveAt', (RobustObjective,), {'sigma': float(sigma)})):
-        yield
 
 
 def run_robust_oracle(case, sigma, obs, vis, **kw):
@@ -82,9 +31,7 @@ def run_robust_oracle(case, sigma, obs, vis, **kw):
     mocap = MocapSession(case['mocap_fname'], case['cfg'].mocap.unit)
     mocap.markers = np.where(vis[..., None], obs, 0.0)
     mocap.labels = list(case['latent_labels'])
-    with robust_oracle(sigma):
-        return oracle_stageii.mosh_stageii(case['mocap_fname'], case['cfg'], case['markers_latent'], case['latent_labels'],
-                                           case['betas'], case['marker_meta'], mocap=mocap, **kw)
+    return run_oracle(case, mocap=mocap, robust_data_sigma=sigma, **kw)
 
 
 # ---- corrupted captures -----------------------------------------------------------------------------------------------------
@@ -184,14 +131,15 @@ def test_closed_form_equals_the_reference_gmof():
 def test_oracle_robust_jacobian_matches_finite_differences(cases, name):
     case = cases(name)
     obs, vis, _ = small_corruption(case)
-    solver = oracle_stageii.StageIISolver(case['cfg'], case['markers_latent'], case['latent_labels'], case['betas'], case['marker_meta'])
+    solver = oracle_stageii.StageIISolver(case['cfg'], case['markers_latent'], case['latent_labels'], case['betas'], case['marker_meta'],
+                                          robust_data_sigma=SIGMA)
     f = 3                                                        # a frame of the swap
     vi = np.flatnonzero(vis[f])
     rng = np.random.default_rng(1)
     solver.pose[:] = rng.normal(0, 0.1, solver.pose.shape)
     solver.trans[:] = obs[f, vi].mean(0)
     terms, _ = solver.frame_terms(len(vi), velo_target=np.zeros_like(solver.pose))
-    obj = type('RO', (RobustObjective,), {'sigma': SIGMA})(solver, obs[f, vi], vi, terms, solver.step2_ids, solver.nd > 0)
+    obj = oracle_stageii._Objective(solver, obs[f, vi], vi, terms, solver.step2_ids, solver.nd > 0)
     x0 = obj.x0()
     r0, J = obj(x0, True)
     e = (solver.evaluate(False)['markers'][vi] - obs[f, vi]).reshape(-1)

@@ -2,197 +2,19 @@
 fitted with a given shape.  Each frame's model carries the given shape plus its own expressions; the jaw and the expressions
 are free, with their poseF / expr terms, in the two detailed annealing steps only.  CPU: the oracle against finite
 differences, and the product's block solve on the host build of the device source against the oracle.  `-m gpu`: the
-CUDA library, alone and feeding Stage II.
-
-The float64 oracle of the face objective, ``FaceOracle``, is built here on ``oracle/stagei.py``: the terms that do not see
-the expressions (pose prior, init, surface, fingers) come from ``StageISolver.residual`` evaluated with no data rows; the
-data term is restated with each frame's own betas and its columns wrt the expressions, and the poseF / expr terms are added."""
+CUDA library, alone and feeding Stage II.  The float64 oracle is ``oracle.stagei`` with the face on (``optimize_face`` and a
+given shape)."""
 import copy
 
 import numpy as np
 import pytest
-from sklearn.neighbors import NearestNeighbors
 
 from conftest import EmuStageIBackend, stagei_case
 from moshpp_b200 import lib
 from moshpp_b200 import stagei as product
 from oracle import stagei as oracle
-from oracle.dogleg import minimize_dogleg
-from oracle.lbs import LBS
-from oracle.markers import TransformedCoeffs, transformed_lms
 
 POSEF, EXPR = lib.ERR_NAMES.index('poseF'), lib.ERR_NAMES.index('expr')
-
-
-class FaceOracle(oracle.StageISolver):
-    """Stage I with optimize_face and a given shape (chmosh.py:136-151,163-170,283-295,322-324,396-401): every frame's model
-    has its own betas, the given shape plus the frame's expressions at betas[betas_expr_start_id:][:num_expressions]; the
-    canonical body keeps zero expressions.  In the detailed steps the jaw joins pose_ids and every frame's expressions are
-    free, after its pose in the frame block: [trans | pose[pose_ids] | expressions]."""
-
-    def __init__(self, stagei_frames, cfg, marker_meta, betas):
-        super().__init__(stagei_frames, cfg, marker_meta, betas=betas)
-        sm = cfg.surface_model
-        assert sm.type == 'smplx' and not self.optimize_betas
-        self.face_ids = [66, 67, 68]                                                            # the jaw
-        es = int(sm.betas_expr_start_id)
-        self.expr_ids = np.arange(es, es + int(sm.num_expressions))
-        self.expr = np.zeros((self.n_frames, len(self.expr_ids)))
-
-    def pose_ids_for(self, detailed):
-        ids = super().pose_ids_for(detailed)
-        return np.asarray(sorted(set(ids.tolist()) | set(self.face_ids)), dtype=np.int64) if detailed else ids
-
-    def weights_for(self, anneal):
-        out = super().weights_for(anneal)
-        w = self.cfg.opt_settings.weights
-        out['poseF'], out['expr'] = w['stagei_wt_poseF'] * anneal, w['stagei_wt_expr'] * anneal
-        return out
-
-    def frame_betas(self, f):
-        b = self.betas.copy()
-        b[self.expr_ids] = self.expr[f]
-        return b
-
-    def markers_sim_all(self, tc=None, can_v=None):
-        can_v = self.can_v() if can_v is None else can_v
-        tc = TransformedCoeffs(can_v, self.ml) if tc is None else tc
-        lbs = LBS(self.model, tc.closest[:, :3].reshape(-1))
-        out = []
-        for f in range(self.n_frames):
-            v = lbs(self.pose[f], self.frame_betas(f), self.trans[f]).reshape(-1, 3, 3)
-            out.append(transformed_lms(tc, v[:, 0], v[:, 1], v[:, 2]))
-        return out
-
-    # ---- unknowns: the base layout (no free betas) with the free expressions appended to every frame block
-    def face_layout(self, pose_ids, detailed):
-        _, off_ml, off_fr, per0, _ = self.layout(pose_ids, False)
-        per = per0 + (len(self.expr_ids) if detailed else 0)
-        return off_ml, off_fr, per0, per, off_fr + self.n_frames * per
-
-    def get_face_x(self, pose_ids, detailed):
-        _, off_fr, per0, per, _ = self.face_layout(pose_ids, detailed)
-        x0 = self.get_x(pose_ids, False)
-        fr = np.hstack([x0[off_fr:].reshape(self.n_frames, per0), self.expr[:, :per - per0]])
-        return np.concatenate([x0[:off_fr], fr.reshape(-1)])
-
-    def set_face_x(self, x, pose_ids, detailed):
-        _, off_fr, per0, per, _ = self.face_layout(pose_ids, detailed)
-        fr = x[off_fr:].reshape(self.n_frames, per)
-        self.expr[:, :per - per0] = fr[:, per0:]
-        self.set_x(np.concatenate([x[:off_fr], fr[:, :per0].reshape(-1)]), pose_ids, False)
-
-    def face_residual(self, x, want_jac, pose_ids, wts, detailed, per_term=None):
-        self.set_face_x(x, pose_ids, detailed)
-        off_ml, off_fr, per0, per, n = self.face_layout(pose_ids, detailed)
-        M, F, npi = self.n_markers, self.n_frames, len(pose_ids)
-        # the base class's terms with the data rows left out
-        obs, lm_ids = self.obs, self.lm_ids
-        self.obs, self.lm_ids = [o[:0] for o in obs], [i[:0] for i in lm_ids]
-        try:
-            base = self.residual(self.get_x(pose_ids, False), want_jac, pose_ids, False, wts, detailed, per_term)
-        finally:
-            self.obs, self.lm_ids = obs, lm_ids
-        rs, Js = [base[0] if want_jac else base], []
-        if want_jac:
-            J0 = base[1]
-            J = np.zeros((J0.shape[0], n))
-            J[:, :off_fr] = J0[:, :off_fr]
-            for f in range(F):
-                J[:, off_fr + f * per:off_fr + f * per + per0] = J0[:, off_fr + f * per0:off_fr + (f + 1) * per0]
-            Js.append(J)
-
-        def block(name, r, J=None):
-            rs.append(r)
-            if per_term is not None:
-                per_term[name] = per_term.get(name, 0.0) + float((r ** 2).sum())
-            if want_jac:
-                Js.append(J)
-
-        # ---- data, posed on each frame's own model (its columns wrt the expressions: the posed vertices only)
-        can_v = self.can_v()
-        tc = TransformedCoeffs(can_v, self.ml)
-        tri = tc.closest[:, :3]
-        lbs = LBS(self.model, tri.reshape(-1))
-        xids = self.expr_ids if detailed else self.expr_ids[:0]
-        Fcan = np.stack([oracle.coeff_jacobians(can_v[tri[i]], self.ml[i])[1] for i in range(M)]) if want_jac else None
-        for f in range(F):
-            ids = self.lm_ids[f]
-            res = lbs(self.pose[f], self.frame_betas(f), self.trans[f], want_jac, beta_ids=xids)
-            verts = (res[0] if want_jac else res).reshape(M, 3, 3)
-            if not want_jac:
-                sim = transformed_lms(tc, verts[:, 0], verts[:, 1], verts[:, 2])
-                block('data', ((self.obs[f] - sim[ids]) * wts['data']).reshape(-1))
-                continue
-            sim, loc = transformed_lms(tc, verts[:, 0], verts[:, 1], verts[:, 2], True)
-            dv_pose = res[1].reshape(M, 3, 3, -1)
-            dv_beta = res[2].reshape(M, 3, 3, -1)
-            J = np.zeros((len(ids), 3, n))
-            c0 = off_fr + f * per
-            for row, i in enumerate(ids):
-                e1, e2 = verts[i, 1] - verts[i, 0], verts[i, 2] - verts[i, 0]
-                f1 = e1 / np.linalg.norm(e1)
-                nn = np.cross(e1, e2)
-                f2 = nn / np.linalg.norm(nn)
-                Fp = np.stack([f1, f2, np.cross(f1, f2)], axis=1)             # columns: posed frame
-                J[row, :, c0:c0 + 3] = np.eye(3)
-                J[row, :, c0 + 3:c0 + per0] = sum(loc[i, :, 3 * t:3 * t + 3].dot(dv_pose[i, t]) for t in range(3))[:, pose_ids]
-                J[row, :, off_ml + 3 * i:off_ml + 3 * i + 3] = Fp.dot(Fcan[i])
-                J[row, :, c0 + per0:c0 + per] = sum(loc[i, :, 3 * t:3 * t + 3].dot(dv_beta[i, t]) for t in range(3))
-            block('data', ((self.obs[f] - sim[ids]) * wts['data']).reshape(-1), -J.reshape(-1, n) * wts['data'])
-        # ---- the jaw and the expressions of every frame
-        if detailed:
-            col = {pid: c for c, pid in enumerate(pose_ids)}
-            for name, w in (('poseF', wts['poseF']), ('expr', wts['expr'])):
-                for f in range(F):
-                    c0 = off_fr + f * per
-                    cols = [c0 + 3 + col[p] for p in self.face_ids] if name == 'poseF' else list(range(c0 + per0, c0 + per))
-                    r = (self.pose[f, self.face_ids] if name == 'poseF' else self.expr[f]) * w
-                    J = None
-                    if want_jac:
-                        J = np.zeros((r.size, n))
-                        J[np.arange(r.size), cols] = w
-                    block(name, r, J)
-        r = np.concatenate(rs)
-        return (r, np.vstack(Js)) if want_jac else r
-
-    def run(self):
-        cfg = self.cfg
-        self.rigid_adjust()
-        ann = list(cfg.opt_settings.weights['stagei_wt_annealing'])
-        errs = {}
-        for tidx, a in enumerate(ann):
-            detailed = tidx > len(ann) - 3                                                      # chmosh.py:311
-            wts = self.weights_for(a)
-            pose_ids = self.pose_ids_for(detailed)
-
-            def obj(x, want_jac):
-                return self.face_residual(x, want_jac, pose_ids, wts, detailed)
-
-            x, st = minimize_dogleg(obj, self.get_face_x(pose_ids, detailed), e_3=float(cfg.opt_settings.stagei_lr),
-                                    delta_0=0.5, maxiter=int(cfg.opt_settings.maxiter))
-            self.set_face_x(x, pose_ids, detailed)
-            self.stats['r_evals'] += st.r_evals
-            self.stats['j_evals'] += st.j_evals
-            self.stats['iterations'] += st.iterations
-            self.stats['minimizations'] += 1
-            errs = {}
-            self.face_residual(x, False, pose_ids, wts, detailed, per_term=errs)
-        return errs
-
-
-def face_oracle_stagei(stagei_frames, cfg, betas_fname, marker_meta):
-    """The return dictionary of oracle.stagei.mosh_stagei, with the expressions as ``opt_models_expression``."""
-    s = FaceOracle(stagei_frames, cfg, marker_meta, np.load(betas_fname)['betas'])
-    errs = s.run()
-    _, closest = NearestNeighbors(algorithm='kd_tree', n_neighbors=1).fit(s.can_v()).kneighbors(s.ml)
-    sims_all = s.markers_sim_all()
-    dbg = {'opt_models_trans': [t.copy() for t in s.trans], 'opt_models_pose': [p.copy() for p in s.pose],
-           'opt_models_expression': [e.copy() for e in s.expr], 'stagei_errs': errs, 'stagei_markers_sim_all': sims_all,
-           'stagei_markers_sim': [sims_all[f][s.lm_ids[f]] for f in range(s.n_frames)], 'stagei_markers_obs': s.obs,
-           'stagei_labels_obs': s.labels_obs, 'oracle_stats': dict(s.stats)}
-    return {'betas': s.betas.copy(), 'markers_latent': s.ml.copy(), 'latent_labels': s.latent_labels, 'marker_meta': marker_meta,
-            'markers_latent_vids': {l: int(c[0]) for l, c in zip(s.latent_labels, closest.tolist())}, 'stagei_debug_details': dbg}
 
 
 def face_case(cases, tmp_path, n_pick=4):
@@ -236,21 +58,21 @@ def _face_labels(meta):
 
 def test_oracle_face_jacobian_equals_finite_differences(cases, tmp_path):
     case, cfg, frames, _ = face_case(cases, tmp_path, 3)
-    s = FaceOracle(frames, cfg, case['marker_meta'], case['betas'])
+    s = oracle.StageISolver(frames, cfg, case['marker_meta'], case['betas'])
     assert len(s.expr_ids) == 8
     s.rigid_adjust()
     wts = s.weights_for(0.25)
     pose_ids = s.pose_ids_for(True)
     assert {66, 67, 68} <= set(pose_ids.tolist())
-    off_ml, off_fr, _, per, n = s.face_layout(pose_ids, True)
+    _, off_ml, off_fr, per, n = s.layout(pose_ids, False, True)
     npi, M = len(pose_ids), s.n_markers
     rng = np.random.default_rng(0)
-    x0 = s.get_face_x(pose_ids, True)
+    x0 = s.get_x(pose_ids, False, True)
     ids = np.arange(len(x0))
     frame_part = ids >= off_fr
     is_expr = frame_part & ((ids - off_fr) % per >= 3 + npi)
     x0 = x0 + rng.normal(0, 0.02, x0.shape) * (frame_part & ~is_expr) + rng.normal(0, 0.5, x0.shape) * is_expr
-    r, J = s.face_residual(x0, True, pose_ids, wts, True)
+    r, J = s.residual(x0, True, pose_ids, False, wts, True, free_expr=True)
     jaw = int(np.nonzero(pose_ids == 66)[0][0])
     face_marker = s.latent_labels.index(_face_labels(case['marker_meta'])[3])
     cols = [off_fr + 3 + jaw, off_fr + per + 3 + jaw + 2,                                  # the jaw of frames 0 and 1
@@ -262,7 +84,7 @@ def test_oracle_face_jacobian_equals_finite_differences(cases, tmp_path):
     def at(c, dx):
         x = x0.copy()
         x[c] += dx
-        return s.face_residual(x, False, pose_ids, wts, True)
+        return s.residual(x, False, pose_ids, False, wts, True, free_expr=True)
     for c in cols:
         # (a small step: the surface distance of the latent face marker curves strongly, its O(h^2) error at h = 1e-6 is 1e-5)
         h = 1e-7
@@ -277,7 +99,7 @@ def test_face_block_solve_on_device_source_equals_oracle(cases, tmp_path):
     cfg.opt_settings.maxiter = 6
     meta = case['marker_meta']
     assert any(len(fr) < len(meta['marker_vids']) for fr in frames)
-    ref = face_oracle_stagei(frames, cfg, fn, meta)
+    ref = oracle.mosh_stagei(frames, cfg, betas_fname=fn, marker_meta=meta)
     out = product.mosh_stagei(frames, cfg, betas_fname=fn, marker_meta=meta, backend=EmuStageIBackend())
     _compare(out, ref, 1e-9)
     st, rs = out['stagei_debug_details']['b200'], ref['stagei_debug_details']['oracle_stats']
@@ -396,7 +218,7 @@ def gpu_face_stagei(cases, tmp_path_factory):
     import time
     case, cfg, frames, fn = face_case(cases, tmp_path_factory.mktemp('face'))
     cfg.opt_settings.maxiter = 12
-    ref = face_oracle_stagei(frames, cfg, fn, case['marker_meta'])
+    ref = oracle.mosh_stagei(frames, cfg, betas_fname=fn, marker_meta=case['marker_meta'])
     product.DeviceBackend()                 # (loads the library outside the timed call)
     t0 = time.perf_counter()
     out = product.mosh_stagei(frames, cfg, betas_fname=fn, marker_meta=case['marker_meta'])

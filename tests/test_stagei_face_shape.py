@@ -2,11 +2,9 @@
 picked frame's jaw and expressions fitted together.  The reference refuses this case (chmosh.py:103-118,287-291) and suggests
 two Stage-I runs instead; here it is the union of the free-shape objective and the face objective.
 
-The float64 oracle of the joint objective, ``JointOracle``, extends ``FaceOracle`` (tests/test_stagei_face.py) onto the
-free-shape ``oracle.StageISolver``: the data rows of a frame are posed on the frame's own betas (the shape plus its
-expressions), and their columns wrt the shape come through both the frame's model and the marker attachment on the canonical
-body (zero expressions).  Unknowns: [betas (nb) | latent markers (3 M) | frame 0 | frame 1 | ...], a frame's block
-[trans | pose[pose_ids] | expressions (detailed steps)].
+The float64 oracle is ``oracle.stagei`` with ``face_with_free_shape=True``: the data rows of a frame are posed on the frame's
+own betas (the shape plus its expressions), and their columns wrt the shape come through both the frame's model and the
+marker attachment on the canonical body (zero expressions).
 
 CPU: the oracle against finite differences, the product on the host build of the device source against the oracle, the rules
 that turn the face off, and the workspace plans at the reference's size.  `-m gpu`: the CUDA library against the oracle at CF
@@ -21,145 +19,13 @@ import shutil
 
 import numpy as np
 import pytest
-from sklearn.neighbors import NearestNeighbors
 
 from conftest import EmuStageIBackend, stagei_case
 from moshpp_b200 import stagei as product
 from moshpp_b200 import synth
 from oracle import stagei as oracle
-from oracle.lbs import LBS
-from oracle.markers import TransformedCoeffs, transformed_lms
 from test_face_reference_size import _NoBackend, _assert_plans, _relayout, emu_plan, face80_case  # noqa: F401 (emu_plan: a fixture)
-from test_stagei_face import FaceOracle, _assert_same_result, _compare, _face_labels
-
-
-class JointOracle(FaceOracle):
-    """Stage I with a free shape and optimize_face: FaceOracle's frame models, jaw and expressions on the free-shape unknowns.
-    The canonical body keeps zero expressions, so the attachment, init, surface and beta terms are those of the free-shape
-    solver (``StageISolver.residual`` with free betas and no data rows)."""
-
-    def __init__(self, stagei_frames, cfg, marker_meta, betas=None):
-        oracle.StageISolver.__init__(self, stagei_frames, cfg, marker_meta, betas=betas)
-        sm = cfg.surface_model
-        assert sm.type == 'smplx' and self.optimize_betas
-        self.face_ids = [66, 67, 68]                                                            # the jaw
-        es = int(sm.betas_expr_start_id)
-        self.expr_ids = np.arange(es, es + int(sm.num_expressions))
-        self.expr = np.zeros((self.n_frames, len(self.expr_ids)))
-
-    def face_layout(self, pose_ids, detailed):
-        _, off_ml, off_fr, per0, _ = self.layout(pose_ids, True)
-        per = per0 + (len(self.expr_ids) if detailed else 0)
-        return off_ml, off_fr, per0, per, off_fr + self.n_frames * per
-
-    def get_face_x(self, pose_ids, detailed):
-        _, off_fr, per0, per, _ = self.face_layout(pose_ids, detailed)
-        x0 = self.get_x(pose_ids, True)
-        fr = np.hstack([x0[off_fr:].reshape(self.n_frames, per0), self.expr[:, :per - per0]])
-        return np.concatenate([x0[:off_fr], fr.reshape(-1)])
-
-    def set_face_x(self, x, pose_ids, detailed):
-        _, off_fr, per0, per, _ = self.face_layout(pose_ids, detailed)
-        fr = x[off_fr:].reshape(self.n_frames, per)
-        self.expr[:, :per - per0] = fr[:, per0:]
-        self.set_x(np.concatenate([x[:off_fr], fr[:, :per0].reshape(-1)]), pose_ids, True)
-
-    def face_residual(self, x, want_jac, pose_ids, wts, detailed, per_term=None):
-        self.set_face_x(x, pose_ids, detailed)
-        off_ml, off_fr, per0, per, n = self.face_layout(pose_ids, detailed)
-        M, F, nb = self.n_markers, self.n_frames, self.nb
-        # the free-shape terms with the data rows left out (their shape columns included)
-        obs, lm_ids = self.obs, self.lm_ids
-        self.obs, self.lm_ids = [o[:0] for o in obs], [i[:0] for i in lm_ids]
-        try:
-            base = self.residual(self.get_x(pose_ids, True), want_jac, pose_ids, True, wts, detailed, per_term)
-        finally:
-            self.obs, self.lm_ids = obs, lm_ids
-        rs, Js = [base[0] if want_jac else base], []
-        if want_jac:
-            J0 = base[1]
-            J = np.zeros((J0.shape[0], n))
-            J[:, :off_fr] = J0[:, :off_fr]
-            for f in range(F):
-                J[:, off_fr + f * per:off_fr + f * per + per0] = J0[:, off_fr + f * per0:off_fr + (f + 1) * per0]
-            Js.append(J)
-
-        def block(name, r, J=None):
-            rs.append(r)
-            if per_term is not None:
-                per_term[name] = per_term.get(name, 0.0) + float((r ** 2).sum())
-            if want_jac:
-                Js.append(J)
-
-        # ---- data, posed on each frame's own model: columns wrt the shape through the frame's model and the attachment,
-        #      wrt the frame's expressions through the posed vertices only
-        can_v = self.can_v()
-        tc = TransformedCoeffs(can_v, self.ml)
-        tri = tc.closest[:, :3]
-        lbs = LBS(self.model, tri.reshape(-1))
-        xids = self.expr_ids if detailed else self.expr_ids[:0]
-        bids = np.r_[np.arange(nb), xids]
-        if want_jac:
-            Fcan, dk_db = np.zeros((M, 3, 3)), np.zeros((M, 3, nb))
-            for i in range(M):
-                _, Fcan[i], dk_dv = oracle.coeff_jacobians(can_v[tri[i]], self.ml[i])
-                for t in range(3):
-                    dk_db[i] += dk_dv[:, 3 * t:3 * t + 3].dot(self.Sdirs[tri[i, t]][:, :nb])
-        for f in range(F):
-            ids = self.lm_ids[f]
-            res = lbs(self.pose[f], self.frame_betas(f), self.trans[f], want_jac, beta_ids=bids)
-            verts = (res[0] if want_jac else res).reshape(M, 3, 3)
-            if not want_jac:
-                sim = transformed_lms(tc, verts[:, 0], verts[:, 1], verts[:, 2])
-                block('data', ((self.obs[f] - sim[ids]) * wts['data']).reshape(-1))
-                continue
-            sim, loc = transformed_lms(tc, verts[:, 0], verts[:, 1], verts[:, 2], True)
-            dv_pose = res[1].reshape(M, 3, 3, -1)
-            dv_beta = res[2].reshape(M, 3, 3, -1)
-            J = np.zeros((len(ids), 3, n))
-            c0 = off_fr + f * per
-            for row, i in enumerate(ids):
-                e1, e2 = verts[i, 1] - verts[i, 0], verts[i, 2] - verts[i, 0]
-                f1 = e1 / np.linalg.norm(e1)
-                nn = np.cross(e1, e2)
-                f2 = nn / np.linalg.norm(nn)
-                Fp = np.stack([f1, f2, np.cross(f1, f2)], axis=1)             # columns: posed frame
-                db = sum(loc[i, :, 3 * t:3 * t + 3].dot(dv_beta[i, t]) for t in range(3))
-                J[row, :, :nb] = db[:, :nb] + Fp.dot(dk_db[i])
-                J[row, :, off_ml + 3 * i:off_ml + 3 * i + 3] = Fp.dot(Fcan[i])
-                J[row, :, c0:c0 + 3] = np.eye(3)
-                J[row, :, c0 + 3:c0 + per0] = sum(loc[i, :, 3 * t:3 * t + 3].dot(dv_pose[i, t]) for t in range(3))[:, pose_ids]
-                J[row, :, c0 + per0:c0 + per] = db[:, nb:]
-            block('data', ((self.obs[f] - sim[ids]) * wts['data']).reshape(-1), -J.reshape(-1, n) * wts['data'])
-        # ---- the jaw and the expressions of every frame
-        if detailed:
-            col = {pid: c for c, pid in enumerate(pose_ids)}
-            for name, w in (('poseF', wts['poseF']), ('expr', wts['expr'])):
-                for f in range(F):
-                    c0 = off_fr + f * per
-                    cols = [c0 + 3 + col[p] for p in self.face_ids] if name == 'poseF' else list(range(c0 + per0, c0 + per))
-                    r = (self.pose[f, self.face_ids] if name == 'poseF' else self.expr[f]) * w
-                    J = None
-                    if want_jac:
-                        J = np.zeros((r.size, n))
-                        J[np.arange(r.size), cols] = w
-                    block(name, r, J)
-        r = np.concatenate(rs)
-        return (r, np.vstack(Js)) if want_jac else r
-
-
-def joint_oracle_stagei(stagei_frames, cfg, marker_meta):
-    """The return dictionary of oracle.stagei.mosh_stagei, with the expressions as ``opt_models_expression``."""
-    s = JointOracle(stagei_frames, cfg, marker_meta)
-    errs = s.run()
-    _, closest = NearestNeighbors(algorithm='kd_tree', n_neighbors=1).fit(s.can_v()).kneighbors(s.ml)
-    sims_all = s.markers_sim_all()
-    dbg = {'opt_models_trans': [t.copy() for t in s.trans], 'opt_models_pose': [p.copy() for p in s.pose],
-           'opt_models_expression': [e.copy() for e in s.expr], 'stagei_errs': errs, 'stagei_markers_sim_all': sims_all,
-           'stagei_markers_sim': [sims_all[f][s.lm_ids[f]] for f in range(s.n_frames)], 'stagei_markers_obs': s.obs,
-           'stagei_labels_obs': s.labels_obs, 'oracle_stats': dict(s.stats)}
-    return {'betas': s.betas.copy(), 'markers_latent': s.ml.copy(), 'latent_labels': s.latent_labels, 'marker_meta': marker_meta,
-            'markers_latent_vids': {l: int(c[0]) for l, c in zip(s.latent_labels, closest.tolist())}, 'stagei_debug_details': dbg}
+from test_stagei_face import _assert_same_result, _compare, _face_labels
 
 
 def joint_case(cases, n_pick=4, frames=40, **kw):
@@ -185,21 +51,23 @@ def _check_joint_result(out, cfg, n_expr):
 # ---------------------------------------------------------------------------------------------------------------------
 def test_joint_oracle_jacobian_equals_finite_differences(cases):
     case, cfg, frames = joint_case(cases, 3)
-    s = JointOracle(frames, cfg, case['marker_meta'])
+    s = oracle.StageISolver(frames, cfg, case['marker_meta'], face_with_free_shape=True)
     s.rigid_adjust()
     wts = s.weights_for(0.25)
     pose_ids = s.pose_ids_for(True)
-    off_ml, off_fr, per0, per, n = s.face_layout(pose_ids, True)
+    _, off_ml, off_fr, per, n = s.layout(pose_ids, True, True)
+    per0 = s.layout(pose_ids, True)[3]
     nb, npi = s.nb, len(pose_ids)
     assert off_ml == nb == 16 and per == per0 + 8 and n == off_fr + 3 * per
     rng = np.random.default_rng(0)
-    x0 = s.get_face_x(pose_ids, True)
+    x0 = s.get_x(pose_ids, True, True)
     ids = np.arange(len(x0))
     frame_part = ids >= off_fr
     is_expr = frame_part & ((ids - off_fr) % per >= 3 + npi)
     x0 = (x0 + rng.normal(0, 0.02, x0.shape) * (frame_part & ~is_expr) + rng.normal(0, 0.5, x0.shape) * is_expr
           + rng.normal(0, 0.3, x0.shape) * (ids < nb))                                      # non-zero shape and expressions
-    r, J = s.face_residual(x0, True, pose_ids, wts, True)
+    rows = {}
+    r, J = s.residual(x0, True, pose_ids, True, wts, True, free_expr=True, rows=rows)
     assert J.shape == (len(r), n)
     jaw = int(np.nonzero(pose_ids == 66)[0][0])
     face_marker = s.latent_labels.index(_face_labels(case['marker_meta'])[3])
@@ -212,10 +80,9 @@ def test_joint_oracle_jacobian_equals_finite_differences(cases):
     def at(c, dx):
         x = x0.copy()
         x[c] += dx
-        return s.face_residual(x, False, pose_ids, wts, True)
-    # the data rows of frames 0..2 (after the base terms, before poseF / expr): their shape columns see the frame's expressions
-    n_data = 3 * sum(len(i) for i in s.lm_ids)
-    data = np.arange(len(r) - 3 * (3 + 8) - n_data, len(r) - 3 * (3 + 8))
+        return s.residual(x, False, pose_ids, True, wts, True, free_expr=True)
+    # the data rows of frames 0..2: their shape columns see the frame's expressions
+    data = np.arange(len(r))[rows['data']]
     for c in cols:
         # (a small step: the surface distance of the latent face marker curves strongly, its O(h^2) error at h = 1e-6 is 1e-5;
         # the shape columns, large in the init and surface rows, take a larger one against rounding)
@@ -233,7 +100,7 @@ def test_joint_block_solve_on_device_source_equals_oracle(cases):
     cfg.opt_settings.maxiter = 6
     meta = case['marker_meta']
     assert any(len(fr) < len(meta['marker_vids']) for fr in frames)
-    ref = joint_oracle_stagei(frames, cfg, meta)
+    ref = oracle.mosh_stagei(frames, cfg, marker_meta=meta, face_with_free_shape=True)
     out = product.mosh_stagei(frames, cfg, marker_meta=meta, backend=EmuStageIBackend(), face_with_free_shape=True)
     _compare(out, ref, 1e-9)
     st, rs = out['stagei_debug_details']['b200'], ref['stagei_debug_details']['oracle_stats']
@@ -332,7 +199,7 @@ def test_joint_stagei_on_the_gpu_equals_oracle(cases):
     """Per-frame linearisations from mosh2_job_linearize, closest points and distances from mosh2_mesh_distance."""
     case, cfg, frames = joint_case(cases)
     cfg.opt_settings.maxiter = 12
-    ref = joint_oracle_stagei(frames, cfg, case['marker_meta'])
+    ref = oracle.mosh_stagei(frames, cfg, marker_meta=case['marker_meta'], face_with_free_shape=True)
     out = product.mosh_stagei(frames, cfg, marker_meta=case['marker_meta'], face_with_free_shape=True)
     _compare(out, ref, 1e-6)
     _check_joint_result(out, cfg, 8)
@@ -342,7 +209,7 @@ def test_joint_stagei_on_the_gpu_equals_oracle(cases):
 def test_joint80_stagei_on_the_gpu_equals_oracle(cases):
     case, cfg, frames = joint_case(cases, 3, **synth.REFERENCE_FACE)
     cfg.opt_settings.maxiter = 4
-    ref = joint_oracle_stagei(frames, cfg, case['marker_meta'])
+    ref = oracle.mosh_stagei(frames, cfg, marker_meta=case['marker_meta'], face_with_free_shape=True)
     out = product.mosh_stagei(frames, cfg, marker_meta=case['marker_meta'], face_with_free_shape=True)
     _compare(out, ref, 1e-6)
     _check_joint_result(out, cfg, 80)

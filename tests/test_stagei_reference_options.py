@@ -2,10 +2,9 @@
 reference chmosh.py:252-266,360-373) and the extra initial rigid adjustment (``opt_settings.extra_initial_rigid_adjustment``,
 chmosh.py:230-232), as the reference runs them.
 
-The float64 oracle of both options, ``ReferenceOptions``, is a mixin over the unchanged ``oracle.StageISolver`` and the face
-oracles built on it (``FaceOracle``, ``JointOracle``):
-  - the init terms are restated: every type other than 'head' covers its markers minus the correlated ones, the 'head' type is
-    dropped, and ``init_head_corr = corr (ml - init)[head_ids] * wt`` with wt the 'body' type's init weight, else the base one;
+The float64 oracle is ``oracle.stagei`` with ``reference_options=True``:
+  - the init terms: every type other than 'head' covers its markers minus the correlated ones, the 'head' type is dropped,
+    and ``init_head_corr = corr (ml - init)[head_ids] * wt`` with wt the 'body' type's init weight, else the base one;
   - after the per-frame rigid fit, one dog-leg over the unweighted data residual wrt every frame's root orientation and
     translation (e_3 = 1e-3, delta_0 = 0.5, maxiter), the rest fixed.
 
@@ -22,151 +21,14 @@ import shutil
 
 import numpy as np
 import pytest
-from sklearn.neighbors import NearestNeighbors
 
 from conftest import EmuStageIBackend, stagei_case
 from moshpp_b200 import stagei as product
-from moshpp_b200.chmosh import _get
 from oracle import stagei as oracle
-from oracle.dogleg import minimize_dogleg
-from oracle.markers import transformed_lms
 from test_stagei import _compare as _compare_body
-from test_stagei_face import FaceOracle, _compare as _compare_face, face_case
-from test_stagei_face_shape import JointOracle
+from test_stagei_face import _compare as _compare_face, face_case
 
 HEAD = ['LFHD', 'RFHD', 'LBHD', 'RBHD']
-
-
-class ReferenceOptions:
-    """Mixin over an oracle Stage-I solver: the head-marker correlation prior and the extra initial rigid adjustment."""
-
-    def __init__(self, *args, **kw):
-        super().__init__(*args, **kw)
-        self.head_ids, self.head_corr = None, None
-        fname = _get(self.cfg.moshpp, 'head_marker_corr_fname')
-        if fname is not None:
-            head = np.load(fname)
-            if all(m in self.marker_meta['marker_vids'] for m in head['mrk_labels']):
-                self.head_ids = [self.latent_labels.index(m) for m in head['mrk_labels']]
-                self.head_corr = np.asarray(head['corr'], dtype=np.float64)
-        self.extra_rigid = bool(_get(self.cfg.opt_settings, 'extra_initial_rigid_adjustment', False))
-
-    def weights_for(self, anneal):
-        out = super().weights_for(anneal)
-        out['head_corr'] = out['init'].get('body', self.cfg.opt_settings.weights['stagei_wt_init'] * anneal)
-        return out
-
-    def residual(self, x, want_jac, pose_ids, free_betas, wts, detailed, per_term=None):
-        if self.head_ids is None:
-            return super().residual(x, want_jac, pose_ids, free_betas, wts, detailed, per_term)
-        # the solver's terms with every init weight 0 (their rows vanish), then the init terms of the prior
-        terms = {}
-        base = super().residual(x, want_jac, pose_ids, free_betas, dict(wts, init={k: 0.0 for k in wts['init']}), detailed,
-                                terms)
-        rs, Js = [base[0] if want_jac else base], [base[1]] if want_jac else []
-
-        def block(name, r, J=None):
-            rs.append(r)
-            terms[name] = terms.get(name, 0.0) + float((r ** 2).sum())
-            if want_jac:
-                Js.append(J)
-        nbf, off_ml, _, _, n = self.layout(pose_ids, free_betas)
-        can_v = self.can_v()
-        t0 = self.tc0.closest[:, :3]
-        init, loc0 = transformed_lms(self.tc0, can_v[t0[:, 0]], can_v[t0[:, 1]], can_v[t0[:, 2]], True)
-        diff = self.ml - init
-
-        def dinit_db(i):
-            return sum(loc0[i, :, 3 * t:3 * t + 3].dot(self.Sdirs[t0[i, t]][:, :nbf]) for t in range(3))
-        for k, mask in self.marker_meta['marker_type_mask'].items():
-            if k == 'head':
-                continue
-            ids = sorted(set(np.nonzero(np.asarray(mask, dtype=bool))[0].tolist()) - set(self.head_ids))
-            w = wts['init'][k]
-            J = None
-            if want_jac:
-                J = np.zeros((len(ids), 3, n))
-                for row, i in enumerate(ids):
-                    J[row, :, off_ml + 3 * i:off_ml + 3 * i + 3] = np.eye(3)
-                    if nbf:
-                        J[row, :, :nbf] = -dinit_db(i)
-                J = J.reshape(-1, n) * w
-            block(f'init_{k}', (diff[ids] * w).reshape(-1), J)
-        w, C = wts['head_corr'], self.head_corr
-        J = None
-        if want_jac:
-            J = np.zeros((len(C), 3, n))
-            for j, i in enumerate(self.head_ids):
-                for q in range(len(C)):
-                    J[q, :, off_ml + 3 * i:off_ml + 3 * i + 3] += C[q, j] * np.eye(3)
-                    if nbf:
-                        J[q, :, :nbf] -= C[q, j] * dinit_db(i)
-            J = J.reshape(-1, n) * w
-        block('init_head_corr', (C.dot(diff[self.head_ids]) * w).reshape(-1), J)
-        if per_term is not None:        # (the solver's zero-weighted init terms were added to; the 'head' type has none)
-            for k, v in terms.items():
-                if k != 'init_head':
-                    per_term[k] = per_term.get(k, 0.0) + v
-        r = np.concatenate(rs)
-        return (r, np.vstack(Js)) if want_jac else r
-
-    # ---- the extra rigid adjustment: unknowns [trans | pose[:3]] of every frame, the data residual unweighted
-    def rigid_weights(self):
-        w = {'data': 1.0, 'poseB': 0.0, 'poseH': 0.0, 'beta': 0.0, 'surf': 0.0, 'head_corr': 0.0}
-        w['init'] = {k: 0.0 for k in self.marker_meta['marker_type_mask']}
-        return w
-
-    def rigid_residual(self, xr, want_jac):
-        """The solver's residual at pose_ids [0, 1, 2] and a fixed shape, with every weight but the data's 0: its rows beyond
-        the data are 0, its columns beyond the frame blocks (the latent markers) are dropped."""
-        pose_ids = np.arange(3)
-        off = 3 * self.n_markers
-        x = self.get_x(pose_ids, False)
-        x[off:] = xr
-        out = oracle.StageISolver.residual(self, x, want_jac, pose_ids, False, self.rigid_weights(), False)
-        return (out[0], out[1][:, off:]) if want_jac else out
-
-    def rigid_adjust(self):
-        super().rigid_adjust()
-        if not self.extra_rigid:
-            return
-        pose_ids, off = np.arange(3), 3 * self.n_markers
-        xr, st = minimize_dogleg(self.rigid_residual, self.get_x(pose_ids, False)[off:], e_3=1e-3, delta_0=0.5,
-                                 maxiter=int(self.cfg.opt_settings.maxiter))
-        x = self.get_x(pose_ids, False)
-        x[off:] = xr
-        self.set_x(x, pose_ids, False)
-        self.stats['r_evals'] += st.r_evals
-        self.stats['j_evals'] += st.j_evals
-        self.stats['iterations'] += st.iterations
-        self.stats['minimizations'] += 1
-
-
-class BodyRefOracle(ReferenceOptions, oracle.StageISolver):
-    pass
-
-
-class FaceRefOracle(ReferenceOptions, FaceOracle):
-    pass
-
-
-class JointRefOracle(ReferenceOptions, JointOracle):
-    pass
-
-
-def oracle_result(s):
-    """The return dictionary of oracle.stagei.mosh_stagei for a constructed solver (with the face: the expressions too)."""
-    errs = s.run()
-    _, closest = NearestNeighbors(algorithm='kd_tree', n_neighbors=1).fit(s.can_v()).kneighbors(s.ml)
-    sims_all = s.markers_sim_all()
-    dbg = {'opt_models_trans': [t.copy() for t in s.trans], 'opt_models_pose': [p.copy() for p in s.pose], 'stagei_errs': errs,
-           'stagei_markers_sim_all': sims_all, 'stagei_markers_sim': [sims_all[f][s.lm_ids[f]] for f in range(s.n_frames)],
-           'stagei_markers_obs': s.obs, 'stagei_labels_obs': s.labels_obs, 'oracle_stats': dict(s.stats)}
-    if hasattr(s, 'expr'):
-        dbg['opt_models_expression'] = [e.copy() for e in s.expr]
-    return {'betas': s.betas.copy(), 'markers_latent': s.ml.copy(), 'latent_labels': s.latent_labels,
-            'marker_meta': s.marker_meta, 'stagei_debug_details': dbg,
-            'markers_latent_vids': {l: int(c[0]) for l, c in zip(s.latent_labels, closest.tolist())}}
 
 
 def write_corr(fname, labels, extra_rows=2, seed=0):
@@ -235,8 +97,8 @@ def test_oracle_new_rows_equal_finite_differences(cases, tmp_path):
     case, cfg, frames = stagei_case(cases, 'C2', 3, frames=40, n_verts=1500, dropout=0.0)
     cfg.moshpp.head_marker_corr_fname = write_corr(str(tmp_path / 'head_corr.npz'), HEAD)
     cfg.opt_settings.extra_initial_rigid_adjustment = True
-    s = BodyRefOracle(frames, cfg, case['marker_meta'])
-    oracle.StageISolver.rigid_adjust(s)
+    s = oracle.StageISolver(frames, cfg, case['marker_meta'], reference_options=True)
+    s.rigid_adjust()
     wts = s.weights_for(0.5)
     pose_ids = s.pose_ids_for(True)
     rng = np.random.default_rng(0)
@@ -244,18 +106,20 @@ def test_oracle_new_rows_equal_finite_differences(cases, tmp_path):
     nb, M = s.nb, s.n_markers
     ids = np.arange(len(x0))
     x0 = x0 + rng.normal(0, 0.02, x0.shape) * (ids >= nb + 3 * M) + rng.normal(0, 0.3, x0.shape) * (ids < nb)
-    r, J = s.residual(x0, True, pose_ids, True, wts, True)
+    at = {}
+    r, J = s.residual(x0, True, pose_ids, True, wts, True, rows=at)
     n_new = 3 * (M - len(HEAD)) + 3 * (len(HEAD) + 2)                     # init rows of the other markers + K x 3 corr rows
-    rows = np.arange(len(r) - n_new, len(r))
-    h0, h1 = s.head_ids[0], s.head_ids[3]
+    rows = np.concatenate([np.arange(len(r))[sl] for k, sl in at.items() if k.startswith('init_')])     # init_head_corr last
+    assert len(rows) == n_new
+    h0, h1 = s.corr_ids[0], s.corr_ids[3]
     body = s.latent_labels.index('C7')
     cols = [0, 3, nb - 1, nb + 3 * h0, nb + 3 * h1 + 2, nb + 3 * body + 1]
     _fd_check(lambda x: s.residual(x, False, pose_ids, True, wts, True), x0, J, cols, rows, 1e-5, 5e-8)
     # the head rows couple the correlated markers densely, the other init rows do not see them
     assert np.count_nonzero(J[rows[-3 * (len(HEAD) + 2):], nb:nb + 3 * M].any(0)) == 3 * len(HEAD)
-    assert not J[rows[:-3 * (len(HEAD) + 2)]][:, [nb + 3 * i + c for i in s.head_ids for c in range(3)]].any()
+    assert not J[rows[:-3 * (len(HEAD) + 2)]][:, [nb + 3 * i + c for i in s.corr_ids for c in range(3)]].any()
 
-    xr = s.get_x(np.arange(3), False)[3 * M:] + rng.normal(0, 0.02, 6 * s.n_frames)
+    xr = np.hstack([s.trans, s.pose[:, :3]]).reshape(-1) + rng.normal(0, 0.02, 6 * s.n_frames)
     r, J = s.rigid_residual(xr, True)
     data = np.arange(3 * sum(len(i) for i in s.lm_ids))
     assert J.shape == (len(r), 6 * s.n_frames) and not r[len(data):].any() and not J[len(data):].any()
@@ -270,7 +134,7 @@ def test_head_corr_on_device_source_equals_oracle(cases, tmp_path):
     case, cfg, frames = body_case(cases, tmp_path)
     cfg.opt_settings.maxiter = 6
     meta = case['marker_meta']
-    ref = oracle_result(BodyRefOracle(frames, cfg, meta))
+    ref = oracle.mosh_stagei(frames, cfg, marker_meta=meta, reference_options=True)
     out = _emu(frames, cfg, meta, reference_options=True)
     _compare_body(out, ref, 1e-9)
     _check_stats(out, ref, 4)
@@ -284,7 +148,7 @@ def test_head_typed_markers_on_device_source_equal_oracle(cases, tmp_path):
     case, cfg, frames = body_case(cases, tmp_path)
     cfg.opt_settings.maxiter = 6
     meta = relabel(case['marker_meta'], {'LFHD': 'head', 'RFHD': 'head', 'ARIEL': 'head'})
-    ref = oracle_result(BodyRefOracle(frames, cfg, meta))
+    ref = oracle.mosh_stagei(frames, cfg, marker_meta=meta, reference_options=True)
     out = _emu(frames, cfg, meta, reference_options=True)
     _compare_body(out, ref, 1e-9)
     _check_stats(out, ref, 4)
@@ -307,7 +171,7 @@ def test_extra_rigid_adjustment_on_device_source_equals_oracle(cases, tmp_path):
     cfg.opt_settings.maxiter = 6
     cfg.opt_settings.extra_initial_rigid_adjustment = True
     meta = case['marker_meta']
-    ref = oracle_result(FaceRefOracle(frames, cfg, meta, np.load(fn)['betas']))
+    ref = oracle.mosh_stagei(frames, cfg, betas_fname=fn, marker_meta=meta, reference_options=True)
     out = _emu(frames, cfg, meta, betas_fname=fn, reference_options=True)
     _compare_face(out, ref, 1e-9)
     _check_stats(out, ref, 5)
@@ -321,7 +185,7 @@ def test_both_options_with_free_shape_face_on_device_source_equal_oracle(cases, 
     cfg.opt_settings.extra_initial_rigid_adjustment = True
     cfg.moshpp.head_marker_corr_fname = write_corr(str(tmp_path / 'head_corr.npz'), HEAD, seed=1)
     meta = case['marker_meta']
-    ref = oracle_result(JointRefOracle(frames, cfg, meta))
+    ref = oracle.mosh_stagei(frames, cfg, marker_meta=meta, face_with_free_shape=True, reference_options=True)
     out = _emu(frames, cfg, meta, face_with_free_shape=True, reference_options=True)
     _compare_face(out, ref, 1e-9)
     _check_stats(out, ref, 5)
@@ -373,7 +237,7 @@ def test_reported_init_terms(cases, tmp_path):
     assert e['init_headband'] == 0.0 and e['init_body'] > 0
     assert {k for k in e if k.startswith('init_')} == {'init_body', 'init_finger_left', 'init_finger_right', 'init_headband',
                                                        'init_head_corr'}
-    o = BodyRefOracle(frames, cfg, meta)
+    o = oracle.StageISolver(frames, cfg, meta, reference_options=True)
     o.ml += move
     terms = {}
     o.residual(o.get_x(o.pose_ids_for(False), True), False, o.pose_ids_for(False), True, o.weights_for(1.0), False, terms)
@@ -460,7 +324,7 @@ def test_head_corr_on_the_gpu_equals_oracle(cases, tmp_path):
     case, cfg, frames = body_case(cases, tmp_path)
     cfg.opt_settings.maxiter = 12
     meta = case['marker_meta']
-    ref = oracle_result(BodyRefOracle(frames, cfg, meta))
+    ref = oracle.mosh_stagei(frames, cfg, marker_meta=meta, reference_options=True)
     out = product.mosh_stagei(frames, cfg, marker_meta=meta, reference_options=True)
     _compare_body(out, ref, 1e-6)
     assert out['stagei_debug_details']['stagei_errs']['init_head_corr'] > 0
@@ -472,7 +336,7 @@ def test_extra_rigid_adjustment_on_the_gpu_equals_oracle(cases, tmp_path):
     cfg.opt_settings.maxiter = 12
     cfg.opt_settings.extra_initial_rigid_adjustment = True
     meta = case['marker_meta']
-    ref = oracle_result(FaceRefOracle(frames, cfg, meta, np.load(fn)['betas']))
+    ref = oracle.mosh_stagei(frames, cfg, betas_fname=fn, marker_meta=meta, reference_options=True)
     out = product.mosh_stagei(frames, cfg, betas_fname=fn, marker_meta=meta, reference_options=True)
     _compare_face(out, ref, 1e-6)
     assert out['stagei_debug_details']['b200']['minimisations'] == 5

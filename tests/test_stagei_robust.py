@@ -3,15 +3,14 @@ annealing steps and of the extra rigid adjustment is wd psi(e), psi(e) = sigma e
 visible marker's e = sim - obs, its Jacobian row the least-squares one times psi'(e) = (sigma^2 / (sigma^2 + e^2))^(3/2).  The
 Procrustes start and the init, head-correlation, shape, surface and pose terms stay least squares.
 
-The float64 oracle of the robust objective, ``RobustData``, is a mixin over the oracle Stage-I solvers: the unchanged
-``oracle.StageISolver``, ``FaceOracle``, ``JointOracle`` and the ``ReferenceOptions`` mixin of the Stage-I test modules.
+The float64 oracle is ``oracle.stagei`` with ``robust_data_sigma``, alone and with the face, ``face_with_free_shape`` and
+``reference_options``.
 
 CPU: the oracle against finite differences on rows of a swapped label and a ghost marker; the product on the host build of the
 device source against the oracle on corrupted picked frames (C2 with a free shape, CF with the face and a given shape, CF with
 ``face_with_free_shape``, C2 with ``reference_options``); the keyword off and bad values; the recovery of the shape and the
 latent markers from corrupted picked frames, and what that does to a least-squares Stage II downstream; the head.  ``-m gpu``:
 one CUDA linearisation against the host build's, the CUDA library against the oracle, and the head with both stages robust."""
-import copy
 import ctypes as C
 import functools
 import json
@@ -26,76 +25,11 @@ from conftest import EmuStageIBackend, dense_obs, stagei_case
 from moshpp_b200 import build, chmosh, lib
 from moshpp_b200 import stagei as product
 from oracle import stagei as oracle
-from test_robust_data import SIGMA, corrupt, gm_dpsi, gm_psi
+from oracle.robust import gm_dpsi, gm_psi
+from test_robust_data import SIGMA, corrupt
 from test_stagei import _compare as _compare_body
-from test_stagei_face import FaceOracle, _compare as _compare_face, face_case
-from test_stagei_face_shape import JointOracle
-from test_stagei_reference_options import HEAD, ReferenceOptions, _assert_bit_identical, _check_stats, oracle_result, write_corr
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# the float64 oracle of the robust objective
-# ---------------------------------------------------------------------------------------------------------------------
-class RobustData:
-    """Mixin over an oracle Stage-I solver: the data rows wd psi(e) and their Jacobian rows times psi'(e).
-
-    The oracle writes a data row as wd (obs - sim) = -wd e; psi is odd and psi' even, so wd psi(obs - sim) is the product's row
-    up to its sign, and the objective is the same.  Where the data rows sit: first in ``StageISolver.residual`` (also under
-    ``ReferenceOptions``, whose rows follow the solver's) and in ``rigid_residual`` (weight 1); in ``face_residual`` after the
-    rows of the other terms and before the poseF / expr rows of the detailed steps (``StageISolver.residual`` there runs with
-    no observations, so it has no data rows)."""
-    sigma = SIGMA
-
-    def _robust(self, out, want_jac, lo, wd, per_term):
-        nd = 3 * sum(len(i) for i in self.lm_ids)
-        r, J = out if want_jac else (out, None)
-        e = r[lo:lo + nd] / wd
-        r = r.copy()
-        r[lo:lo + nd] = wd * gm_psi(e, self.sigma)
-        if per_term is not None:
-            per_term['data'] = float((r[lo:lo + nd] ** 2).sum())
-        if not want_jac:
-            return r
-        J = J.copy()
-        J[lo:lo + nd] *= gm_dpsi(e, self.sigma)[:, None]
-        return r, J
-
-    def residual(self, x, want_jac, pose_ids, free_betas, wts, detailed, per_term=None):
-        out = super().residual(x, want_jac, pose_ids, free_betas, wts, detailed, per_term)
-        return self._robust(out, want_jac, 0, wts['data'], per_term)
-
-    def face_residual(self, x, want_jac, pose_ids, wts, detailed, per_term=None):
-        out = super().face_residual(x, want_jac, pose_ids, wts, detailed, per_term)
-        rows = len(out[0] if want_jac else out)
-        tail = self.n_frames * (len(self.face_ids) + len(self.expr_ids)) if detailed else 0
-        return self._robust(out, want_jac, rows - tail - 3 * sum(len(i) for i in self.lm_ids), wts['data'], per_term)
-
-    def rigid_residual(self, xr, want_jac):
-        return self._robust(super().rigid_residual(xr, want_jac), want_jac, 0, 1.0, None)
-
-
-class RobustBody(RobustData, oracle.StageISolver):
-    pass
-
-
-class RobustFace(RobustData, FaceOracle):
-    pass
-
-
-class RobustJoint(RobustData, JointOracle):
-    pass
-
-
-class RobustBodyRef(RobustData, ReferenceOptions, oracle.StageISolver):
-    def run(self):
-        # oracle.StageISolver.run refuses the extra rigid adjustment, which ReferenceOptions.rigid_adjust carries out
-        cfg = self.cfg
-        self.cfg = copy.deepcopy(cfg)
-        self.cfg.opt_settings.extra_initial_rigid_adjustment = False
-        try:
-            return super().run()
-        finally:
-            self.cfg = cfg
+from test_stagei_face import _compare as _compare_face, face_case
+from test_stagei_reference_options import HEAD, _assert_bit_identical, _check_stats, write_corr
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -151,8 +85,8 @@ def test_oracle_robust_jacobian_equals_finite_differences(cases, tmp_path):
     meta = case['marker_meta']
     frames, moved = corrupt_frames(frames, meta, swap=slice(1, 2), ghost=slice(2, 3))
     cfg.opt_settings.extra_initial_rigid_adjustment = True
-    s = RobustBodyRef(frames, cfg, meta)
-    oracle.StageISolver.rigid_adjust(s)
+    s = oracle.StageISolver(frames, cfg, meta, reference_options=True, robust_data_sigma=SIGMA)
+    s.rigid_adjust()
     wts = s.weights_for(0.5)
     pose_ids = s.pose_ids_for(True)
     rng = np.random.default_rng(0)
@@ -160,9 +94,12 @@ def test_oracle_robust_jacobian_equals_finite_differences(cases, tmp_path):
     nb, M = s.nb, s.n_markers
     ids = np.arange(len(x0))
     x0 = x0 + rng.normal(0, 0.02, x0.shape) * (ids >= nb + 3 * M) + rng.normal(0, 0.3, x0.shape) * (ids < nb)
-    r, J = s.residual(x0, True, pose_ids, True, wts, True)
+    at = {}
+    r, J = s.residual(x0, True, pose_ids, True, wts, True, rows=at)
+    data = np.arange(len(r))[at['data']]
     nd = 3 * sum(len(i) for i in s.lm_ids)
-    e = oracle.StageISolver.residual(s, x0, False, pose_ids, True, wts, True)[:nd] / wts['data']       # (least squares: -e)
+    sims = s.markers_sim_all()
+    e = np.concatenate([(s.obs[f] - sims[f][s.lm_ids[f]]).reshape(-1) for f in range(s.n_frames)])     # (least squares: -e)
     dpsi = gm_dpsi(e, SIGMA)
     # rows of the corrupted labels (swapped in frame 1, the ghost in frame 2): psi' far below 1
     off = np.cumsum([0] + [3 * len(i) for i in s.lm_ids])
@@ -175,11 +112,12 @@ def test_oracle_robust_jacobian_equals_finite_differences(cases, tmp_path):
     cols = [nb + 3 * i + c for i in moved for c in (0, 2)] + [f1, f1 + 4, f1 + per + 1, f1 + per + 5, nb + 3 * M + 2]
     res = lambda x: s.residual(x, False, pose_ids, True, wts, True)      # noqa: E731
     # (the shape columns with a longer step: their differences lose more to rounding, as in the least-squares rows)
-    assert _fd(res, x0, J, [0, nb - 1], np.arange(nd), 2e-5) < 5e-8
-    assert _fd(res, x0, J, cols, np.arange(nd), 1e-6) < 5e-8
-    assert _fd(res, x0, J, cols[:6], bad, 1e-6) < 5e-8
+    assert len(data) == nd
+    assert _fd(res, x0, J, [0, nb - 1], data, 2e-5) < 5e-8
+    assert _fd(res, x0, J, cols, data, 1e-6) < 5e-8
+    assert _fd(res, x0, J, cols[:6], data[bad], 1e-6) < 5e-8
 
-    xr = s.get_x(np.arange(3), False)[3 * M:] + rng.normal(0, 0.02, 6 * s.n_frames)
+    xr = np.hstack([s.trans, s.pose[:, :3]]).reshape(-1) + rng.normal(0, 0.02, 6 * s.n_frames)
     r, J = s.rigid_residual(xr, True)
     assert product.data_dpsi_gm(r[bad], 1.0, SIGMA).min() < 0.05
     assert _fd(lambda x: s.rigid_residual(x, False), xr, J, [0, 2, 3, 5, 6 + 4, 12 + 1], np.arange(nd), 1e-6) < 5e-8
@@ -194,7 +132,7 @@ def test_free_shape_on_device_source_equals_oracle(cases):
     cfg.opt_settings.maxiter = 6
     meta = case['marker_meta']
     frames, _ = corrupt_frames(frames, meta, swap=slice(1, 2), ghost=slice(2, 3), spikes=[2])
-    ref = oracle_result(RobustBody(frames, cfg, meta))
+    ref = oracle.mosh_stagei(frames, cfg, marker_meta=meta, robust_data_sigma=SIGMA)
     out = _emu(frames, cfg, meta, robust_data_sigma=SIGMA)
     _compare_body(out, ref, 1e-9)
     _check_stats(out, ref, 4)
@@ -207,7 +145,7 @@ def test_face_given_shape_on_device_source_equals_oracle(cases, tmp_path):
     cfg.opt_settings.maxiter = 6
     meta = case['marker_meta']
     frames, _ = corrupt_frames(frames, meta, swap=slice(1, 2), ghost=slice(3, 4))
-    ref = oracle_result(RobustFace(frames, cfg, meta, np.load(fn)['betas']))
+    ref = oracle.mosh_stagei(frames, cfg, betas_fname=fn, marker_meta=meta, robust_data_sigma=SIGMA)
     out = _emu(frames, cfg, meta, betas_fname=fn, robust_data_sigma=SIGMA)
     _compare_face(out, ref, 1e-9)
     _check_stats(out, ref, 4)
@@ -219,7 +157,7 @@ def test_face_with_free_shape_on_device_source_equals_oracle(cases):
     cfg.opt_settings.maxiter = 6
     meta = case['marker_meta']
     frames, _ = corrupt_frames(frames, meta, swap=slice(1, 2), ghost=slice(2, 3), spikes=[2])
-    ref = oracle_result(RobustJoint(frames, cfg, meta))
+    ref = oracle.mosh_stagei(frames, cfg, marker_meta=meta, face_with_free_shape=True, robust_data_sigma=SIGMA)
     out = _emu(frames, cfg, meta, face_with_free_shape=True, robust_data_sigma=SIGMA)
     _compare_face(out, ref, 1e-9)
     _check_stats(out, ref, 4)
@@ -233,7 +171,7 @@ def test_reference_options_on_device_source_equal_oracle(cases, tmp_path):
     cfg.moshpp.head_marker_corr_fname = write_corr(str(tmp_path / 'head_corr.npz'), HEAD)
     meta = case['marker_meta']
     frames, _ = corrupt_frames(frames, meta, swap=slice(2, 3), ghost=slice(1, 2))
-    ref = oracle_result(RobustBodyRef(frames, cfg, meta))
+    ref = oracle.mosh_stagei(frames, cfg, marker_meta=meta, reference_options=True, robust_data_sigma=SIGMA)
     out = _emu(frames, cfg, meta, reference_options=True, robust_data_sigma=SIGMA)
     _compare_body(out, ref, 1e-9)
     _check_stats(out, ref, 5)
@@ -247,11 +185,11 @@ def test_rigid_adjustment_rows_are_robust(cases, tmp_path):
     frames, _ = corrupt_frames(frames, meta, swap=slice(1, 2), ghost=slice(2, 3))
     cfg.opt_settings.extra_initial_rigid_adjustment = True
     s = product.StageI(frames, cfg, meta, backend=EmuStageIBackend(), reference_options=True, robust_data_sigma=SIGMA)
-    o = RobustBodyRef(frames, cfg, meta)
-    oracle.StageISolver.rigid_adjust(o)
+    o = oracle.StageISolver(frames, cfg, meta, reference_options=True, robust_data_sigma=SIGMA)
+    o.rigid_adjust()
     s.pose[:], s.trans[:] = o.pose, o.trans
     A, g = s.evaluate_rigid(True)
-    r, J = o.rigid_residual(o.get_x(np.arange(3), False)[3 * o.n_markers:], True)
+    r, J = o.rigid_residual(np.hstack([o.trans, o.pose[:, :3]]).reshape(-1), True)
     assert abs(s._last_total - (r ** 2).sum()) <= 1e-10 * (r ** 2).sum()
     assert np.abs(A - J.T.dot(J)).max() <= 1e-9 * np.abs(A).max()
     assert np.abs(g + J.T.dot(r)).max() <= 1e-9 * np.abs(g).max()       # g = -J^T r (the oracle's rows and J: the sign of both flipped)
@@ -469,7 +407,7 @@ def test_free_shape_on_the_gpu_equals_oracle(cases):
     case, cfg, frames = _corrupted_c2(cases)
     cfg.opt_settings.maxiter = 12
     meta = case['marker_meta']
-    ref = oracle_result(RobustBody(frames, cfg, meta))
+    ref = oracle.mosh_stagei(frames, cfg, marker_meta=meta, robust_data_sigma=SIGMA)
     out = product.mosh_stagei(frames, cfg, marker_meta=meta, backend=DeviceLinearisation(), robust_data_sigma=SIGMA)
     _compare_body(out, ref, 1e-9)
     _check_stats(out, ref, 4)
@@ -486,7 +424,7 @@ def test_face_with_free_shape_on_the_gpu_equals_oracle(cases):
     cfg.opt_settings.maxiter = 12
     meta = case['marker_meta']
     frames, _ = corrupt_frames(frames, meta, swap=slice(1, 2), ghost=slice(2, 3), spikes=[2])
-    ref = oracle_result(RobustJoint(frames, cfg, meta))
+    ref = oracle.mosh_stagei(frames, cfg, marker_meta=meta, face_with_free_shape=True, robust_data_sigma=SIGMA)
     out = product.mosh_stagei(frames, cfg, marker_meta=meta, face_with_free_shape=True, robust_data_sigma=SIGMA)
     _compare_face(out, ref, 1e-6)
 

@@ -4,8 +4,8 @@ coefficients -- through moshpp_b200.stagei.mosh_stagei; with --oracle also the f
 jaw and expressions fitted together (face_with_free_shape).
 --reference-options: with the head-marker correlation prior (a synthetic K x H file over the LFHD / RFHD / LBHD / RBHD
 markers) and the extra initial rigid adjustment, both through reference_options=True.
---robust-data-sigma S: the Geman-McClure data term at sigma = S metres (robust_data_sigma); with --oracle the oracle is the
-robust one of tests/test_stagei_robust.py.
+--robust-data-sigma S: the Geman-McClure data term at sigma = S metres (robust_data_sigma).
+With --oracle the float64 oracle runs with the same keywords as the library.
 Usage: python tools/gpu_stagei.py [--oracle] [--frames 12] [--face80] [--reference-options] [--robust-data-sigma S]"""
 import argparse
 import copy
@@ -69,22 +69,19 @@ def main():
         line['workload'] += ', head-marker correlation prior + extra initial rigid adjustment'
     if a.robust_data_sigma is not None:
         line['workload'] += f', Geman-McClure data term at sigma = {a.robust_data_sigma} m'
-    if a.oracle and not (a.face80 or a.reference_options):
+    if a.oracle:
         from oracle import stagei as ostagei
         t0 = time.perf_counter()
-        if a.robust_data_sigma is None:
-            ref = ostagei.mosh_stagei(frames, cfg, marker_meta=case['marker_meta'])
-        else:
-            sys.path.insert(0, os.path.join(ROOT, 'tests'))
-            from test_stagei_reference_options import oracle_result
-            from test_stagei_robust import RobustBody
-            ref = oracle_result(type('RobustAt', (RobustBody,), {'sigma': a.robust_data_sigma})(frames, cfg, case['marker_meta']))
+        ref = ostagei.mosh_stagei(frames, cfg, marker_meta=case['marker_meta'], **kw)
         line['oracle_seconds'] = time.perf_counter() - t0
         line['oracle_stats'] = ref['stagei_debug_details']['oracle_stats']
         line['d_betas'] = float(np.abs(out['betas'] - ref['betas']).max())
         line['d_latent'] = float(np.abs(out['markers_latent'] - ref['markers_latent']).max())
         line['d_pose'] = float(max(np.abs(p - q).max() for p, q in zip(out['stagei_debug_details']['opt_models_pose'],
                                                                         ref['stagei_debug_details']['opt_models_pose'])))
+        if 'opt_models_expression' in ref['stagei_debug_details']:
+            line['d_expr'] = float(max(np.abs(p - q).max() for p, q in zip(out['stagei_debug_details']['opt_models_expression'],
+                                                                            ref['stagei_debug_details']['opt_models_expression'])))
     print(json.dumps(line))
 
 
