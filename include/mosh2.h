@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MOSH2_VERSION 108
+#define MOSH2_VERSION 109
 
 enum {
     MOSH2_OK = 0,
@@ -231,6 +231,21 @@ int mosh2_job_boundary_deltas(mosh2_job *j, int32_t body_ids, float *out);
  * a crossing must start on that branch, u (theta + 2 pi turns), to solve the sequential pass's problem.  async */
 int mosh2_job_relaunch_chunks(mosh2_job *j, int32_t n, const int32_t *chunk_ids, int32_t chunk_warmup, int32_t warmup_full,
                               double merge_tol, const int32_t *root_turns);
+/* One sweep of the joint minimisation of the sequence objective over the rows the job holds (DESIGN.md section 11).  The
+ * reference solves frame t with w (p_t - 2 p_{t-1} + p_{t-2}) and 6 (d_t - d_{t-1}) against the earlier frames held fixed
+ * (chmosh.py:584-724); the sum over the frames of those per-frame objectives, S, couples every processed frame (at least one
+ * visible marker) to its two processed neighbours on each side within its own sequence.  A sweep is three launches, one per
+ * colour k = 0, 1, 2 (mod 3) of the processed index k: every frame of a colour re-runs the reference's Step-2 dog-leg from its
+ * current row on its own terms plus every temporal residual that contains it, against its neighbours' current rows, and writes
+ * the row, markers_sim, errs and status flags back; counters add up.  Frames of one colour share no residual, so every launch
+ * lowers S.  After a sweep the velo / extrap_dmpl columns of errs hold the SSE of all temporal residuals that contain the frame
+ * (the residuals as the reference assigns them to frames are the caller's to recompute from the rows).  Call after a launch
+ * (and its repairs); max_delta [4] (may be NULL) receives the largest change of any processed frame's row during the sweep,
+ * per group as in mosh2_job_boundary_deltas (root + body pose, other pose coefficients, translation, dmpl / expressions).
+ * The stop rule is the caller's and covers every processed frame of the job: in a job of several sequences, all of them are swept
+ * until the caller stops.  MOSH2_E_INVALID before the job's first mosh2_job_launch (or after a mosh2_job_linearize).
+ * Synchronous. */
+int mosh2_job_sequence_sweep(mosh2_job *j, double *max_delta);
 int mosh2_job_download(mosh2_job *j, const mosh2_result *res); /* async D2H + stream sync */
 int mosh2_job_sync(mosh2_job *j);
 /* Results as ONE packed float32 device row per frame, for device-side consumers (NCCL gather): row f =

@@ -538,6 +538,83 @@ def with_robust_sigma(opts, robust_data_sigma):
     return o
 
 
+def check_sequence_sweeps(sequence_sweeps) -> Optional[int]:
+    """The ``sequence_sweeps`` keyword of the Stage-II entry points: None (off: the reference's causal solve) or an int >= 1,
+    the most sweeps of the joint minimisation of the sequence objective (``sequence_solve``)."""
+    if sequence_sweeps is None:
+        return None
+    if isinstance(sequence_sweeps, (bool, np.bool_)) or not isinstance(sequence_sweeps, (int, np.integer)) or sequence_sweeps < 1:
+        raise ValueError(f'sequence_sweeps must be None or an int >= 1, not {sequence_sweeps!r}')
+    return int(sequence_sweeps)
+
+
+def sequence_temporal_sse(pose: np.ndarray, dmpls: Optional[np.ndarray], wt_velo: float, wt_extrap: float, n_dm: int):
+    """The temporal residuals of the reference as it assigns them to the processed frames k = 0 .. F'-1 of one capture (rows in
+    processed order): velo_k = |wt_velo (p_k - 2 p_{k-1} + p_{k-2})|^2 for k >= 2 over the whole reduced pose, and with ``n_dm``
+    DMPL coefficients extrap_k = |wt_extrap (d_k - d_{k-1})|^2 for k >= 1 (chmosh.py:624-626,694-697; SURVEY.md App. B-1); zero
+    where the reference has no such term."""
+    n = len(pose)
+    velo, extrap = np.zeros(n), np.zeros(n)
+    if n > 2:
+        velo[2:] = wt_velo ** 2 * ((pose[2:] - 2.0 * pose[1:-1] + pose[:-2]) ** 2).sum(1)
+    if n_dm and dmpls is not None and n > 1:
+        d = dmpls[:, :n_dm]
+        extrap[1:] = wt_extrap ** 2 * ((d[1:] - d[:-1]) ** 2).sum(1)
+    return velo, extrap
+
+
+def sequence_objective(errs: np.ndarray, pose: np.ndarray, dmpls: Optional[np.ndarray], wt_velo: float, wt_extrap: float,
+                       n_dm: int) -> float:
+    """S of one capture (DESIGN.md section 11): the sum over its processed frames (rows in processed order) of the frame's own
+    Step-2 terms -- the errs columns data, poseB, poseH (or joint angles), dmpl, poseF, expr -- plus every temporal residual
+    (``sequence_temporal_sse``)."""
+    velo, extrap = sequence_temporal_sse(pose, dmpls, wt_velo, wt_extrap, n_dm)
+    return float(errs[:, [0, 1, 3, 4, 6, 7]].sum() + velo.sum() + extrap.sum())
+
+
+def sequence_solve(job, res, seq_ranges, opts, n_dm: int, max_sweeps: int, tol):
+    """Minimise the sequence objective S jointly, from the causal rows the job holds, by up to ``max_sweeps`` three-colour
+    sweeps (mosh2_job_sequence_sweep); stop once a sweep moves no processed frame by more than ``tol`` (per group, as
+    ``BOUNDARY_TOL``).  ``res``: the downloaded causal result (its buffers are the job's and are overwritten by the next
+    download).  ``seq_ranges``: the captures' [a, b) on the job's frame axis.  Returns the final ResultArrays, whose velo /
+    extrap_dmpl errs columns hold the residuals as the reference assigns them, and one ``sequence_solve`` record per capture.
+
+    The stop rule covers the whole launch: in a batch or multi-subject launch every capture is swept until no frame of ANY
+    capture moves by more than ``tol``, so ``sweeps``, ``converged`` and ``max_delta`` of each record are the launch's.  A
+    capture's result then equals its own call only once both have converged (further sweeps of a converged capture move it by
+    less than ``tol``); ``objective_causal`` and ``objective`` are the capture's own S."""
+    wv, wx = float(opts.wt_velo), float(opts.wt_extrap_dmpl)
+
+    def objectives(r):
+        out = []
+        for a, b in seq_ranges:
+            ok = (r.status[a:b] & _lib.ST_SOLVED) != 0
+            out.append(sequence_objective(r.errs[a:b][ok], r.pose[a:b][ok], r.dmpls[a:b][ok] if n_dm else None, wv, wx, n_dm))
+        return out
+
+    s_causal = objectives(res)
+    short = res.status & _lib.ST_SHORT_WARMUP
+    tol = np.asarray(tol, dtype=np.float64)
+    sweeps, converged, md, ms = 0, False, np.zeros(4), []
+    while sweeps < max_sweeps:
+        md = job.sequence_sweep()
+        ms.append(job.kernel_ms())
+        sweeps += 1
+        if (md <= tol).all():
+            converged = True
+            break
+    res = job.download()
+    res.status |= short
+    for a, b in seq_ranges:
+        fid = np.flatnonzero((res.status[a:b] & _lib.ST_SOLVED) != 0) + a
+        velo, extrap = sequence_temporal_sse(res.pose[fid], res.dmpls[fid] if n_dm else None, wv, wx, n_dm)
+        res.errs[fid, 2] = velo
+        res.errs[fid, 5] = extrap if n_dm else 0.0
+    s_joint = objectives(res)
+    return res, [dict(sweeps=sweeps, converged=converged, objective_causal=sc, objective=sj, max_delta=md.tolist(), sweep_ms=list(ms))
+                 for sc, sj in zip(s_causal, s_joint)]
+
+
 def _subject(seqs, cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname, device: int,
              subject_cache: bool = True, robust_data_sigma=None) -> dict:
     """A subject of a launch: its captures ``seqs`` (``_read_capture``) with its pack, options, flags and device model from
@@ -597,7 +674,7 @@ class _SeqResult:
         self.nd = res.nd
 
 
-def _solve_launch(subs, sched: dict, t0: float, laps: Optional[_Laps] = None):
+def _solve_launch(subs, sched: dict, t0: float, laps: Optional[_Laps] = None, sequence_sweeps: Optional[int] = None):
     """One verified launch of the captures of the subjects ``subs`` (``_subject``), back to back on the job's frame axis in
     the order given: a batch job of the subject's model (mosh2_job_create_batch) for one subject, a multi-model job
     (mosh2_job_create_multi) for several.  ``sched``: ``_resolve_schedule``.  Every capture uploads its own raw marker table
@@ -605,7 +682,9 @@ def _solve_launch(subs, sched: dict, t0: float, laps: Optional[_Laps] = None):
 
     Returns the per-capture dictionaries, in frame-axis order, each with the capture's own ``b200`` entries (status, counters,
     frame ids, adapter), and the figures of the launch (device time, chunks, schedule, boundary check, totals).  Sets the
-    ``offset`` of every capture record on the frame axis.  ``laps``: the host-time laps of ``mosh_stageii``."""
+    ``offset`` of every capture record on the frame axis.  ``laps``: the host-time laps of ``mosh_stageii``.
+    ``sequence_sweeps``: None, or the sweep cap of ``sequence_solve``, run on the launch's result (tolerance: the mode's
+    ``BOUNDARY_TOL``); its record goes to every capture's ``b200['sequence_solve']``."""
     laps = laps or _Laps()
     seqs = [(sub, s) for sub in subs for s in sub['seqs']]
     counts = [s['F'] for _, s in seqs]
@@ -652,6 +731,11 @@ def _solve_launch(subs, sched: dict, t0: float, laps: Optional[_Laps] = None):
 
             bad, report = launch_verified(job, sched['tol'], while_running=host_side)
             res = download_verified(job, bad, report)
+            seq_records = None
+            if sequence_sweeps is not None:
+                n_dm = subs[0]['pk'].n_dmpl - subs[0]['pk'].n_expr if subs[0]['opts'].optimize_dynamics else 0
+                res, seq_records = sequence_solve(job, res, list(zip(offsets[:-1], offsets[1:])), subs[0]['opts'], n_dm,
+                                                  sequence_sweeps, BOUNDARY_TOL[sched['mode']])
             laps('solve_ms')
             laps.ms['overlapped_host_ms'] = side['ms']
             n_chunks, totals = job.num_chunks, job.totals()
@@ -681,6 +765,8 @@ def _solve_launch(subs, sched: dict, t0: float, laps: Optional[_Laps] = None):
         })
         if sub.get('robust_data_sigma') is not None:
             data['stageii_debug_details']['b200']['robust_data_sigma'] = sub['robust_data_sigma']
+        if seq_records is not None:
+            data['stageii_debug_details']['b200']['sequence_solve'] = seq_records[q]
         outs.append(data)
     laps('assemble_ms')
     n_fb = int(((res.status & _lib.ST_GN_FALLBACK) != 0).sum())
@@ -697,7 +783,8 @@ def mosh_stageii(mocap_fname: str, cfg, markers_latent: np.ndarray, latent_label
                  chunk_len: Optional[int] = None, chunk_warmup: Optional[int] = None, warmup_full: Optional[int] = None,
                  first_extra: Optional[int] = None, precision: Optional[str] = None, verify: bool = True, boundary_tol=None,
                  sm_budget: int = NUM_SMS, labels_map='general', subject_cache: bool = True,
-                 device_adapter: bool = True, robust_data_sigma: Optional[float] = None) -> dict:
+                 device_adapter: bool = True, robust_data_sigma: Optional[float] = None,
+                 sequence_sweeps: Optional[int] = None) -> dict:
     """Stage II of MoSh++ on one H100.  Positional arguments as in the reference (chmosh.py:458-459).
 
     Keyword-only extras.  ``mode``: 'fast' (default) = float32, chunked in time with a verified warm-up -- within
@@ -716,11 +803,18 @@ def mosh_stageii(mocap_fname: str, cfg, markers_latent: np.ndarray, latent_label
     e = sim - obs, in every dog-leg of every frame (warm-up and boundary repair included) but not in the first frame's
     Procrustes start.  ``stageii_errs['data']`` then reports the robust SSE, the value minimised; sigma is recorded in
     ``b200['robust_data_sigma']`` (absent without it).
+    ``sequence_sweeps``: None (default) = the reference's causal solve; an int >= 1 = then minimise the sum over the frames
+    of the reference's per-frame objectives, S, jointly by at most that many three-colour sweeps (DESIGN.md section 11,
+    ``sequence_solve``), stopping once a sweep moves no frame by more than the mode's ``BOUNDARY_TOL``.  ``fullpose``,
+    ``trans``, ``dmpls``, ``expression`` and ``markers_sim`` then come from the joint solution, ``stageii_errs['velo']`` /
+    ``['extrap_dmpl']`` report its temporal residuals as the reference assigns them to frames, and
+    ``b200['sequence_solve']`` holds sweeps, converged, objective_causal, objective, max_delta (absent without it).
     """
     t0 = time.time()
     laps = _Laps()
     _check_mode(mode)
     check_robust_sigma(robust_data_sigma)
+    check_sequence_sweeps(sequence_sweeps)
     cap = _read_capture(mocap_fname, cfg, latent_labels, labels_map, device_adapter)
     laps('read_mocap_ms')
     sub = _subject([cap], cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname, device, subject_cache,
@@ -729,7 +823,7 @@ def mosh_stageii(mocap_fname: str, cfg, markers_latent: np.ndarray, latent_label
     sched = _resolve_schedule(sub['pk'], mode, [cap['F']], chunk_len, chunk_warmup, warmup_full, first_extra, precision, verify,
                               boundary_tol, sm_budget)
     laps('dense_view_ms')
-    (data,), figures = _solve_launch([sub], sched, t0, laps)
+    (data,), figures = _solve_launch([sub], sched, t0, laps, check_sequence_sweeps(sequence_sweeps))
     if cap['raw_cols'] is not None:             # the table rows the selection spans (float64) and the column map
         h2d = ((cap['F'] - 1) * cap['sel'].step + 1) * cap['mocap'].raw.shape[1] * 24 + 4 * len(cap['labels'])
     else:
@@ -743,7 +837,7 @@ def mosh_stageii_batch(mocap_fnames, cfg, markers_latent: np.ndarray, latent_lab
                        chunk_warmup: Optional[int] = None, warmup_full: Optional[int] = None, first_extra: Optional[int] = None,
                        precision: Optional[str] = None, verify: bool = True, boundary_tol=None, sm_budget: int = NUM_SMS,
                        labels_map='general', subject_cache: bool = True, device_adapter: bool = True,
-                       robust_data_sigma: Optional[float] = None) -> list:
+                       robust_data_sigma: Optional[float] = None, sequence_sweeps: Optional[int] = None) -> list:
     """Stage II of several captures of ONE subject (one Stage-I result, one ``cfg`` apart from ``mocap.fname``) in one launch.
 
     Returns one dictionary per capture, in the order of ``mocap_fnames``: what ``mosh_stageii`` returns for that capture with
@@ -754,10 +848,13 @@ def mosh_stageii_batch(mocap_fnames, cfg, markers_latent: np.ndarray, latent_lab
     into its range of the job (mosh2_job_upload_markers_range); a capture whose labels own several columns or whose frame
     selection is not a forward range takes the host adapter, as in ``mosh_stageii``.  ``b200`` holds the capture's own
     status / counters / frame ids and, under ``'batch'``, the figures of the whole launch (device time, chunks, boundary
-    check, totals), marked ``'shared': True`` -- the same for every capture of the call."""
+    check, totals), marked ``'shared': True`` -- the same for every capture of the call.  ``sequence_sweeps`` as
+    in ``mosh_stageii``: the sweeps run over the whole launch, and no temporal residual crosses from one capture to the next.  The
+    stop rule is the launch's (``sequence_solve``): every capture's record holds the launch's sweeps and deltas."""
     t0 = time.time()
     _check_mode(mode)
     check_robust_sigma(robust_data_sigma)
+    check_sequence_sweeps(sequence_sweeps)
     seqs = [_read_capture(fn, cfg, latent_labels, labels_map, device_adapter) for fn in mocap_fnames]
     if not seqs:
         raise ValueError('no captures given')
@@ -766,7 +863,7 @@ def mosh_stageii_batch(mocap_fnames, cfg, markers_latent: np.ndarray, latent_lab
     counts = [s['F'] for s in seqs]
     sched = _resolve_schedule(sub['pk'], mode, counts, chunk_len, chunk_warmup, warmup_full, first_extra, precision, verify,
                               boundary_tol, sm_budget)
-    outs, figures = _solve_launch([sub], sched, t0)
+    outs, figures = _solve_launch([sub], sched, t0, sequence_sweeps=check_sequence_sweeps(sequence_sweeps))
     batch = {'shared': True, 'captures': len(seqs), 'frames': int(sum(counts)), **figures, 'subject_cache_hit': sub['cache_hit']}
     for q, (s, data) in enumerate(zip(seqs, outs)):
         data['stageii_debug_details']['b200'].update(batch=batch, batch_index=q, frame_offset=s['offset'])
@@ -806,7 +903,8 @@ def launch_groups(keys) -> list:
 def mosh_stageii_subjects(subjects, *, device: int = 0, mode: str = 'fast', chunk_len: Optional[int] = None,
                           chunk_warmup: Optional[int] = None, warmup_full: Optional[int] = None, first_extra: Optional[int] = None,
                           precision: Optional[str] = None, verify: bool = True, boundary_tol=None, sm_budget: int = NUM_SMS,
-                          labels_map='general', device_adapter: bool = True, robust_data_sigma: Optional[float] = None) -> list:
+                          labels_map='general', device_adapter: bool = True, robust_data_sigma: Optional[float] = None,
+                          sequence_sweeps: Optional[int] = None) -> list:
     """Stage II of the captures of SEVERAL subjects, with as few launches as their models allow.
 
     ``subjects``: dictionaries with ``cfg``, ``mocap_fnames`` and the subject's Stage-I outputs ``markers_latent``,
@@ -824,11 +922,12 @@ def mosh_stageii_subjects(subjects, *, device: int = 0, mode: str = 'fast', chun
 
     ``robust_data_sigma`` (as in ``mosh_stageii``) applies to every subject; a subject dictionary may carry its own
     ``robust_data_sigma``, which takes its place for that subject.  The value is part of the options, so subjects with
-    different values never share a launch."""
+    different values never share a launch.  ``sequence_sweeps`` (as in ``mosh_stageii``) applies to every launch of the call."""
     global SUBJECT_CACHE_SIZE
     t0 = time.time()
     _check_mode(mode)
     check_robust_sigma(robust_data_sigma)
+    check_sequence_sweeps(sequence_sweeps)
     subjects = list(subjects)
     for s in subjects:
         check_robust_sigma(s.get('robust_data_sigma', robust_data_sigma))
@@ -849,7 +948,7 @@ def mosh_stageii_subjects(subjects, *, device: int = 0, mode: str = 'fast', chun
             counts = [s['F'] for sub in group for s in sub['seqs']]
             sched = _resolve_schedule(group[0]['pk'], mode, counts, chunk_len, chunk_warmup, warmup_full, first_extra, precision,
                                       verify, boundary_tol, sm_budget)
-            outs, figures = _solve_launch(group, sched, t0)
+            outs, figures = _solve_launch(group, sched, t0, sequence_sweeps=check_sequence_sweeps(sequence_sweeps))
             batch = {'shared': True, 'launch': g, 'launches': len(groups), 'subjects': len(group), 'captures': len(counts),
                      'frames': int(sum(counts)), **figures, 'subject_cache_hits': [sub['cache_hit'] for sub in group]}
             seqs = [(k, i, s) for k, i in enumerate(members) for s in subs[i]['seqs']]

@@ -114,7 +114,7 @@ using mosh2_host::plan_workspace;
 #endif
 template <class real> constexpr int threads_for() { return sizeof(real) == 4 ? MOSH2_F32_THREADS : 256; }
 
-template <class real, bool BIG>
+template <class real, bool BIG, bool SWEEP = false>
 __global__ void __launch_bounds__(threads_for<real>(), 1)
 mosh2_stageii_kernel(const __grid_constant__ mosh2::Model<real> m, const __grid_constant__ mosh2::Job<real> job,
                      const __grid_constant__ mosh2::Work<real, BIG> w, const __grid_constant__ mosh2::Dims d) {
@@ -126,7 +126,7 @@ mosh2_stageii_kernel(const __grid_constant__ mosh2::Model<real> m, const __grid_
         __syncthreads();
     }
     mosh2::Cta c{int(threadIdx.x), int(blockDim.x)};
-    mosh2::Solver<real, BIG> s(m, job, w, d, c);
+    mosh2::Solver<real, BIG, SWEEP> s(m, job, w, d, c);
     s.run_chunk(job.chunk_ids ? job.chunk_ids[blockIdx.x] : int(blockIdx.x));
 }
 
@@ -134,7 +134,7 @@ mosh2_stageii_kernel(const __grid_constant__ mosh2::Model<real> m, const __grid_
 // kernel shape, so `w` and `d` serve every chunk.  The block copies its chunk's Model record from the device array `models`
 // into the shared-memory header (mosh2_host::multi_smem_header, behind the global-workspace base) and binds its Solver to
 // that copy; the Solver stages that model's tables (Model::stage_blob) as in the single-model kernel.
-template <class real, bool BIG>
+template <class real, bool BIG, bool SWEEP = false>
 __global__ void __launch_bounds__(threads_for<real>(), 1)
 mosh2_stageii_multi_kernel(const mosh2::Model<real> *__restrict__ models, const int *__restrict__ model_of_chunk,
                            const __grid_constant__ mosh2::Job<real> job, const __grid_constant__ mosh2::Work<real, BIG> w,
@@ -150,7 +150,7 @@ mosh2_stageii_multi_kernel(const mosh2::Model<real> *__restrict__ models, const 
     if (BIG && threadIdx.x == 0) *reinterpret_cast<char **>(mosh2::m2_smem()) = job.gws + size_t(blockIdx.x) * job.gws_stride;
     __syncthreads();
     mosh2::Cta c{int(threadIdx.x), int(blockDim.x)};
-    mosh2::Solver<real, BIG> s(*rec, job, w, d, c);
+    mosh2::Solver<real, BIG, SWEEP> s(*rec, job, w, d, c);
     s.run_chunk(chunk);
 }
 
@@ -345,29 +345,39 @@ struct mosh2_job {
     std::vector<unsigned char> h_models;
     void *d_models = nullptr;
     int *d_model_of_chunk = nullptr;
+    std::vector<int> model_of_frame;             // multi-model job: model index of every frame (sequence sweeps)
+    int *d_model_of_frame = nullptr;
+    // sequence sweep (mosh2_job_sequence_sweep): neighbour table, the frames of the three colours back to back, per-frame deltas;
+    // `seq_ids` points at the frames of the current launch.  gws_slots: per-CTA global workspaces allocated (BIG layout).
+    int *d_seq_nbr = nullptr, *d_seq_ids = nullptr;
+    const int *seq_ids = nullptr;
+    double *d_seq_delta = nullptr;
+    size_t gws_slots = 0;
+    bool ev0_held = false;                       // a sweep times its three launches as one
+    bool launched = false;                       // mosh2_job_launch has run: status and rows hold a solve (a sweep needs them)
     size_t n_obs = 0, n_out = 0;
     size_t o_fullpose = 0, o_pose = 0, o_trans = 0, o_dmpls = 0, o_mk = 0, o_errs = 0;   // element offsets in d_out
 };
 
 namespace {
 
-template <class real, bool BIG>
+template <class real, bool BIG, bool SWEEP>
 cudaError_t launch_kernel(mosh2_job *j, const mosh2::Model<real> &m, const mosh2::Job<real> &job, int threads) {
     const mosh2_host::Layout<real, BIG> L = mosh2_host::layout<real, BIG>(m, mosh2::kSmemHeader);
-    const cudaError_t e = cudaFuncSetAttribute(mosh2_stageii_kernel<real, BIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(j->smem));
+    const cudaError_t e = cudaFuncSetAttribute(mosh2_stageii_kernel<real, BIG, SWEEP>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(j->smem));
     if (e != cudaSuccess) return e;
-    mosh2_stageii_kernel<real, BIG><<<j->launch_blocks, threads, j->smem, j->stream>>>(m, job, L.w, L.d);
+    mosh2_stageii_kernel<real, BIG, SWEEP><<<j->launch_blocks, threads, j->smem, j->stream>>>(m, job, L.w, L.d);
     return cudaGetLastError();
 }
 
-template <class real, bool BIG>
+template <class real, bool BIG, bool SWEEP>
 cudaError_t launch_multi_kernel(mosh2_job *j, const mosh2::Job<real> &job, int threads) {
     const mosh2::Model<real> &m = *reinterpret_cast<const mosh2::Model<real> *>(j->h_models.data());
     const mosh2_host::Layout<real, BIG> L = mosh2_host::layout<real, BIG>(m, mosh2_host::multi_smem_header<real>());
-    const cudaError_t e = cudaFuncSetAttribute(mosh2_stageii_multi_kernel<real, BIG>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(j->smem));
+    const cudaError_t e = cudaFuncSetAttribute(mosh2_stageii_multi_kernel<real, BIG, SWEEP>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(j->smem));
     if (e != cudaSuccess) return e;
-    mosh2_stageii_multi_kernel<real, BIG><<<j->launch_blocks, threads, j->smem, j->stream>>>(
-        static_cast<const mosh2::Model<real> *>(j->d_models), j->d_model_of_chunk, job, L.w, L.d);
+    mosh2_stageii_multi_kernel<real, BIG, SWEEP><<<j->launch_blocks, threads, j->smem, j->stream>>>(
+        static_cast<const mosh2::Model<real> *>(j->d_models), j->lin_mode == 3 ? j->d_model_of_frame : j->d_model_of_chunk, job, L.w, L.d);
     return cudaGetLastError();
 }
 
@@ -386,19 +396,27 @@ int launch(mosh2_job *j, const mosh2::Model<real> &m) {
     job.status = j->d_status; job.counters = j->d_counters; job.totals = j->d_totals; job.prof = j->d_prof;
     job.gws = static_cast<char *>(j->d_gws); job.gws_stride = j->gws_stride;
     job.lin_mode = j->lin_mode; job.lin_step = j->lin_step;
-    if (j->lin_mode) mosh2_host::bind_lin(job, static_cast<real *>(j->d_lin), j->lin);
+    if (j->lin_mode == 1 || j->lin_mode == 2) mosh2_host::bind_lin(job, static_cast<real *>(j->d_lin), j->lin);
+    if (j->lin_mode == 3) {                      // sequence sweep: one block per frame of the colour; no chunk records
+        job.chunk_ids = j->seq_ids;
+        job.seq_nbr = j->d_seq_nbr; job.seq_delta = j->d_seq_delta;
+        job.warm_x = nullptr; job.warm_f = nullptr;
+    }
     job.opt = j->opt;
     int threads = threads_for<real>();
     if (const char *e = getenv("MOSH2_DEV_THREADS")) {      // development aid: any multiple of 32 from 128 up to the launch bound
         const int t = atoi(e);
         if (t >= 128 && t <= threads && t % 32 == 0) threads = t;
     }
-    CU(cudaEventRecord(j->ev0, j->stream));
+    if (!j->ev0_held) CU(cudaEventRecord(j->ev0, j->stream));
+    const bool sweep = j->lin_mode == 3;         // (the sequence sweep is a kernel of its own: the causal one is compiled without it)
     if (j->d_models) {
-        if (j->big_in_global) CU((launch_multi_kernel<real, true>(j, job, threads)));
-        else CU((launch_multi_kernel<real, false>(j, job, threads)));
-    } else if (j->big_in_global) CU((launch_kernel<real, true>(j, m, job, threads)));
-    else CU((launch_kernel<real, false>(j, m, job, threads)));
+        if (sweep) CU(j->big_in_global ? (launch_multi_kernel<real, true, true>(j, job, threads)) : (launch_multi_kernel<real, false, true>(j, job, threads)));
+        else if (j->big_in_global) CU((launch_multi_kernel<real, true, false>(j, job, threads)));
+        else CU((launch_multi_kernel<real, false, false>(j, job, threads)));
+    } else if (sweep) CU(j->big_in_global ? (launch_kernel<real, true, true>(j, m, job, threads)) : (launch_kernel<real, false, true>(j, m, job, threads)));
+    else if (j->big_in_global) CU((launch_kernel<real, true, false>(j, m, job, threads)));
+    else CU((launch_kernel<real, false, false>(j, m, job, threads)));
     CU(cudaGetLastError());
     CU(cudaEventRecord(j->ev1, j->stream));
     return 0;
@@ -444,6 +462,65 @@ int linearize(mosh2_job *j, const mosh2::Model<real> &m, int32_t step, int32_t b
     CU(cudaStreamSynchronize(j->stream));
     for (const Back &e : b)
         if (e.dst) for (size_t i = 0; i < e.cnt; ++i) e.dst[i] = double(e.h[i]);
+    return 0;
+}
+
+// Per-CTA global workspaces a BIG-layout sweep launch may use: two thread blocks per SM of an H100 SXM (132 SMs).  A colour with
+// more frames runs in launches of this many blocks; the job's own workspaces (one per chunk) are used if there are more of them.
+constexpr size_t kSweepGwsSlots = 2 * 132;
+
+// mosh2_job_sequence_sweep in the job's compute type: the neighbour table and the colours from the status of the last launch,
+// then one launch per colour (in batches of the per-CTA global workspaces there are, in the BIG layout), then the deltas
+template <class real>
+int sequence_sweep(mosh2_job *j, const mosh2::Model<real> &m, double *max_delta) {
+    const int F = j->n_frames, dv = j->model->device;
+    if (!j->d_seq_nbr) {
+        CU(g_blocks.get(dv, size_t(F) * 4 * sizeof(int), reinterpret_cast<void **>(&j->d_seq_nbr)));
+        CU(g_blocks.get(dv, size_t(F) * sizeof(int), reinterpret_cast<void **>(&j->d_seq_ids)));
+        CU(g_blocks.get(dv, size_t(F) * 4 * sizeof(double), reinterpret_cast<void **>(&j->d_seq_delta)));
+    }
+    CU(cudaMemcpyAsync(j->h_status, j->d_status, size_t(F) * sizeof(int), cudaMemcpyDeviceToHost, j->stream));
+    CU(cudaStreamSynchronize(j->stream));
+    std::vector<int> nbr, colour[3];
+    mosh2_host::sequence_tables(j->h_status, F, j->tab0, nbr, colour);
+    std::vector<int> ids;
+    size_t widest = 0;
+    for (const auto &c : colour) { ids.insert(ids.end(), c.begin(), c.end()); widest = std::max(widest, c.size()); }
+    CU(cudaMemcpy(j->d_seq_nbr, nbr.data(), nbr.size() * sizeof(int), cudaMemcpyHostToDevice));
+    if (!ids.empty()) CU(cudaMemcpy(j->d_seq_ids, ids.data(), ids.size() * sizeof(int), cudaMemcpyHostToDevice));
+    CU(cudaMemsetAsync(j->d_seq_delta, 0, size_t(F) * 4 * sizeof(double), j->stream));
+    size_t slots = widest;
+    if (j->gws_stride) {                         // BIG layout: one global workspace per block of a launch
+        slots = std::max(j->gws_slots, std::min(widest, kSweepGwsSlots));
+        if (slots > j->gws_slots) {
+            g_blocks.put(dv, j->d_gws);
+            j->d_gws = nullptr; j->gws_slots = 0;
+            CU(g_blocks.get(dv, j->gws_stride * slots, &j->d_gws));
+            j->gws_slots = slots;
+        }
+    }
+    j->lin_mode = 3;
+    int rc = 0;
+    size_t off = 0;
+    for (int c = 0; c < 3 && !rc; ++c) {
+        for (size_t b = 0; b < colour[c].size() && !rc; b += slots) {
+            j->seq_ids = j->d_seq_ids + off + b;
+            j->launch_blocks = int(std::min(slots, colour[c].size() - b));
+            rc = launch<real>(j, m);
+            j->ev0_held = true;
+        }
+        off += colour[c].size();
+    }
+    j->lin_mode = 0; j->ev0_held = false; j->seq_ids = nullptr; j->launch_blocks = j->n_chunks;
+    if (rc) return rc;
+    std::vector<double> dl(size_t(F) * 4);
+    CU(cudaMemcpyAsync(dl.data(), j->d_seq_delta, dl.size() * sizeof(double), cudaMemcpyDeviceToHost, j->stream));
+    CU(cudaStreamSynchronize(j->stream));
+    if (max_delta) {
+        for (int q = 0; q < 4; ++q) max_delta[q] = 0;
+        for (int f = 0; f < F; ++f)
+            for (int q = 0; q < 4; ++q) max_delta[q] = std::max(max_delta[q], dl[size_t(f) * 4 + q]);
+    }
     return 0;
 }
 
@@ -572,6 +649,7 @@ int mosh2_job_create_batch(mosh2_model *m, const mosh2_options *opt, int32_t n_s
     if (e == cudaSuccess) chk(cudaMemcpy(j->d_chunk_tab, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice));
     chk(g_blocks.get(m->device, 32 * sizeof(long long), reinterpret_cast<void **>(&j->d_prof)));
     if (j->gws_stride) chk(g_blocks.get(m->device, j->gws_stride * j->n_chunks, reinterpret_cast<void **>(&j->d_gws)));
+    j->gws_slots = size_t(j->n_chunks);
     chk(g_blocks.get(-1, j->n_obs * j->esz, reinterpret_cast<void **>(&j->h_obs)));
     chk(g_blocks.get(-1, j->n_out * j->esz, reinterpret_cast<void **>(&j->h_out)));
     chk(g_blocks.get(-1, F * M, reinterpret_cast<void **>(&j->h_vis)));
@@ -610,6 +688,7 @@ int make_multi(mosh2_job *j, mosh2_model *const *models, int32_t n_models, int32
         CU(g_blocks.get(dv, stride * j->n_chunks, &j->d_gws));
     }
     j->smem = smem; j->big_in_global = big; j->gws_stride = stride;
+    j->gws_slots = size_t(j->n_chunks);
     std::vector<mosh2::Model<real>> recs(n_models);
     for (int k = 0; k < n_models; ++k) {
         recs[k] = dev_model(models[k]);
@@ -621,6 +700,10 @@ int make_multi(mosh2_job *j, mosh2_model *const *models, int32_t n_models, int32
     CU(g_blocks.get(dv, moc.size() * sizeof(int), reinterpret_cast<void **>(&j->d_model_of_chunk)));
     CU(cudaMemcpy(j->d_models, j->h_models.data(), j->h_models.size(), cudaMemcpyHostToDevice));
     CU(cudaMemcpy(j->d_model_of_chunk, moc.data(), moc.size() * sizeof(int), cudaMemcpyHostToDevice));
+    j->model_of_frame.clear();
+    for (int q = 0; q < n_seq; ++q) j->model_of_frame.insert(j->model_of_frame.end(), size_t(frame_counts[q]), model_of_seq[q]);
+    CU(g_blocks.get(dv, j->model_of_frame.size() * sizeof(int), reinterpret_cast<void **>(&j->d_model_of_frame)));
+    CU(cudaMemcpy(j->d_model_of_frame, j->model_of_frame.data(), j->model_of_frame.size() * sizeof(int), cudaMemcpyHostToDevice));
     j->models.assign(models, models + n_models);
     return 0;
 }
@@ -750,6 +833,7 @@ int mosh2_job_linearize(mosh2_job *j, const mosh2_options *opt, int32_t step, in
     if (opt && !mosh2_host::robust_sigma_ok(*opt)) return fail(MOSH2_E_INVALID, "robust_sigma must be 0 (off) or a finite sigma > 0");
     CU(cudaSetDevice(j->model->device));
     if (opt) mosh2_host::apply_call_weights(j->opt, *opt);
+    j->launched = false;                          // (the linearisation clears the rows)
     if (j->precision == MOSH2_F64) return linearize<double>(j, j->model->f64.m, step, build, x, out);
     return linearize<float>(j, j->model->f32.m, step, build, x, out);
 }
@@ -769,6 +853,7 @@ int mosh2_job_launch(mosh2_job *j) {
     }
     j->subset = false;
     j->launch_blocks = j->n_chunks;
+    j->launched = true;
     if (j->precision == MOSH2_F64) return launch<double>(j, j->model->f64.m);
     return launch<float>(j, j->model->f32.m);
 }
@@ -795,6 +880,14 @@ int mosh2_job_relaunch_chunks(mosh2_job *j, int32_t n, const int32_t *chunk_ids,
     j->launch_blocks = n;
     if (j->precision == MOSH2_F64) return launch<double>(j, j->model->f64.m);
     return launch<float>(j, j->model->f32.m);
+}
+
+int mosh2_job_sequence_sweep(mosh2_job *j, double *max_delta) {
+    if (!j) return fail(MOSH2_E_INVALID, "null job");
+    if (!j->launched) return fail(MOSH2_E_INVALID, "mosh2_job_sequence_sweep needs a solve of the job first (mosh2_job_launch)");
+    CU(cudaSetDevice(j->model->device));
+    if (j->precision == MOSH2_F64) return sequence_sweep<double>(j, j->model->f64.m, max_delta);
+    return sequence_sweep<float>(j, j->model->f32.m, max_delta);
 }
 
 int mosh2_job_boundary_deltas(mosh2_job *j, int32_t body_ids, float *out) {
@@ -967,6 +1060,10 @@ void mosh2_job_destroy(mosh2_job *j) {
     g_blocks.put(dv, j->d_lin);
     g_blocks.put(dv, j->d_models);
     g_blocks.put(dv, j->d_model_of_chunk);
+    g_blocks.put(dv, j->d_model_of_frame);
+    g_blocks.put(dv, j->d_seq_nbr);
+    g_blocks.put(dv, j->d_seq_ids);
+    g_blocks.put(dv, j->d_seq_delta);
     for (void *p : {j->h_obs, j->h_out, static_cast<void *>(j->h_vis), static_cast<void *>(j->h_status), static_cast<void *>(j->h_counters)})
         g_blocks.put(-1, p);
     for (auto &s : j->range_slots) {        // (the stream is idle: every slot's copy and kernel have finished)

@@ -192,6 +192,11 @@ struct Job {
     real *lin_A, *lin_g;    // [F][n][n], [F][n]: normal equations of the frame's own terms (data, pose prior, fingers)
     real *lin_J, *lin_r;    // [F][3M][n], [F][3M]: weighted data rows d r / d x_free and r = (sim - obs) wd (zero where invisible)
     real *lin_vp;           // [F][3M][3]: posed attachment vertices (slot = 3 marker + t)
+    // Sequence sweep (lin_mode == 3, mosh2_job_sequence_sweep): the block's "chunk" is a processed frame f (chunk_ids lists the
+    // frames of one colour).  Step 2 of f runs again from f's emitted row, with every second difference of the reduced pose and
+    // every first difference of the DMPL coefficients that contains f taken against its neighbours' rows; the row goes back.
+    const int *seq_nbr;     // [F][4] processed-order neighbours: two before, one before, one after, two after (-1: none)
+    double *seq_delta;      // [F][4] max |new - old| of the row: root+body pose, other pose coefficients, translation, linear block
     Options opt;
 };
 
@@ -657,7 +662,8 @@ struct StepCfg {
 // ---------------------------------------------------------------------------------------------
 // the solver
 // ---------------------------------------------------------------------------------------------
-template <class real, bool BIG = false>
+// SWEEP: the sequence-sweep instantiation (Job::lin_mode == 3, its own kernel): the causal program is compiled without it
+template <class real, bool BIG = false, bool SWEEP = false>
 struct Solver {
     const Model<real> &m;
     const Job<real> &job;
@@ -677,6 +683,7 @@ struct Solver {
     int root_turns = 0;       // full turns added to the angle of the cold start's root (run_chunk, procrustes)
     real resume_diff = 0;     // ... and how far the frame just solved is from the row it replaces
     int lin_f = -1;           // linearise mode: the frame this block works on (else -1)
+    real seq_cv = 0, seq_cx = 0;   // sequence sweep: the constants of the collapsed temporal terms (sequence_terms)
 
     M2_D Solver(const Model<real> &m_, const Job<real> &j_, const Work<real, BIG> &w_, const Dims &d_, Cta c_)
         : m(m_), job(j_), w(w_), cta(c_), d(d_) {}
@@ -1076,6 +1083,10 @@ struct Solver {
             }
             w.isc[0] = ks;
             part[ERR_POSEB] = sp;
+            if (SWEEP) {                      // sequence sweep: the SSE of the temporal residuals themselves, not of the collapsed form
+                if (c.velo) part[ERR_VELO] += seq_cv;
+                if (c.extrap) part[ERR_EXTRAP] += seq_cx;
+            }
             real tot = 0;
             for (int i = 0; i < N_ERR; ++i) { w.sc[1 + i] = part[i]; tot += part[i]; }
             w.sc[0] = tot;
@@ -2257,7 +2268,8 @@ struct Solver {
         const real e1 = real(1e-15), e2 = real(1e-15);
         enum { OP_PROCRUSTES, OP_BEGIN, OP_TRIAL, OP_OUTPUT };
         int op = first ? OP_PROCRUSTES : OP_BEGIN;
-        int stage = first ? 0 : (light ? 4 : 3);   // 0..2 first-frame annealing (chmosh.py:637-653), 3 Step 1 (665-671), 4 Step 2 (676-705)
+        // 0..2 first-frame annealing (chmosh.py:637-653), 3 Step 1 (665-671), 4 Step 2 (676-705); a sequence sweep runs Step 2 only
+        int stage = first ? 0 : (light || SWEEP ? 4 : 3);
         if (lin_f >= 0) stage = job.lin_step == 2 ? 4 : 3;      // linearise mode: the stage names the free-variable list
         const int maxit = light ? 1 : o.maxiter;
         StepCfg<real> c;
@@ -2462,6 +2474,19 @@ struct Solver {
             cta_max(dm);
             resume_diff = dm[0];
         }
+        if (SWEEP && emit) {
+            // sequence sweep: how far the frame moved, per group of chmosh.BOUNDARY_TOL (the stop rule of the sweeps)
+            real dm[4] = {0, 0, 0, 0};
+            const int nbody = m.body_dof < 66 ? m.body_dof : 66;
+            CTA_FOR(i, d.PR) {
+                const real e = r_abs(w.x[3 + i] - job.pose[size_t(f) * d.PR + i]);
+                if (i < nbody) dm[0] = e > dm[0] ? e : dm[0]; else dm[1] = e > dm[1] ? e : dm[1];
+            }
+            CTA_FOR(i, 3) { const real e = r_abs(w.x[i] - job.trans[size_t(f) * 3 + i]); dm[2] = e > dm[2] ? e : dm[2]; }
+            if (job.dmpls) CTA_FOR(i, d.nd) { const real e = r_abs(w.x[3 + d.PR + i] - job.dmpls[size_t(f) * d.nd + i]); dm[3] = e > dm[3] ? e : dm[3]; }
+            for (int q = 0; q < 4; ++q) cta_max(dm + q);
+            if (cta.tid == 0) for (int q = 0; q < 4; ++q) job.seq_delta[4 * size_t(f) + q] = double(dm[q]);
+        }
         if (emit) {
             CTA_FOR(i, d.PF) job.fullpose[size_t(f) * d.PF + i] = w.fullpose[i];
             CTA_FOR(i, d.PR) job.pose[size_t(f) * d.PR + i] = w.x[3 + i];
@@ -2469,7 +2494,15 @@ struct Solver {
             if (job.dmpls) CTA_FOR(i, d.nd) job.dmpls[size_t(f) * d.nd + i] = w.x[3 + d.PR + i];
             CTA_FOR(i, 3 * d.M) job.markers_sim[size_t(f) * 3 * d.M + i] = w.mk[i];
             CTA_FOR(i, N_ERR) job.errs[size_t(f) * N_ERR + i] = w.sc[1 + i];
-            if (cta.tid == 0) {
+            if (SWEEP && cta.tid == 0) {
+                // sequence sweep: the causal pass's velocity / extrapolation bits stay (they say which frames the reference
+                // gives those terms); the counters add up over the causal pass and every sweep
+                job.status[f] |= frame_flags;
+                job.counters[4 * f + 0] += n_iter;
+                job.counters[4 * f + 1] += n_eval;
+                job.counters[4 * f + 2] += n_build;
+                job.counters[4 * f + 3] += n_min;
+            } else if (cta.tid == 0) {
                 job.status[f] = ST_SOLVED | frame_flags | (has_velo ? ST_HAS_VELO : 0) | (has_extrap ? ST_HAS_EXTRAP : 0);
                 job.counters[4 * f + 0] = n_iter;
                 job.counters[4 * f + 1] = n_eval;
@@ -2624,6 +2657,49 @@ struct Solver {
         stage_tables(1);
     }
 
+    // ---- sequence sweep (Job::lin_mode == 3): frame f's state from its emitted row, and its temporal terms against the rows of
+    //      its processed-order neighbours.  The second differences w (p_j - 2 p_{j-1} + p_{j-2}) that contain p_f are
+    //      w (a_j p_f + b_j), a = 1, -2, 1 for j = f, f+1, f+2; their sum of squares is w^2 A |p_f - t|^2 + w^2 sum_j |a_j t + b_j|^2
+    //      with A = sum a_j^2 and t = -sum a_j b_j / A.  So the velocity term of Step 2 runs with weight w sqrt(A) and target t,
+    //      and eval() adds the constant: the dog-leg's relative stop rule (e_3) must see the true SSE.  The same for the DMPL
+    //      differences 6 (d_j - d_{j-1}), j = f, f+1 (a = 1, -1).
+    M2_D void sequence_terms(int f, bool dyn) {
+        const Options &o = job.opt;
+        const int *nb = job.seq_nbr + 4 * size_t(f);
+        const int p2 = nb[0], p1 = nb[1], n1 = nb[2], n2 = nb[3];
+        CTA_FOR(i, 3) w.x[i] = job.trans[size_t(f) * 3 + i];
+        CTA_FOR(i, d.PR) w.x[3 + i] = job.pose[size_t(f) * d.PR + i];
+        if (job.dmpls) CTA_FOR(i, d.nd) w.x[3 + d.PR + i] = job.dmpls[size_t(f) * d.nd + i];
+        const bool r0 = p1 >= 0 && p2 >= 0, r1 = p1 >= 0 && n1 >= 0, r2 = n1 >= 0 && n2 >= 0;
+        const int av = (r0 ? 1 : 0) + (r1 ? 4 : 0) + (r2 ? 1 : 0), ad = (p1 >= 0 ? 1 : 0) + (n1 >= 0 ? 1 : 0);
+        has_velo = av > 0;
+        has_extrap = dyn && ad > 0;
+        real cst[2] = {0, 0};
+        if (has_velo) CTA_FOR(i, d.PR) {
+            const real *P = job.pose + i;
+            const real b0 = r0 ? P[size_t(p2) * d.PR] - real(2) * P[size_t(p1) * d.PR] : real(0);
+            const real b1 = r1 ? P[size_t(p1) * d.PR] + P[size_t(n1) * d.PR] : real(0);
+            const real b2 = r2 ? P[size_t(n2) * d.PR] - real(2) * P[size_t(n1) * d.PR] : real(0);
+            const real t = (real(2) * b1 - b0 - b2) / real(av);
+            w.velo_tgt[i] = t;
+            const real e0 = r0 ? t + b0 : real(0), e1 = r1 ? b1 - real(2) * t : real(0), e2 = r2 ? t + b2 : real(0);
+            cst[0] += e0 * e0 + e1 * e1 + e2 * e2;
+        }
+        if (has_extrap) CTA_FOR(i, d.nd - m.n_expr) {
+            const real dp = p1 >= 0 ? job.dmpls[size_t(p1) * d.nd + i] : real(0), dn = n1 >= 0 ? job.dmpls[size_t(n1) * d.nd + i] : real(0);
+            const real t = (dp + dn) / real(ad);
+            w.dm_tgt[i] = t;
+            const real e0 = p1 >= 0 ? t - dp : real(0), e1 = n1 >= 0 ? dn - t : real(0);
+            cst[1] += e0 * e0 + e1 * e1;
+        }
+        cta_reduce<real, 2>(cta, cst, w.red);
+        wv = real(o.wt_velo) * r_sqrt(real(av));
+        wex = real(o.wt_extrap) * r_sqrt(real(ad));
+        seq_cv = real(o.wt_velo) * real(o.wt_velo) * cst[0];
+        seq_cx = real(o.wt_extrap) * real(o.wt_extrap) * cst[1];
+        M2_SYNC();
+    }
+
     M2_D void run_chunk(int chunk) {
         const Options &o = job.opt;
         // Linearise mode (Stage I, Job::lin_mode): the block's "chunk" is the single frame `chunk`, taken at the state the
@@ -2632,13 +2708,14 @@ struct Solver {
         // optimize_face, the jaw (poseF) and expression terms -- under the weights of the options as they are (no per-frame
         // visibility scaling: chmosh.py:327,350; the expression weight is never visibility-scaled).  It runs through the
         // same frame loop and the same solve_frame call as a chunk (one call site each: instruction cache, DESIGN.md 3).
-        const bool lin = job.lin_mode != 0;
+        const bool lin = !SWEEP && job.lin_mode != 0, one = lin || SWEEP;
         // chunk table (host-built, mosh2_host::chunk_table): the chunk emits frames [f_emit, f_end) of the sequence that
-        // starts at frame s0 of the job's frame axis (a job may hold several sequences of one subject back to back)
+        // starts at frame s0 of the job's frame axis (a job may hold several sequences of one subject back to back).  Linearise
+        // mode and the sequence sweep work on the single frame `chunk`.
         const int *rec = job.chunk_tab + kChunkRec * chunk;
-        const int f_emit = lin ? chunk : rec[0], f_end = lin ? chunk + 1 : rec[1], s0 = lin ? chunk : rec[2];
-        const int warmup = lin ? 0 : rec[3], warm_full = lin ? 0 : rec[4];
-        root_turns = lin ? 0 : rec[5];
+        const int f_emit = one ? chunk : rec[0], f_end = one ? chunk + 1 : rec[1], s0 = one ? chunk : rec[2];
+        const int warmup = one ? 0 : rec[3], warm_full = one ? 0 : rec[4];
+        root_turns = one ? 0 : rec[5];
         int f_begin = f_emit, f_full = f_emit;
         bool short_warmup = false;
         if (cta.tid == 0 && job.warm_f) job.warm_f[chunk] = -1;
@@ -2765,6 +2842,10 @@ struct Solver {
             }
             has_extrap = dyn && have_dm_prev;
             if (short_warmup && f >= f_emit) frame_flags |= ST_SHORT_WARMUP;
+            if (SWEEP) {
+                sequence_terms(f, dyn);
+                first = false;
+            }
             if (lin) {
                 lin_f = f;
                 CTA_FOR(i, d.NX) w.x[i] = job.lin_x[size_t(f) * d.NX + i];

@@ -358,6 +358,35 @@ void bind_lin(mosh2::Job<real> &job, real *p, const LinLayout &L) {
     job.lin_x = p + L.x; job.lin_A = p + L.A; job.lin_g = p + L.g; job.lin_J = p + L.J; job.lin_r = p + L.r; job.lin_vp = p + L.vp;
 }
 
+// ---- sequence sweep (mosh2_job_sequence_sweep) ----------------------------------------------------------------------------------
+// The processed frames of a job (status has MOSH2_ST_SOLVED: at least one visible marker) in the processed order of their own
+// sequence, from the status of the last launch and the chunk table `tab` (chunk_table; field 2 of a record is the first frame of
+// the chunk's sequence).  nbr [F][4]: the two processed frames before and the two after each frame, -1 where the sequence ends
+// first (skipped frames are passed over, sequences never neighbour each other).  colour[c]: the processed frames with processed
+// index k = c (mod 3) within their sequence -- frames of one colour share no temporal residual.
+inline void sequence_tables(const int *status, int n_frames, const std::vector<int> &tab, std::vector<int> &nbr,
+                            std::vector<int> colour[3]) {
+    std::vector<int> seq_start(n_frames, 0);
+    for (size_t c = 0; c < tab.size() / mosh2::kChunkRec; ++c)
+        for (int f = tab[c * mosh2::kChunkRec]; f < tab[c * mosh2::kChunkRec + 1]; ++f) seq_start[f] = tab[c * mosh2::kChunkRec + 2];
+    nbr.assign(size_t(n_frames) * 4, -1);
+    for (int c = 0; c < 3; ++c) colour[c].clear();
+    std::vector<int> run;                                   // processed frames of the current sequence
+    for (int f = 0; f <= n_frames; ++f) {
+        if (f == n_frames || (f > 0 && seq_start[f] != seq_start[f - 1])) {
+            const int n = int(run.size());
+            for (int k = 0; k < n; ++k) {
+                int *q = &nbr[size_t(run[k]) * 4];
+                q[0] = k >= 2 ? run[k - 2] : -1; q[1] = k >= 1 ? run[k - 1] : -1;
+                q[2] = k + 1 < n ? run[k + 1] : -1; q[3] = k + 2 < n ? run[k + 2] : -1;
+                colour[k % 3].push_back(run[k]);
+            }
+            run.clear();
+        }
+        if (f < n_frames && (status[f] & MOSH2_ST_SOLVED)) run.push_back(f);
+    }
+}
+
 // ---- mosh2_job_upload_markers_range ---------------------------------------------------------------------------------------------
 // Argument checks of an upload of frames [frame0, frame0 + n) of a job of n_frames frames and M markers: 0, or MOSH2_E_INVALID
 // with the reason in *msg.

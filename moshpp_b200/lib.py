@@ -13,7 +13,7 @@ import numpy as np
 
 from .pack import StageIIPack
 
-ABI_VERSION = 108          # MOSH2_VERSION of include/mosh2.h that the ctypes structs below encode
+ABI_VERSION = 109          # MOSH2_VERSION of include/mosh2.h that the ctypes structs below encode
 MOSH2_F32, MOSH2_F64 = 0, 1
 ST_SOLVED, ST_SKIPPED, ST_HAS_VELO, ST_HAS_EXTRAP, ST_GN_FALLBACK, ST_MAXITER, ST_SHORT_WARMUP = 1, 2, 4, 8, 16, 32, 64
 ERR_NAMES = ('data', 'poseB', 'velo', 'poseH', 'dmpl', 'extrap_dmpl', 'poseF', 'expr')   # column order of mosh2_result.errs
@@ -132,6 +132,7 @@ def load_library(path: Optional[str] = None):
     lib.mosh2_job_warm_states.argtypes = [vp, _f64p, _i32p]
     lib.mosh2_job_boundary_deltas.argtypes = [vp, C.c_int32, C.POINTER(C.c_float)]
     lib.mosh2_job_relaunch_chunks.argtypes = [vp, C.c_int32, _i32p, C.c_int32, C.c_int32, C.c_double, _i32p]
+    lib.mosh2_job_sequence_sweep.argtypes = [vp, _f64p]
     lib.mosh2_job_download.argtypes = [vp, C.POINTER(Result)]
     lib.mosh2_job_sync.argtypes = [vp]
     lib.mosh2_job_kernel_ms.argtypes = [vp, C.POINTER(C.c_float)]
@@ -155,7 +156,8 @@ EXPORTED_SYMBOLS = (
     'mosh2_solve', 'mosh2_job_upload_device', 'mosh2_job_row_width', 'mosh2_job_download_device', 'mosh2_job_span_ms',
     'mosh2_job_create_batch', 'mosh2_job_upload_device_range', 'mosh2_job_warm_states', 'mosh2_job_relaunch_chunks',
     'mosh2_job_boundary_deltas', 'mosh2_release_cached_memory', 'mosh2_mesh_distance', 'mosh2_job_upload_markers', 'mosh2_job_linearize',
-    'mosh2_job_chunk_ranges', 'mosh2_job_upload_markers_range', 'mosh2_job_create_multi')
+    'mosh2_job_chunk_ranges', 'mosh2_job_upload_markers_range', 'mosh2_job_create_multi',
+    'mosh2_job_sequence_sweep')
 
 
 def _ptr(a: np.ndarray, typ):
@@ -431,6 +433,13 @@ class Job:
                                                              int(warmup_full), float(merge_tol),
                                                              None if turns is None else _ptr(turns, _i32p)),
                           'mosh2_job_relaunch_chunks')
+
+    def sequence_sweep(self) -> np.ndarray:
+        """One sweep of the joint minimisation of the sequence objective over the job's rows (mosh2_job_sequence_sweep); returns
+        the largest change of any processed frame's row, per group as in ``boundary_deltas``."""
+        out = np.zeros(4)
+        self.model._check(self.lib.mosh2_job_sequence_sweep(self.handle, _ptr(out, _f64p)), 'mosh2_job_sequence_sweep')
+        return out
 
     def download(self) -> ResultArrays:
         self.model._check(self.lib.mosh2_job_download(self.handle, C.byref(self.result.c)), 'mosh2_job_download')
