@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MOSH2_VERSION 109
+#define MOSH2_VERSION 110
 
 enum {
     MOSH2_OK = 0,
@@ -183,6 +183,23 @@ int mosh2_job_upload_markers(mosh2_job *j, const double *markers, int32_t n_file
 int mosh2_job_upload_markers_range(mosh2_job *j, int32_t frame0, int32_t n, const double *markers, int32_t n_file_frames, int32_t n_cols,
                                    const int32_t *col_of_marker, int32_t frame_start, int32_t frame_step, double unit_per_metre,
                                    const double *rot3x3);
+/* Held-out marker validation (DESIGN.md section 12): n_folds copies of ONE capture, each with some markers deleted, in the
+ * sequences [seq0, seq0 + n_folds) of a batch job (mosh2_job_create_batch; those sequences must have one frame count n).  The
+ * capture's raw marker table is staged once and one kernel writes every fold's observations and visibility, per sample by the
+ * rule of mosh2_job_upload_markers_range (arguments as there; job frame (offset of sequence seq0 + k) + t is file frame
+ * frame_start + t * frame_step).  hide [n_folds * M] 0/1: the markers fold k deletes (at least one per fold); their samples are
+ * missing for the fold in every frame and go to a side buffer instead, for mosh2_job_heldout_errors.  Async on the job's
+ * stream; the caller's buffers may be freed when the call returns. */
+int mosh2_job_upload_markers_folds(mosh2_job *j, int32_t seq0, int32_t n_folds, const double *markers, int32_t n_file_frames,
+                                   int32_t n_cols, const int32_t *col_of_marker, const uint8_t *hide, int32_t frame_start,
+                                   int32_t frame_step, double unit_per_metre, const double *rot3x3);
+/* Held-out errors of the last fold upload, computed on the device from the job's current rows (call after the launch and any
+ * repairs or sequence sweeps): err [n_folds][n][K] float64, K = the most markers one fold hides, entry (k, t, r) = |simulated -
+ * observed| in metres of the r-th marker (in marker order) fold k hides, in frame t of the capture; NaN where the fold did not
+ * process t (MOSH2_ST_SOLVED unset), where the capture lacks the sample, or past the fold's count.  status [n_folds][n] (may
+ * be NULL): the status bits of the fold frames.  Only these arrays cross to the host.  MOSH2_E_INVALID without a fold upload
+ * or before the job's first mosh2_job_launch.  Synchronous. */
+int mosh2_job_heldout_errors(mosh2_job *j, double *err, int32_t *status);
 /* ---- Stage I building block (chmosh.py:83-455; SURVEY.md 8(f-2)) ------------------------------------------------------------
  * Linearise mode: the frames of the job are INDEPENDENT problems (the twelve frames of Stage I), each evaluated by one
  * thread block at a state the caller gives -- x [F][3 + p_red + n_dmpl] = trans | reduced pose | linear coefficients.  The

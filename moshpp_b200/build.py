@@ -18,6 +18,7 @@ EMU_SRC = os.path.join(ROOT, 'tests', 'emu', 'mosh2_emu.cpp')
 EMU_ADAPTER_SRC = os.path.join(ROOT, 'tests', 'emu', 'mosh2_emu_adapter.cpp')
 EMU_MULTI_SRC = os.path.join(ROOT, 'tests', 'emu', 'mosh2_emu_multi.cpp')    # includes EMU_SRC: one translation unit
 EMU_SEQUENCE_SRC = os.path.join(ROOT, 'tests', 'emu', 'mosh2_emu_sequence.cpp')
+EMU_HELDOUT_SRC = os.path.join(ROOT, 'tests', 'emu', 'mosh2_emu_heldout.cpp')
 EMU_LIB = os.path.join(ROOT, 'tests', 'emu', '_build', 'libmosh2_emu.so')
 TC_SRC = os.path.join(ROOT, 'tests', 'tc', 'jtj_tf32_test.cu')
 TC_BIN = os.path.join(ROOT, 'tests', 'tc', '_build', 'jtj_test')
@@ -62,12 +63,13 @@ def build_library(force: bool = False, verbose: bool = False, profile: bool = Fa
 def build_emu(force: bool = False) -> str:
     """TEST-ONLY single-thread host build of the CTA program (see tests/emu/mosh2_emu.cpp)."""
     srcs = [EMU_SRC, os.path.join(CSRC, "mosh2_device.cuh"), os.path.join(CSRC, "mosh2_host.h"), os.path.join(ROOT, 'include', 'mosh2.h'),
-            os.path.join(ROOT, 'tests', 'tc', 'gauss_newton_case.h'), EMU_ADAPTER_SRC, EMU_MULTI_SRC, EMU_SEQUENCE_SRC]
+            os.path.join(ROOT, 'tests', 'tc', 'gauss_newton_case.h'), EMU_ADAPTER_SRC, EMU_MULTI_SRC, EMU_SEQUENCE_SRC, EMU_HELDOUT_SRC]
     if force or _stale(EMU_LIB, srcs):
         os.makedirs(os.path.dirname(EMU_LIB), exist_ok=True)
         # (the multi-model job's host build compiles the host build proper inside its own unit; the input adapter's host build)
-        # (the sequence sweep's host build)
-        units = [EMU_MULTI_SRC if os.path.exists(EMU_MULTI_SRC) else EMU_SRC] + [u for u in (EMU_ADAPTER_SRC, EMU_SEQUENCE_SRC) if os.path.exists(u)]
+        # (the sequence sweep's host build; the held-out folds' host build)
+        units = [EMU_MULTI_SRC if os.path.exists(EMU_MULTI_SRC) else EMU_SRC] + [u for u in (EMU_ADAPTER_SRC, EMU_SEQUENCE_SRC, EMU_HELDOUT_SRC)
+                                                                                 if os.path.exists(u)]
         cmd = ['g++', '-O2', '-std=c++17', '-shared', '-fPIC', '-o', EMU_LIB] + units
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

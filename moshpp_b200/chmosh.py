@@ -548,6 +548,93 @@ def check_sequence_sweeps(sequence_sweeps) -> Optional[int]:
     return int(sequence_sweeps)
 
 
+def check_heldout(heldout, latent_labels):
+    """The ``heldout`` keyword of ``mosh_stageii``: None (off), 'each' (leave one out: one fold per latent marker the capture
+    observes) or a list of folds, each a non-empty list of latent labels.  Returns None, 'each' or the folds as lists of latent
+    marker indices in marker order; anything else raises ``ValueError``."""
+    if heldout is None or (isinstance(heldout, str) and heldout == 'each'):
+        return heldout
+    if isinstance(heldout, (str, bytes)) or not isinstance(heldout, (list, tuple)) or not len(heldout):
+        raise ValueError(f"heldout must be None, 'each' or a non-empty list of label lists, not {heldout!r}")
+    index = {l: i for i, l in enumerate(latent_labels)}
+    folds = []
+    for fold in heldout:
+        if isinstance(fold, (str, bytes)) or not isinstance(fold, (list, tuple)) or not len(fold):
+            raise ValueError(f'every heldout fold must be a non-empty list of latent labels, not {fold!r}')
+        unknown = [l for l in fold if not isinstance(l, str) or l not in index]
+        if unknown:
+            raise ValueError(f'heldout fold {fold!r}: unknown labels {unknown!r}')
+        folds.append(sorted({index[l] for l in fold}))
+    return folds
+
+
+def _error_stats(e: np.ndarray) -> dict:
+    """mean / median / p95 / max (metres) and count of the defined (finite) errors in ``e``; NaN statistics when there are none."""
+    e = np.asarray(e, dtype=np.float64).ravel()
+    e = e[np.isfinite(e)]
+    if not len(e):
+        return dict(mean=np.nan, median=np.nan, p95=np.nan, max=np.nan, n=0)
+    return dict(mean=float(e.mean()), median=float(np.median(e)), p95=float(np.percentile(e, 95)), max=float(e.max()), n=int(len(e)))
+
+
+def heldout_validation(cap: dict, sub: dict, data: dict, heldout, mode: str, schedule_kw: dict, sequence_sweeps: Optional[int],
+                       t0: float, fold_rows: bool = False) -> dict:
+    """Held-out marker validation of a Stage-II result (DESIGN.md section 12).  ``cap`` / ``sub``: the capture and subject of the
+    main solve, ``data``: its output dictionary, ``heldout``: ``check_heldout``.  Every fold is the capture with its markers
+    deleted in every frame, solved with the main solve's options in one verified batch launch (``_solve_launch`` with
+    ``folds``; the schedule from ``schedule_kw`` over the fold frame counts).  A fold none of whose markers the capture observes
+    is skipped and listed in ``skipped_folds`` (with 'each': every latent marker the capture never observes).  Returns the ``b200['heldout']`` record: folds, skipped_folds, labels / fold_of_row / err [held-out marker, row
+    of the main result] (metres, NaN where undefined), per-label and overall error statistics (``_error_stats``), the same of
+    the main solve's residual on the visible markers, per-fold status counts and the figures of the fold launch."""
+    labels = cap['labels']
+    M, F = len(labels), cap['F']
+    observed = cap['vis'].any(0)
+    folds = [[i] for i in range(M)] if heldout == 'each' else heldout
+    run = [f for f in folds if observed[f].any()]
+    skipped = [[labels[i] for i in f] for f in folds if not observed[f].any()]
+    fid = np.asarray(data['stageii_debug_details']['b200']['frame_ids'])
+    rec = {'folds': [[labels[i] for i in f] for f in run], 'skipped_folds': skipped}
+    rows, row_labels, fold_of_row, status = [], [], [], []
+    if run:
+        hide = np.zeros((len(run), M), dtype=bool)
+        for k, f in enumerate(run):
+            hide[k, f] = True
+        fsub = dict(sub, seqs=[cap] * len(run), model=sub['model'] if sub['cache'] else None)
+        sched = _resolve_schedule(sub['pk'], mode, [F] * len(run), **schedule_kw)
+        out, figures = _solve_launch([fsub], sched, t0, sequence_sweeps=sequence_sweeps, folds=hide, fold_rows=fold_rows)
+        main = np.zeros(F, dtype=bool)
+        main[fid] = True
+        for k, f in enumerate(run):
+            for r, i in enumerate(f):
+                rows.append(out['err'][k, fid, r])
+                row_labels.append(labels[i])
+                fold_of_row.append(k)
+            st = out['status'][k]
+            solved = (st & _lib.ST_SOLVED) != 0
+            status.append(dict(solved=int(solved.sum()), skipped=int((main & ~solved).sum()),
+                               gn_fallback=int(((st & _lib.ST_GN_FALLBACK) != 0).sum()), maxiter=int(((st & _lib.ST_MAXITER) != 0).sum()),
+                               short_warmup=int(((st & _lib.ST_SHORT_WARMUP) != 0).sum())))
+        rec.update(kernel_ms=figures['kernel_ms'], chunks=figures['chunks'], repair_rounds=figures['boundary_check']['rounds'],
+                   chunk_len=figures['chunk_len'], precision=figures['precision'], device_errors=out['device_errors'])
+        if 'sequence_solve' in out:
+            rec['sequence_solve'] = out['sequence_solve']
+        if fold_rows:
+            rec['rows'] = out['rows']
+    err = np.array(rows, dtype=np.float64).reshape(len(rows), len(fid))
+    rec.update(labels=row_labels, fold_of_row=np.array(fold_of_row, dtype=np.int64), err=err, fold_status=status,
+               overall=_error_stats(err), per_label={l: _error_stats(err[[q for q, x in enumerate(row_labels) if x == l]])
+                                                     for l in dict.fromkeys(row_labels)})
+    # the main solve's own residual on its visible markers, frame-major in marker order as the per-frame lists hold them
+    dbg = data['stageii_debug_details']
+    vis_rows = cap['vis'][fid]
+    res_vis = np.linalg.norm(np.concatenate(dbg['markers_sim']) - np.concatenate(dbg['markers_obs']), axis=1) if len(fid) else np.zeros(0)
+    lab_vis = np.nonzero(vis_rows)[1]
+    rec['visible'] = dict(overall=_error_stats(res_vis),
+                          per_label={labels[i]: _error_stats(res_vis[lab_vis == i]) for i in range(M) if observed[i]})
+    rec['wall_s'] = time.time() - t0
+    return rec
+
+
 def sequence_temporal_sse(pose: np.ndarray, dmpls: Optional[np.ndarray], wt_velo: float, wt_extrap: float, n_dm: int):
     """The temporal residuals of the reference as it assigns them to the processed frames k = 0 .. F'-1 of one capture (rows in
     processed order): velo_k = |wt_velo (p_k - 2 p_{k-1} + p_{k-2})|^2 for k >= 2 over the whole reduced pose, and with ``n_dm``
@@ -572,6 +659,22 @@ def sequence_objective(errs: np.ndarray, pose: np.ndarray, dmpls: Optional[np.nd
     return float(errs[:, [0, 1, 3, 4, 6, 7]].sum() + velo.sum() + extrap.sum())
 
 
+def sweep_until(job, max_sweeps: int, tol):
+    """Up to ``max_sweeps`` sequence sweeps of the job's rows (mosh2_job_sequence_sweep), stopping after the first that moves no
+    processed frame by more than ``tol`` (per group, as ``BOUNDARY_TOL``).  Returns (sweeps, converged, last max_delta, device
+    ms of every sweep)."""
+    tol = np.asarray(tol, dtype=np.float64)
+    sweeps, converged, md, ms = 0, False, np.zeros(4), []
+    while sweeps < max_sweeps:
+        md = job.sequence_sweep()
+        ms.append(job.kernel_ms())
+        sweeps += 1
+        if (md <= tol).all():
+            converged = True
+            break
+    return sweeps, converged, md, ms
+
+
 def sequence_solve(job, res, seq_ranges, opts, n_dm: int, max_sweeps: int, tol):
     """Minimise the sequence objective S jointly, from the causal rows the job holds, by up to ``max_sweeps`` three-colour
     sweeps (mosh2_job_sequence_sweep); stop once a sweep moves no processed frame by more than ``tol`` (per group, as
@@ -594,15 +697,7 @@ def sequence_solve(job, res, seq_ranges, opts, n_dm: int, max_sweeps: int, tol):
 
     s_causal = objectives(res)
     short = res.status & _lib.ST_SHORT_WARMUP
-    tol = np.asarray(tol, dtype=np.float64)
-    sweeps, converged, md, ms = 0, False, np.zeros(4), []
-    while sweeps < max_sweeps:
-        md = job.sequence_sweep()
-        ms.append(job.kernel_ms())
-        sweeps += 1
-        if (md <= tol).all():
-            converged = True
-            break
+    sweeps, converged, md, ms = sweep_until(job, max_sweeps, tol)
     res = job.download()
     res.status |= short
     for a, b in seq_ranges:
@@ -626,7 +721,7 @@ def _subject(seqs, cfg, markers_latent, latent_labels, betas, marker_meta, v_tem
         pk, opts, flags = prepare_stageii(cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname)
         model, cache_hit = None, False
     return dict(seqs=seqs, pk=pk, opts=with_robust_sigma(opts, robust_data_sigma), flags=flags, model=model, cache_hit=cache_hit,
-                device=device, robust_data_sigma=check_robust_sigma(robust_data_sigma))
+                device=device, robust_data_sigma=check_robust_sigma(robust_data_sigma), cache=subject_cache)
 
 
 def _resolve_schedule(pk, mode: str, counts, chunk_len, chunk_warmup, warmup_full, first_extra, precision, verify: bool,
@@ -674,7 +769,61 @@ class _SeqResult:
         self.nd = res.nd
 
 
-def _solve_launch(subs, sched: dict, t0: float, laps: Optional[_Laps] = None, sequence_sweeps: Optional[int] = None):
+def upload_folds(job, cap: dict, hide: np.ndarray):
+    """The held-out folds of the capture ``cap`` (``_read_capture``) into sequences 0 .. n_folds-1 of ``job``: fold k is the
+    capture with the markers ``hide[k]`` missing in every frame.  A device-adapter capture goes up once, raw, and one kernel
+    makes every fold (mosh2_job_upload_markers_folds); a host-adapter capture goes up as copies of its observations with the
+    folds' markers made invisible."""
+    if cap['raw_cols'] is not None:
+        m, rot = cap['mocap'], cap['cfg'].mocap.rotate
+        job.upload_markers_folds(0, hide, m.raw, cap['raw_cols'], cap['sel'].start, cap['sel'].step, m.unit_per_metre,
+                                 None if rot is None else _rotation_xyz(rot))
+    else:
+        vis = cap['vis'][None] & ~hide[:, None, :]
+        obs = np.where(vis[..., None], cap['obs'][None], 0.0)
+        job.upload(obs.reshape(-1, *cap['obs'].shape[1:]), vis.reshape(-1, vis.shape[-1]))
+
+
+def fold_errors(job, bad, cap: dict, hide: np.ndarray, sequence_sweeps: Optional[int], tol, rows: bool = False) -> dict:
+    """After the verified launch of the folds of ``upload_folds``: the sequence sweeps (``sequence_sweeps``, stop rule of
+    ``sweep_until`` at ``tol``), then the held-out errors -- err [n_folds, F, K] in metres of the r-th marker (in marker order)
+    fold k hides, in frame t of the capture, NaN where the fold did not process t or the capture lacks the sample -- and the
+    folds' status [n_folds, F], frames of unverified chunks (``bad``) with MOSH2_ST_SHORT_WARMUP.  A device-adapter capture's
+    errors are formed on the device (mosh2_job_heldout_errors); a host-adapter capture's from the downloaded simulated markers."""
+    n_folds, F = hide.shape[0], cap['F']
+    out = {}
+    if sequence_sweeps is not None:
+        sweeps, converged, md, ms = sweep_until(job, sequence_sweeps, tol)
+        out['sequence_solve'] = dict(sweeps=sweeps, converged=converged, max_delta=md.tolist(), sweep_ms=list(ms))
+    res = None
+    if cap['raw_cols'] is not None:
+        err, st = job.heldout_errors()
+    else:
+        res = job.download()
+        st = res.status.reshape(n_folds, F).copy()
+        K = int(hide.sum(1).max())
+        err = np.full((n_folds, F, K), np.nan)
+        sim = res.markers_sim.reshape(n_folds, F, -1, 3)
+        for k in range(n_folds):
+            idx = np.flatnonzero(hide[k])
+            e = np.linalg.norm(sim[k][:, idx] - cap['obs'][:, idx], axis=-1)
+            e[~cap['vis'][:, idx] | ((st[k] & _lib.ST_SOLVED) == 0)[:, None]] = np.nan
+            err[k, :, :len(idx)] = e
+    if rows and res is None:
+        res = job.download()
+    short = np.zeros(job.n_frames, dtype=bool)
+    ranges = job.chunk_ranges()
+    for c in bad:
+        short[ranges[c, 0]:ranges[c, 1]] = True
+    st |= np.where(short.reshape(n_folds, F) & ((st & _lib.ST_SOLVED) != 0), _lib.ST_SHORT_WARMUP, 0).astype(st.dtype)
+    out.update(err=err, status=st, device_errors=cap['raw_cols'] is not None)
+    if rows:
+        out['rows'] = res
+    return out
+
+
+def _solve_launch(subs, sched: dict, t0: float, laps: Optional[_Laps] = None, sequence_sweeps: Optional[int] = None, folds=None,
+                  fold_rows: bool = False):
     """One verified launch of the captures of the subjects ``subs`` (``_subject``), back to back on the job's frame axis in
     the order given: a batch job of the subject's model (mosh2_job_create_batch) for one subject, a multi-model job
     (mosh2_job_create_multi) for several.  ``sched``: ``_resolve_schedule``.  Every capture uploads its own raw marker table
@@ -684,7 +833,11 @@ def _solve_launch(subs, sched: dict, t0: float, laps: Optional[_Laps] = None, se
     frame ids, adapter), and the figures of the launch (device time, chunks, schedule, boundary check, totals).  Sets the
     ``offset`` of every capture record on the frame axis.  ``laps``: the host-time laps of ``mosh_stageii``.
     ``sequence_sweeps``: None, or the sweep cap of ``sequence_solve``, run on the launch's result (tolerance: the mode's
-    ``BOUNDARY_TOL``); its record goes to every capture's ``b200['sequence_solve']``."""
+    ``BOUNDARY_TOL``); its record goes to every capture's ``b200['sequence_solve']``.
+
+    ``folds``: [n_folds, M] bool, the held-out folds of ONE capture (``heldout_validation``): then the subject's sequences are
+    n_folds copies of that capture, fold k with the markers ``folds[k]`` deleted, and the call returns (``fold_errors``, figures)
+    instead of the per-capture dictionaries; ``fold_rows`` also downloads the folds' result arrays (``rows``)."""
     laps = laps or _Laps()
     seqs = [(sub, s) for sub in subs for s in sub['seqs']]
     counts = [s['F'] for _, s in seqs]
@@ -703,8 +856,10 @@ def _solve_launch(subs, sched: dict, t0: float, laps: Optional[_Laps] = None, se
         laps('job_create_ms')
         try:
             offsets = job.seq_offsets
-            host = [q for q, (_, s) in enumerate(seqs) if s['raw_cols'] is None]
-            if len(seqs) == 1 and host:             # one host-adapter capture fills the frame axis
+            host = [q for q, (_, s) in enumerate(seqs) if s['raw_cols'] is None and folds is None]
+            if folds is not None:
+                upload_folds(job, seqs[0][1], folds)
+            elif len(seqs) == 1 and host:             # one host-adapter capture fills the frame axis
                 job.upload(seqs[0][1]['obs'], seqs[0][1]['vis'])
             elif host:
                 # host-adapter captures: one upload of the whole frame axis; the device-adapter ranges are written over it
@@ -714,7 +869,7 @@ def _solve_launch(subs, sched: dict, t0: float, laps: Optional[_Laps] = None, se
                     obs[offsets[q]:offsets[q + 1]], vis[offsets[q]:offsets[q + 1]] = seqs[q][1]['obs'], seqs[q][1]['vis']
                 job.upload(obs, vis)
             for q, (_, s) in enumerate(seqs):       # issued back to back: every call stages its own rows
-                if s['raw_cols'] is not None:
+                if s['raw_cols'] is not None and folds is None:
                     m, rot = s['mocap'], s['cfg'].mocap.rotate
                     job.upload_markers_range(int(offsets[q]), s['F'], m.raw, s['raw_cols'], s['sel'].start, s['sel'].step,
                                              m.unit_per_metre, None if rot is None else _rotation_xyz(rot))
@@ -729,13 +884,16 @@ def _solve_launch(subs, sched: dict, t0: float, laps: Optional[_Laps] = None, se
                     s['markers_orig'] = s['mocap'].markers[s['sel']]
                 side['ms'] = (time.perf_counter() - t_side) * 1e3
 
-            bad, report = launch_verified(job, sched['tol'], while_running=host_side)
-            res = download_verified(job, bad, report)
-            seq_records = None
-            if sequence_sweeps is not None:
-                n_dm = subs[0]['pk'].n_dmpl - subs[0]['pk'].n_expr if subs[0]['opts'].optimize_dynamics else 0
-                res, seq_records = sequence_solve(job, res, list(zip(offsets[:-1], offsets[1:])), subs[0]['opts'], n_dm,
-                                                  sequence_sweeps, BOUNDARY_TOL[sched['mode']])
+            bad, report = launch_verified(job, sched['tol'], while_running=host_side if folds is None else None)
+            if folds is not None:
+                fold_out = fold_errors(job, bad, seqs[0][1], folds, sequence_sweeps, BOUNDARY_TOL[sched['mode']], fold_rows)
+            else:
+                res = download_verified(job, bad, report)
+                seq_records = None
+                if sequence_sweeps is not None:
+                    n_dm = subs[0]['pk'].n_dmpl - subs[0]['pk'].n_expr if subs[0]['opts'].optimize_dynamics else 0
+                    res, seq_records = sequence_solve(job, res, list(zip(offsets[:-1], offsets[1:])), subs[0]['opts'], n_dm,
+                                                      sequence_sweeps, BOUNDARY_TOL[sched['mode']])
             laps('solve_ms')
             laps.ms['overlapped_host_ms'] = side['ms']
             n_chunks, totals = job.num_chunks, job.totals()
@@ -746,6 +904,14 @@ def _solve_launch(subs, sched: dict, t0: float, laps: Optional[_Laps] = None, se
             sub['model'].close()
     laps('close_ms')
 
+    def launch_figures():
+        figures = {'kernel_ms': float(sum(report['kernel_ms'])), 'wall_s': time.time() - t0, 'chunks': n_chunks}
+        figures.update({k: sched[k] for k in ('chunk_len', 'chunk_warmup', 'warmup_full', 'first_extra', 'precision', 'mode')})
+        figures.update(boundary_check=report, totals=totals)
+        return figures
+
+    if folds is not None:
+        return fold_out, launch_figures()
     outs = []
     for q, (sub, s) in enumerate(seqs):
         s['offset'] = int(offsets[q])
@@ -772,10 +938,7 @@ def _solve_launch(subs, sched: dict, t0: float, laps: Optional[_Laps] = None, se
     n_fb = int(((res.status & _lib.ST_GN_FALLBACK) != 0).sum())
     if n_fb:
         logger.warning('%d frames hit a non-positive-definite Gauss-Newton system (Cauchy step used)', n_fb)
-    figures = {'kernel_ms': float(sum(report['kernel_ms'])), 'wall_s': time.time() - t0, 'chunks': n_chunks}
-    figures.update({k: sched[k] for k in ('chunk_len', 'chunk_warmup', 'warmup_full', 'first_extra', 'precision', 'mode')})
-    figures.update(boundary_check=report, totals=totals)
-    return outs, figures
+    return outs, launch_figures()
 
 
 def mosh_stageii(mocap_fname: str, cfg, markers_latent: np.ndarray, latent_labels: list, betas: np.ndarray,
@@ -784,7 +947,7 @@ def mosh_stageii(mocap_fname: str, cfg, markers_latent: np.ndarray, latent_label
                  first_extra: Optional[int] = None, precision: Optional[str] = None, verify: bool = True, boundary_tol=None,
                  sm_budget: int = NUM_SMS, labels_map='general', subject_cache: bool = True,
                  device_adapter: bool = True, robust_data_sigma: Optional[float] = None,
-                 sequence_sweeps: Optional[int] = None) -> dict:
+                 sequence_sweeps: Optional[int] = None, heldout=None) -> dict:
     """Stage II of MoSh++ on one H100.  Positional arguments as in the reference (chmosh.py:458-459).
 
     Keyword-only extras.  ``mode``: 'fast' (default) = float32, chunked in time with a verified warm-up -- within
@@ -809,12 +972,18 @@ def mosh_stageii(mocap_fname: str, cfg, markers_latent: np.ndarray, latent_label
     ``trans``, ``dmpls``, ``expression`` and ``markers_sim`` then come from the joint solution, ``stageii_errs['velo']`` /
     ``['extrap_dmpl']`` report its temporal residuals as the reference assigns them to frames, and
     ``b200['sequence_solve']`` holds sweeps, converged, objective_causal, objective, max_delta (absent without it).
+    ``heldout``: None (default) = off; 'each' = leave one out, one fold per latent marker the capture observes; a list of label
+    lists = one fold per list.  Every fold is the capture with the fold's markers deleted in every frame, solved with the same
+    Stage-I inputs, mode, schedule keywords, ``robust_data_sigma`` and ``sequence_sweeps`` in one further launch; the error of
+    a held-out marker is its distance from where the camera saw it (DESIGN.md section 12, ``heldout_validation``).  The
+    returned dictionary is the one without the option, plus ``b200['heldout']``.
     """
     t0 = time.time()
     laps = _Laps()
     _check_mode(mode)
     check_robust_sigma(robust_data_sigma)
     check_sequence_sweeps(sequence_sweeps)
+    heldout = check_heldout(heldout, latent_labels)
     cap = _read_capture(mocap_fname, cfg, latent_labels, labels_map, device_adapter)
     laps('read_mocap_ms')
     sub = _subject([cap], cfg, markers_latent, latent_labels, betas, marker_meta, v_template_fname, device, subject_cache,
@@ -829,6 +998,11 @@ def mosh_stageii(mocap_fname: str, cfg, markers_latent: np.ndarray, latent_label
     else:
         h2d = cap['obs'].size * (4 if sched['precision'] == 'f32' else 8) + cap['vis'].size
     data['stageii_debug_details']['b200'].update(figures, host_ms=laps.ms, subject_cache_hit=sub['cache_hit'], h2d_bytes=int(h2d))
+    if heldout is not None:
+        data['stageii_debug_details']['b200']['heldout'] = heldout_validation(
+            cap, sub, data, heldout, mode, dict(chunk_len=chunk_len, chunk_warmup=chunk_warmup, warmup_full=warmup_full,
+                                                first_extra=first_extra, precision=precision, verify=verify, boundary_tol=boundary_tol,
+                                                sm_budget=sm_budget), check_sequence_sweeps(sequence_sweeps), time.time())
     return data
 
 

@@ -251,6 +251,49 @@ __global__ void gather_markers_kernel(const double *__restrict__ raw, int n_cols
     vis[i] = ok ? 1 : 0;
 }
 
+// Held-out folds (mosh2_job_upload_markers_folds): one thread per (fold, frame, marker) over the capture's raw table, staged once;
+// per sample mosh2::fold_marker_sample.  `obs` / `vis` point at the first frame of fold 0, fold k starts k * n_frames frames later;
+// side [n_folds][n_frames][K][3] (metres, float64) takes the samples of the markers a fold hides (slot [n_folds][M]: their rank).
+template <class real>
+__global__ void gather_folds_kernel(const double *__restrict__ raw, int n_cols, const int *__restrict__ col_of_marker, int M,
+                                    int n_frames, int n_folds, int frame_step, double unit_per_metre, const double *__restrict__ rot,
+                                    const int *__restrict__ slot, int K, real *__restrict__ obs, uint8_t *__restrict__ vis,
+                                    double *__restrict__ side) {
+    const size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i >= size_t(n_folds) * n_frames * M) return;
+    const int mk = int(i % M);
+    const size_t ft = i / M;                     // fold * n_frames + frame
+    const int t = int(ft % n_frames), k = int(ft / n_frames), col = col_of_marker[mk], r = slot[size_t(k) * M + mk];
+    double o[3], sd[3];
+    const bool ok = mosh2::fold_marker_sample(col >= 0 ? raw + (size_t(t) * frame_step * n_cols + col) * 3 : nullptr, unit_per_metre,
+                                              rot, r >= 0, o, sd);
+    obs[3 * i] = real(o[0]); obs[3 * i + 1] = real(o[1]); obs[3 * i + 2] = real(o[2]);
+    vis[i] = ok ? 1 : 0;
+    if (r >= 0) {
+        double *p = side + (ft * K + r) * 3;
+        p[0] = sd[0]; p[1] = sd[1]; p[2] = sd[2];
+    }
+}
+
+// Held-out errors (mosh2_job_heldout_errors): one thread per (fold, frame, hidden marker), per sample mosh2::heldout_error from
+// the fold's simulated marker and the side buffer; the thread of the first hidden marker also copies the frame's status.
+template <class real>
+__global__ void heldout_error_kernel(const real *__restrict__ markers_sim, const int *__restrict__ status, const double *__restrict__ side,
+                                     const int *__restrict__ idx, int M, int n_frames, int n_folds, int K, int frame0,
+                                     double *__restrict__ err, int *__restrict__ fold_status) {
+    const size_t i = size_t(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i >= size_t(n_folds) * n_frames * K) return;
+    const int r = int(i % K);
+    const size_t ft = i / K;
+    const int k = int(ft / n_frames), mk = idx[size_t(k) * K + r];
+    const size_t f = size_t(frame0) + ft;
+    if (r == 0) fold_status[ft] = status[f];
+    if (mk < 0) { err[i] = NAN; return; }
+    const real *s = markers_sim + (f * M + mk) * 3;
+    const double sim[3] = {double(s[0]), double(s[1]), double(s[2])};
+    err[i] = mosh2::heldout_error(sim, side + 3 * i, (status[f] & mosh2::ST_SOLVED) != 0);
+}
+
 // Host copy of a model description: the caller's buffers need not outlive mosh2_model_create, and the device copy of a
 // precision is only built when the first job of that precision is created.
 struct HostDesc {
@@ -337,6 +380,12 @@ struct mosh2_job {
     // slot is only refilled once its event has completed, so uploads of several captures can be queued back to back.
     struct RangeSlot { void *h = nullptr, *d = nullptr; size_t bytes = 0; cudaEvent_t done = nullptr; };
     std::vector<RangeSlot> range_slots;
+    std::vector<int> counts;                     // frames of every sequence of the job
+    // the last mosh2_job_upload_markers_folds: its folds (first frame, frames per fold, count, most hidden markers K), the side
+    // buffer [n_folds][n][K][3] (float64), the hidden markers [n_folds][K], and the errors and status of mosh2_job_heldout_errors
+    int fold_frame0 = 0, fold_n = 0, fold_count = 0, fold_K = 0;
+    double *d_fold_side = nullptr, *d_fold_err = nullptr;
+    int *d_fold_idx = nullptr, *d_fold_status = nullptr;
     int *h_status = nullptr, *h_counters = nullptr;
     // multi-model job (mosh2_job_create_multi; `model` is models[0]): the Model records of the job's precision as the kernel
     // reads them (host copy, whose first record also carries the job's workspace plan, and device array), and the model
@@ -462,6 +511,34 @@ int linearize(mosh2_job *j, const mosh2::Model<real> &m, int32_t step, int32_t b
     CU(cudaStreamSynchronize(j->stream));
     for (const Back &e : b)
         if (e.dst) for (size_t i = 0; i < e.cnt; ++i) e.dst[i] = double(e.h[i]);
+    return 0;
+}
+
+// A staging slot of at least `total` bytes (pinned host memory and its device twin) whose last copy and kernel have finished.
+int staging_slot(mosh2_job *j, size_t total, mosh2_job::RangeSlot **out) {
+    const int dv = j->model->device;
+    mosh2_job::RangeSlot *slot = nullptr, *idle = nullptr;
+    for (auto &s : j->range_slots) {
+        const cudaError_t q = cudaEventQuery(s.done);
+        if (q == cudaErrorNotReady) continue;
+        CU(q);
+        if (s.bytes >= total) { slot = &s; break; }
+        if (!idle) idle = &s;
+    }
+    if (!slot) {
+        if (!idle) {
+            j->range_slots.emplace_back();
+            idle = &j->range_slots.back();
+            CU(cudaEventCreateWithFlags(&idle->done, cudaEventDisableTiming));
+        }
+        slot = idle;
+        g_blocks.put(-1, slot->h); g_blocks.put(dv, slot->d);
+        slot->h = slot->d = nullptr; slot->bytes = 0;
+        CU(g_blocks.get(-1, total, &slot->h));
+        CU(g_blocks.get(dv, total, &slot->d));
+        slot->bytes = total;
+    }
+    *out = slot;
     return 0;
 }
 
@@ -601,6 +678,7 @@ int mosh2_job_create_batch(mosh2_model *m, const mosh2_options *opt, int32_t n_s
     mosh2_job *j = new (std::nothrow) mosh2_job;
     if (!j) return fail(MOSH2_E_INVALID, "out of host memory");
     j->model = m; j->precision = precision; j->n_frames = n_frames;
+    j->counts.assign(frame_counts, frame_counts + n_seq);
     j->tab = mosh2_host::schedule_table(sched, frame_counts, n_seq);
     j->tab0 = j->tab;
     const std::vector<int> &tab = j->tab;
@@ -780,31 +858,11 @@ int mosh2_job_upload_markers_range(mosh2_job *j, int32_t frame0, int32_t nfr, co
                                                       frame_step, unit_per_metre, &msg))
         return fail(rc, "%s", msg.c_str());
     CU(cudaSetDevice(j->model->device));
-    const int dv = j->model->device;
     // slot layout: rows [frame_start, last used frame] of the table (all columns) | rotation (9) | column map (M int32)
     const size_t rows = size_t(nfr - 1) * frame_step + 1, bytes = rows * n_cols * 3 * sizeof(double);
     const size_t o_cols = bytes + 9 * sizeof(double), total = o_cols + size_t(M) * sizeof(int32_t);
-    mosh2_job::RangeSlot *slot = nullptr, *idle = nullptr;
-    for (auto &s : j->range_slots) {
-        const cudaError_t q = cudaEventQuery(s.done);
-        if (q == cudaErrorNotReady) continue;
-        CU(q);
-        if (s.bytes >= total) { slot = &s; break; }
-        if (!idle) idle = &s;
-    }
-    if (!slot) {
-        if (!idle) {
-            j->range_slots.emplace_back();
-            idle = &j->range_slots.back();
-            CU(cudaEventCreateWithFlags(&idle->done, cudaEventDisableTiming));
-        }
-        slot = idle;
-        g_blocks.put(-1, slot->h); g_blocks.put(dv, slot->d);
-        slot->h = slot->d = nullptr; slot->bytes = 0;
-        CU(g_blocks.get(-1, total, &slot->h));
-        CU(g_blocks.get(dv, total, &slot->d));
-        slot->bytes = total;
-    }
+    mosh2_job::RangeSlot *slot = nullptr;
+    if (const int rc = staging_slot(j, total, &slot)) return rc;
     char *h = static_cast<char *>(slot->h);
     memcpy(h, markers + size_t(frame_start) * n_cols * 3, bytes);
     if (rot3x3) memcpy(h + bytes, rot3x3, 9 * sizeof(double));
@@ -823,6 +881,88 @@ int mosh2_job_upload_markers_range(mosh2_job *j, int32_t frame0, int32_t nfr, co
                                                                     static_cast<float *>(j->d_obs) + 3 * o0, j->d_vis + o0);
     CU(cudaGetLastError());
     CU(cudaEventRecord(slot->done, j->stream));
+    return 0;
+}
+
+int mosh2_job_upload_markers_folds(mosh2_job *j, int32_t seq0, int32_t n_folds, const double *markers, int32_t n_file_frames,
+                                   int32_t n_cols, const int32_t *col_of_marker, const uint8_t *hide, int32_t frame_start,
+                                   int32_t frame_step, double unit_per_metre, const double *rot3x3) {
+    if (!j) return fail(MOSH2_E_INVALID, "null argument");
+    const int M = j->model->n_markers;
+    std::string msg;
+    if (const int rc = mosh2_host::check_marker_folds(j->counts, M, seq0, n_folds, hide, markers, n_file_frames, n_cols, col_of_marker,
+                                                      frame_start, frame_step, unit_per_metre, &msg))
+        return fail(rc, "%s", msg.c_str());
+    CU(cudaSetDevice(j->model->device));
+    const int dv = j->model->device, n = j->counts[seq0];
+    int frame0 = 0;
+    for (int q = 0; q < seq0; ++q) frame0 += j->counts[q];
+    std::vector<int> slot_of, idx;
+    const int K = mosh2_host::fold_slots(hide, n_folds, M, slot_of, idx);
+    // the fold buffers are replaced once the stream has finished with the previous ones
+    CU(cudaStreamSynchronize(j->stream));
+    for (void *p : {static_cast<void *>(j->d_fold_side), static_cast<void *>(j->d_fold_err), static_cast<void *>(j->d_fold_idx),
+                    static_cast<void *>(j->d_fold_status)})
+        g_blocks.put(dv, p);
+    j->d_fold_side = j->d_fold_err = nullptr; j->d_fold_idx = j->d_fold_status = nullptr; j->fold_count = 0;
+    const size_t nfk = size_t(n_folds) * n * K;
+    CU(g_blocks.get(dv, nfk * 3 * sizeof(double), reinterpret_cast<void **>(&j->d_fold_side)));
+    CU(g_blocks.get(dv, nfk * sizeof(double), reinterpret_cast<void **>(&j->d_fold_err)));
+    CU(g_blocks.get(dv, idx.size() * sizeof(int), reinterpret_cast<void **>(&j->d_fold_idx)));
+    CU(g_blocks.get(dv, size_t(n_folds) * n * sizeof(int), reinterpret_cast<void **>(&j->d_fold_status)));
+    // slot layout: rows [frame_start, last used frame] of the table (all columns) | rotation (9) | column map (M) | hide ranks
+    // [n_folds][M] | hidden markers [n_folds][K]
+    const size_t rows = size_t(n - 1) * frame_step + 1, bytes = rows * n_cols * 3 * sizeof(double);
+    const size_t o_cols = bytes + 9 * sizeof(double), o_slot = o_cols + size_t(M) * sizeof(int32_t);
+    const size_t o_idx = o_slot + slot_of.size() * sizeof(int32_t), total = o_idx + idx.size() * sizeof(int32_t);
+    mosh2_job::RangeSlot *slot = nullptr;
+    if (const int rc = staging_slot(j, total, &slot)) return rc;
+    char *h = static_cast<char *>(slot->h);
+    memcpy(h, markers + size_t(frame_start) * n_cols * 3, bytes);
+    if (rot3x3) memcpy(h + bytes, rot3x3, 9 * sizeof(double));
+    memcpy(h + o_cols, col_of_marker, size_t(M) * sizeof(int32_t));
+    memcpy(h + o_slot, slot_of.data(), slot_of.size() * sizeof(int32_t));
+    memcpy(h + o_idx, idx.data(), idx.size() * sizeof(int32_t));
+    CU(cudaMemcpyAsync(slot->d, h, total, cudaMemcpyHostToDevice, j->stream));
+    CU(cudaMemcpyAsync(j->d_fold_idx, static_cast<char *>(slot->d) + o_idx, idx.size() * sizeof(int32_t), cudaMemcpyDeviceToDevice, j->stream));
+    const char *d = static_cast<const char *>(slot->d);
+    const double *d_table = reinterpret_cast<const double *>(d), *d_rot = rot3x3 ? reinterpret_cast<const double *>(d + bytes) : nullptr;
+    const int *d_cols = reinterpret_cast<const int *>(d + o_cols), *d_slot = reinterpret_cast<const int *>(d + o_slot);
+    const size_t cnt = size_t(n_folds) * n * M, o0 = size_t(frame0) * M;
+    const int blocks = int((cnt + 255) / 256);
+    if (j->precision == MOSH2_F64)
+        gather_folds_kernel<double><<<blocks, 256, 0, j->stream>>>(d_table, n_cols, d_cols, M, n, n_folds, frame_step, unit_per_metre, d_rot,
+                                                                   d_slot, K, static_cast<double *>(j->d_obs) + 3 * o0, j->d_vis + o0,
+                                                                   j->d_fold_side);
+    else
+        gather_folds_kernel<float><<<blocks, 256, 0, j->stream>>>(d_table, n_cols, d_cols, M, n, n_folds, frame_step, unit_per_metre, d_rot,
+                                                                  d_slot, K, static_cast<float *>(j->d_obs) + 3 * o0, j->d_vis + o0,
+                                                                  j->d_fold_side);
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(slot->done, j->stream));
+    j->fold_frame0 = frame0; j->fold_n = n; j->fold_count = n_folds; j->fold_K = K;
+    return 0;
+}
+
+int mosh2_job_heldout_errors(mosh2_job *j, double *err, int32_t *status) {
+    if (!j || !err) return fail(MOSH2_E_INVALID, "null argument");
+    if (!j->fold_count) return fail(MOSH2_E_INVALID, "mosh2_job_heldout_errors needs a fold upload (mosh2_job_upload_markers_folds)");
+    if (!j->launched) return fail(MOSH2_E_INVALID, "mosh2_job_heldout_errors needs a solve of the job first (mosh2_job_launch)");
+    CU(cudaSetDevice(j->model->device));
+    const size_t nfk = size_t(j->fold_count) * j->fold_n * j->fold_K, nf = size_t(j->fold_count) * j->fold_n;
+    const int blocks = int((nfk + 255) / 256), M = j->model->n_markers;
+    if (j->precision == MOSH2_F64)
+        heldout_error_kernel<double><<<blocks, 256, 0, j->stream>>>(static_cast<const double *>(j->d_out) + j->o_mk, j->d_status, j->d_fold_side,
+                                                                    j->d_fold_idx, M, j->fold_n, j->fold_count, j->fold_K, j->fold_frame0,
+                                                                    j->d_fold_err, j->d_fold_status);
+    else
+        heldout_error_kernel<float><<<blocks, 256, 0, j->stream>>>(static_cast<const float *>(j->d_out) + j->o_mk, j->d_status, j->d_fold_side,
+                                                                   j->d_fold_idx, M, j->fold_n, j->fold_count, j->fold_K, j->fold_frame0,
+                                                                   j->d_fold_err, j->d_fold_status);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(err, j->d_fold_err, nfk * sizeof(double), cudaMemcpyDeviceToHost, j->stream));
+    if (status) CU(cudaMemcpyAsync(status, j->d_fold_status, nf * sizeof(int), cudaMemcpyDeviceToHost, j->stream));
+    CU(cudaStreamSynchronize(j->stream));
     return 0;
 }
 
@@ -1064,6 +1204,9 @@ void mosh2_job_destroy(mosh2_job *j) {
     g_blocks.put(dv, j->d_seq_nbr);
     g_blocks.put(dv, j->d_seq_ids);
     g_blocks.put(dv, j->d_seq_delta);
+    for (void *p : {static_cast<void *>(j->d_fold_side), static_cast<void *>(j->d_fold_err), static_cast<void *>(j->d_fold_idx),
+                    static_cast<void *>(j->d_fold_status)})
+        g_blocks.put(dv, p);
     for (void *p : {j->h_obs, j->h_out, static_cast<void *>(j->h_vis), static_cast<void *>(j->h_status), static_cast<void *>(j->h_counters)})
         g_blocks.put(-1, p);
     for (auto &s : j->range_slots) {        // (the stream is idle: every slot's copy and kernel have finished)

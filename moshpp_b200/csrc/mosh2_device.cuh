@@ -91,6 +91,27 @@ M2_HD bool gather_marker_sample(const double *p, double unit_per_metre, const do
     return ok;
 }
 
+// One sample of a held-out fold (mosh2.cu gather_folds_kernel): the sample as gather_marker_sample makes it.  A sample of a
+// marker the fold hides is missing for the fold (zero, invisible) and goes to the fold's side buffer `side` instead, NaN where
+// the capture itself lacks it.  Returns the fold's visibility.
+M2_HD bool fold_marker_sample(const double *p, double unit_per_metre, const double *rot, bool hidden, double obs[3], double side[3]) {
+    double v[3];
+    const bool ok = gather_marker_sample(p, unit_per_metre, rot, v);
+    for (int q = 0; q < 3; ++q) {
+        obs[q] = hidden ? 0.0 : v[q];
+        if (hidden) side[q] = ok ? v[q] : NAN;
+    }
+    return ok && !hidden;
+}
+
+// Held-out error of one sample (mosh2.cu heldout_error_kernel): |sim - side| in metres, for a frame the fold processed; NaN
+// where it did not, or where the capture lacks the sample (side NaN).
+M2_HD double heldout_error(const double sim[3], const double side[3], bool processed) {
+    if (!processed) return NAN;
+    const double dx = sim[0] - side[0], dy = sim[1] - side[1], dz = sim[2] - side[2];
+    return sqrt(fma(dz, dz, fma(dy, dy, dx * dx)));      // (explicit fma: the same rounding in the host build)
+}
+
 template <class T>
 struct SPtr {                            // array in shared memory
     uint32_t ofs;

@@ -404,4 +404,52 @@ inline int check_marker_range(int n_frames, int M, int frame0, int n, const doub
     return 0;
 }
 
+// ---- mosh2_job_upload_markers_folds -----------------------------------------------------------------------------------------------
+// Argument checks of a fold upload into sequences [seq0, seq0 + n_folds) of a job whose sequences have `counts` frames: the folds'
+// sequences exist and have one frame count, every hide mask is 0 / 1 and hides at least one marker, and the capture fits the first
+// fold's range (check_marker_range).  0, or MOSH2_E_INVALID with the reason in *msg.
+inline int check_marker_folds(const std::vector<int> &counts, int M, int seq0, int n_folds, const uint8_t *hide, const double *markers,
+                              int n_file_frames, int n_cols, const int *col_of_marker, int frame_start, int frame_step,
+                              double unit_per_metre, std::string *msg) {
+    if (!hide) return reject(msg, MOSH2_E_INVALID, "null argument");
+    if (seq0 < 0 || n_folds < 1 || size_t(seq0) + size_t(n_folds) > counts.size())
+        return reject(msg, MOSH2_E_INVALID, "folds [%d, %d) outside the job's %d sequences", seq0, seq0 + n_folds, int(counts.size()));
+    for (int k = 1; k < n_folds; ++k)
+        if (counts[seq0 + k] != counts[seq0])
+            return reject(msg, MOSH2_E_INVALID, "fold %d has %d frames, fold 0 %d: every fold is the same capture", k, counts[seq0 + k],
+                          counts[seq0]);
+    for (int k = 0; k < n_folds; ++k) {
+        int n = 0;
+        for (int i = 0; i < M; ++i) {
+            const uint8_t h = hide[size_t(k) * M + i];
+            if (h > 1) return reject(msg, MOSH2_E_INVALID, "hide[%d][%d] = %d (0 or 1)", k, i, int(h));
+            n += h;
+        }
+        if (!n) return reject(msg, MOSH2_E_INVALID, "fold %d hides no marker", k);
+    }
+    int frame0 = 0, total = 0;
+    for (int q = 0; q < seq0; ++q) frame0 += counts[q];
+    for (int c : counts) total += c;
+    return check_marker_range(total, M, frame0, counts[seq0], markers, n_file_frames, n_cols, col_of_marker, frame_start, frame_step,
+                              unit_per_metre, msg);
+}
+
+// Side-buffer layout of a fold upload: slot[k * M + i] = rank of marker i among the markers fold k hides (-1: not hidden);
+// idx[k * K + r] = the r-th marker fold k hides (-1 past its count).  Returns K, the most markers one fold hides.
+inline int fold_slots(const uint8_t *hide, int n_folds, int M, std::vector<int> &slot, std::vector<int> &idx) {
+    int K = 0;
+    slot.assign(size_t(n_folds) * M, -1);
+    for (int k = 0; k < n_folds; ++k) {
+        int r = 0;
+        for (int i = 0; i < M; ++i)
+            if (hide[size_t(k) * M + i]) slot[size_t(k) * M + i] = r++;
+        K = std::max(K, r);
+    }
+    idx.assign(size_t(n_folds) * K, -1);
+    for (int k = 0; k < n_folds; ++k)
+        for (int i = 0; i < M; ++i)
+            if (slot[size_t(k) * M + i] >= 0) idx[size_t(k) * K + slot[size_t(k) * M + i]] = i;
+    return K;
+}
+
 }  // namespace mosh2_host

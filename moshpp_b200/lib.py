@@ -13,7 +13,7 @@ import numpy as np
 
 from .pack import StageIIPack
 
-ABI_VERSION = 109          # MOSH2_VERSION of include/mosh2.h that the ctypes structs below encode
+ABI_VERSION = 110          # MOSH2_VERSION of include/mosh2.h that the ctypes structs below encode
 MOSH2_F32, MOSH2_F64 = 0, 1
 ST_SOLVED, ST_SKIPPED, ST_HAS_VELO, ST_HAS_EXTRAP, ST_GN_FALLBACK, ST_MAXITER, ST_SHORT_WARMUP = 1, 2, 4, 8, 16, 32, 64
 ERR_NAMES = ('data', 'poseB', 'velo', 'poseH', 'dmpl', 'extrap_dmpl', 'poseF', 'expr')   # column order of mosh2_result.errs
@@ -124,6 +124,9 @@ def load_library(path: Optional[str] = None):
     lib.mosh2_job_upload_markers.argtypes = [vp, _f64p, C.c_int32, C.c_int32, _i32p, C.c_int32, C.c_int32, C.c_double, _f64p]
     lib.mosh2_job_upload_markers_range.argtypes = [vp, C.c_int32, C.c_int32, _f64p, C.c_int32, C.c_int32, _i32p, C.c_int32, C.c_int32,
                                                    C.c_double, _f64p]
+    lib.mosh2_job_upload_markers_folds.argtypes = [vp, C.c_int32, C.c_int32, _f64p, C.c_int32, C.c_int32, _i32p, _u8p, C.c_int32,
+                                                   C.c_int32, C.c_double, _f64p]
+    lib.mosh2_job_heldout_errors.argtypes = [vp, _f64p, _i32p]
     lib.mosh2_job_upload_device_range.argtypes = [vp, C.c_int32, C.c_int32, vp, C.c_int32, vp, vp]
     lib.mosh2_job_upload_device.argtypes = [vp, vp, C.c_int32, vp, vp]
     lib.mosh2_job_row_width.argtypes = [vp]
@@ -157,7 +160,7 @@ EXPORTED_SYMBOLS = (
     'mosh2_job_create_batch', 'mosh2_job_upload_device_range', 'mosh2_job_warm_states', 'mosh2_job_relaunch_chunks',
     'mosh2_job_boundary_deltas', 'mosh2_release_cached_memory', 'mosh2_mesh_distance', 'mosh2_job_upload_markers', 'mosh2_job_linearize',
     'mosh2_job_chunk_ranges', 'mosh2_job_upload_markers_range', 'mosh2_job_create_multi',
-    'mosh2_job_sequence_sweep')
+    'mosh2_job_sequence_sweep', 'mosh2_job_upload_markers_folds', 'mosh2_job_heldout_errors')
 
 
 def _ptr(a: np.ndarray, typ):
@@ -357,6 +360,34 @@ class Job:
                                                                   raw.shape[1], _ptr(cols, _i32p), int(frame_start), int(frame_step),
                                                                   float(unit_per_metre), _ptr(rot, _f64p) if rot is not None else None),
                           'mosh2_job_upload_markers_range')
+
+    def upload_markers_folds(self, seq0: int, hide, raw: np.ndarray, col_of_marker, frame_start: int, frame_step: int,
+                             unit_per_metre: float, rot3x3=None):
+        """Held-out folds of one capture (mosh2_job_upload_markers_folds): sequence seq0 + k of the job is the capture with the
+        markers ``hide[k]`` ([n_folds, M] bool) deleted; the other arguments as in ``upload_markers_range``.  The raw table is
+        staged once for all folds."""
+        raw = np.ascontiguousarray(raw, dtype=np.float64)
+        cols = np.ascontiguousarray(col_of_marker, dtype=np.int32)
+        h = np.ascontiguousarray(hide, dtype=np.uint8)
+        assert raw.ndim == 3 and raw.shape[2] == 3 and cols.shape == (self.model.pk.n_markers,)
+        assert h.ndim == 2 and h.shape[1] == self.model.pk.n_markers
+        rot = None if rot3x3 is None else np.ascontiguousarray(rot3x3, dtype=np.float64).reshape(3, 3)
+        self.model._check(self.lib.mosh2_job_upload_markers_folds(self.handle, int(seq0), h.shape[0], _ptr(raw, _f64p), raw.shape[0],
+                                                                  raw.shape[1], _ptr(cols, _i32p), _ptr(h, _u8p), int(frame_start),
+                                                                  int(frame_step), float(unit_per_metre),
+                                                                  _ptr(rot, _f64p) if rot is not None else None),
+                          'mosh2_job_upload_markers_folds')
+        self.folds = (int(seq0), h.shape[0], int(h.sum(1).max()))
+
+    def heldout_errors(self):
+        """(err [n_folds, n, K], status [n_folds, n]) of the last ``upload_markers_folds``, computed on the device from the job's
+        current rows (mosh2_job_heldout_errors): the error in metres of the r-th marker fold k hides in frame t, NaN where undefined."""
+        seq0, n_folds, K = self.folds
+        n = int(self.frame_counts[seq0])
+        err = np.zeros((n_folds, n, K))
+        st = np.zeros((n_folds, n), dtype=np.int32)
+        self.model._check(self.lib.mosh2_job_heldout_errors(self.handle, _ptr(err, _f64p), _ptr(st, _i32p)), 'mosh2_job_heldout_errors')
+        return err, st
 
     def linearize(self, x: np.ndarray, options: Options, step: int, build: bool) -> Dict[str, np.ndarray]:
         """mosh2_job_linearize: every frame of the job evaluated (and, with ``build``, linearised) at its row of ``x``
